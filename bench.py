@@ -1,6 +1,6 @@
 """bench.py — sentences/sec of the bert_bilstm_crf hot path (BASELINE.json metric).
 
-  python bench.py --gpus N --steps K --warmup W            our arm (sm_100a kernels)
+  python bench.py --gpus N --steps K --warmup W            our arm (sm_90a kernels)
   python bench.py --impl reference --gpus N --steps K ...  the reference's CPU path (oracle port)
 
 One "step" = one PREDICT pass of model.bert_bilstm_crf.build_graph over one synthetic
@@ -28,19 +28,21 @@ B_PER_GPU, SEQ_LEN, LABELS = 64, 128, 10
 METRIC = "sentences/sec bert_bilstm_crf MSRA L=128"
 WORKLOAD = ("bert_bilstm_crf msra seq_len=128 bs=64/GPU PREDICT step: BERT-base fwd (12L, H768) + BiLSTM(H128, relu) "
             "+ logits + CRF Viterbi -> pred_ids (the log-likelihood is part of the graph but PREDICT does not fetch it, as "
-            "in the reference's Estimator); bf16 tcgen05 GEMM operands, fp32 residual/LSTM/CRF; MSRA-shaped lengths")
+            "in the reference's Estimator); bf16 wgmma GEMM operands, fp32 residual/LSTM/CRF; MSRA-shaped lengths")
 
 
 def measured_peaks():
+    """HBM GB/s and dense bf16 TFLOP/s the rooflines divide by: MEASURED_PEAKS.json when present, else the H100 SXM data
+    sheet (3.35 TB/s, 989 TFLOP/s at 700 W; a power-limited card reaches less)."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-    return 6650.0, 1400.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops_sustained", 989.0), "measured"
+    return 3350.0, 989.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """SM clock / throttle-reason sampling DURING the timed regions (B200_PROFILING.md recipe).  NVML is polled
+    """SM clock / throttle-reason sampling DURING the timed regions.  NVML is polled
     from a thread every ~2 ms (the timed regions last tens of ms, shorter than one `nvidia-smi -lms` period);
     `nvidia-smi` is the fallback when the NVML binding is unavailable."""
 
@@ -357,7 +359,7 @@ def crf_sample_check(x, tr, lens, tags, ll, pred, n=2048, seed=4321):
 
 def crf_rooflines(hbm_peak, peak_src, B=262144, L=128, K=LABELS):
     """SURVEY 8(d) "CRF kernel roofline run": B = 262 144 sequences, L = 128, K = 10, full lengths (1.34 GB of emission
-    logits >> 126 MB L2, so every launch is L2-cold by construction).  Algorithmic bytes per sentence (SURVEY 8(d)):
+    logits >> 50 MB L2, so every launch is L2-cold by construction).  Algorithmic bytes per sentence (SURVEY 8(d)):
     forward-alpha L*(4K+4)+8, Viterbi read L*4K+4 + write L*4+4 (backpointers stay on chip and are not counted)."""
     from chinesener_b200 import ops
     g = torch.Generator(device="cuda").manual_seed(1234)
@@ -430,7 +432,7 @@ def other_configs(steps, flush):
 
     # config 2: bert_crf msra seq_len=128 bs=32 fp32 (split-bf16 dense + fp32 attention/LayerNorm: the 1e-3 mode)
     B, L = 32, 128
-    out["config2_bert_crf_fp32"] = {"workload": "bert_crf msra seq_len=128 bs=32, bert_precision='fp32' (3 bf16 tcgen05 GEMMs per dense "
+    out["config2_bert_crf_fp32"] = {"workload": "bert_crf msra seq_len=128 bs=32, bert_precision='fp32' (3 bf16 wgmma GEMMs per dense "
                                                 "layer, fp32 attention), MSRA-shaped lengths, PREDICT", "dtype": "f32 (split bf16)"}
     est = engine.Estimator("bert_crf", dict(synthetic.data_params(L, LABELS), pretrain_dir="", bert_precision="fp32"))
     run("config2_bert_crf_fp32", est, synthetic.msra_batch(B, L, seed=21), B)
@@ -466,7 +468,7 @@ def other_configs(steps, flush):
 
 
 class GemmTimer:
-    """Per-launch CUDA-event timing of the dominant kernel (tcgen05 GEMM) on the launching stream."""
+    """Per-launch CUDA-event timing of the dominant kernel (wgmma GEMM) on the launching stream."""
 
     def __init__(self):
         self.recs = []
@@ -486,13 +488,22 @@ class GemmTimer:
         return ms, fl, len(self.recs)
 
 
+def dump_outputs(d, arrays):
+    """Each array as d/<name>.npy in float32 (float64 stays float64).  The timed inputs and weights are seeded, so two builds
+    run with the same arguments can be compared output for output."""
+    os.makedirs(d, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy() if torch.is_tensor(t) else np.asarray(t)
+        np.save(os.path.join(d, name + ".npy"), a.astype(np.float64 if a.dtype == np.float64 else np.float32))
+
+
 def run_ours(args):
     from chinesener_b200 import _lib
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a CUDA device: the sm_100a kernels have no CPU fallback")
+        raise SystemExit("bench.py needs a CUDA device: the sm_90a kernels have no CPU fallback")
     torch.cuda.set_device(local)
     numa = bind_to_gpu_numa_node(local) if world > 1 else None   # N=1 keeps every host CPU for the cpu_baseline leg
     dist = None
@@ -504,7 +515,7 @@ def run_ours(args):
     nb = 4
     batches = host_batches(nb, seed0=1234 + 100 * rank)
     dev_batches = [est.to_device(b) for b in batches]
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device="cuda")  # > 50 MB L2
 
     def step_resident(i):
         return est.predict_device(dev_batches[i % nb])     # the PREDICT path of Estimator.predict*, inputs resident
@@ -528,24 +539,27 @@ def run_ours(args):
     evs = []
     barrier()
     l0 = _lib.LAUNCHES
+    last = None
     for i in range(args.steps):
         flush.zero_()
         s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         s.record()
-        step_resident(i)
+        last = step_resident(i)
         e.record()
         evs.append((s, e))
     barrier()
     launches = _lib.LAUNCHES - l0
     t_res = sum(s.elapsed_time(e) for s, e in evs) / 1e3
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"pred_ids": last})
 
     # ---- the same K steps as a throughput pipeline (sentences are independent, SURVEY 8(e)):
     #      * NS CUDA streams: consecutive calls alternate over streams, so the SMs one call's kernel leaves idle in its
     #        partial last wave run another call's kernels;
-    #      * G batches stacked per call: the packed token count of one 64-sentence MSRA batch (~3.2 k rows) is 0.5 / 1.5 /
-    #        2.0 waves of 128x256 tiles on 148 SMs, two batches are 1.0 / 3.0 / 4.0.
+    #      * G batches stacked per call: the packed token count of one 64-sentence MSRA batch (~3.2 k rows) is 0.6 / 1.7 /
+    #        2.3 waves of 128x256 tiles on 132 SMs, two batches are 1.1 / 3.4 / 4.5.
     #      One event pair around the K steps; no flush kernel (the 170 MB of bf16 weights streamed per call exceed the
-    #      126 MB L2).  Every combination processes the same K batches; the best one is the line's `value`.
+    #      50 MB L2).  Every combination processes the same K batches; the best one is the line's `value`.
     from chinesener_b200 import ops as _ops
     stacked = {1: dev_batches}
 
@@ -605,7 +619,7 @@ def run_ours(args):
     #      tf.estimator.Estimator.predict): every step copies its pinned host batch H2D and its pred_ids D2H inside
     #      the timed region; the next call is enqueued while the previous result is awaited.  One event pair around
     #      the K steps (per-step brackets do not exist in a pipelined loop); no flush kernel here: the 170 MB of
-    #      bf16 weights streamed every call already exceed the 126 MB L2.  Same (streams, batches per call) as `value`.
+    #      bf16 weights streamed every call already exceed the 50 MB L2.  Same (streams, batches per call) as `value`.
     #      The API's own pipeline parameters are chosen the same way as for `value`: the two best resident combinations are
     #      timed end to end and the better one is reported (a deep stack pays a longer fill / drain over only K = 20 steps).
     def time_e2e(ns_, g_):
@@ -729,7 +743,7 @@ def run_ours(args):
         t_res, t_e2e, t_res2 = float(t[0]), float(t[1]), float(t[3])
         t_train = float(t[2]) if t_train is not None else None
 
-    # ---- roofline of the dominant kernel (tcgen05 GEMM), instrumented pass on rank 0
+    # ---- roofline of the dominant kernel (wgmma GEMM), instrumented pass on rank 0
     roof = cpu = None
     if rank == 0:
         hbm_peak, tf_peak, how = measured_peaks()
@@ -750,10 +764,9 @@ def run_ours(args):
         _lib._HOOK = None
         ms, fl, n = timer.summary()
         achieved = fl / (ms * 1e-3) / 1e12 if ms > 0 else 0.0
-        roof = {"bound": "tensor", "kernel": "gemm_bf16_tc_kernel (tcgen05.mma kind::f16, all dense layers)",
+        roof = {"bound": "tensor", "kernel": "gemm_bf16_tc_kernel (wgmma.mma_async bf16, all dense layers)",
                 "achieved": achieved, "peak": tf_peak, "unit": "TFLOP/s", "frac": achieved / tf_peak,
-                # DRAM bytes per launch are not measurable inside an un-profiled run; the `ncu --set full` capture of an
-                # in-step launch lives in profiles/ (README there) and is quoted in DESIGN.md, not here
+                # DRAM bytes per launch are not measurable inside an un-profiled run
                 "traffic": None,
                 "peak_source": f"{how} bf16_tflops_sustained", "launches_timed": n,
                 "batches_per_timed_call": G if t_res2 <= t_res else 1,
@@ -790,7 +803,7 @@ def run_ours(args):
             "scaling": "weak", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
             "config": {"workload": WORKLOAD, "global_batch": B_PER_GPU * world, "seq_len": SEQ_LEN,
                        "parallelism": f"dp{world} (sentence-sharded, no data-path collective in PREDICT)",
-                       "l2": "working set/step > 126 MB L2 (170 MB bf16 weights + activations); L2 also flushed by an "
+                       "l2": "working set/step > 50 MB L2 (170 MB bf16 weights + activations); L2 also flushed by an "
                              "untimed 256 MB write between timed steps",
                        "lengths": "MSRA-shaped (mean fill ~0.39)",
                        "streams": (f"{NS} CUDA stream(s) per GPU, consecutive calls alternate; {G} batch(es) of 64 sentences stacked per "
@@ -833,7 +846,11 @@ def main():
     ap.add_argument("--group", type=int, default=4, help="batches stacked per PREDICT call in the second pipeline configuration")
     ap.add_argument("--group-streams", dest="group_streams", type=int, default=2, help="CUDA streams of the stacked configuration")
     ap.add_argument("--sweep", action="store_true", help="time more (streams, batches per call) combinations")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", metavar="DIR", default=None,
+                    help="write what the last timed device-resident PREDICT step returned (pred_ids) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -149,7 +149,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise NerB200Error(
                 f"{LIB_PATH} not found: build it with `python -m chinesener_b200.build` "
-                "(there is no CPU fallback for the sm_100a kernels)")
+                "(there is no CPU fallback for the sm_90a kernels)")
         h = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(h, name)
@@ -179,8 +179,8 @@ _raw_stream = getattr(torch._C, "_cuda_getCurrentRawStream", None)
 
 def stream():
     """cudaStream_t of torch's current stream.  The raw getter avoids building a torch.cuda.Stream object per
-    call: with a non-default stream current (predict_iter(streams>1)) that wrapper cost ~0.4 ms per call on the
-    GPU box's host profile — more than the whole step's device time."""
+    call: with a non-default stream current (predict_iter(streams>1)) that wrapper costs more host time per call
+    than the launches it wraps."""
     if _raw_stream is not None:
         return _raw_stream(torch.cuda.current_device())
     return torch.cuda.current_stream().cuda_stream

@@ -1,8 +1,8 @@
-"""BertModel forward on the sm_100a kernels (bert_base.bert.modeling.BertModel as driven by
+"""BertModel forward on the sm_90a kernels (bert_base.bert.modeling.BertModel as driven by
 reference tools/layer.py:63-81; variable names per SURVEY.md §8 a9 / Appendix A.3).
 
-Per layer: fused-QKV tcgen05 GEMM -> attention kernel -> tcgen05 GEMM (+bias, bf16 out) ->
-LayerNorm(+fp32 residual; writes fp32 + bf16 copies) -> tcgen05 GEMM (+bias, GELU) -> tcgen05
+Per layer: fused-QKV wgmma GEMM -> attention kernel -> wgmma GEMM (+bias, bf16 out) ->
+LayerNorm(+fp32 residual; writes fp32 + bf16 copies) -> wgmma GEMM (+bias, GELU) -> wgmma
 GEMM (+bias, bf16 out) -> LayerNorm(+fp32 residual).  The residual stream stays fp32; GEMM
 operands and dense sub-layer outputs are bf16.
 """
@@ -286,7 +286,7 @@ def _tf_casts(store, cfg, scope):
 
 def bert_forward_f32(input_ids, input_mask, segment_ids, cfg, store=None, scope="bert", gelu="tanh"):
     """BertModel forward at fp32 accuracy (BASELINE config 2: "bert_crf ... fp32", logits within 1e-3 of the
-    reference): every dense layer is the 3-term split-bf16 product on the tcgen05 kernel (ops.gemm_split_f32,
+    reference): every dense layer is the 3-term split-bf16 product on the wgmma kernel (ops.gemm_split_f32,
     ~2^-16 relative), attention is the fp32 kernel (ner_attention_f32, head_dim 64), LayerNorm / GELU / residual
     stream in f32.  Padded layout; keys are limited to the mask's prefix length, which equals the additive
     (1-mask)*-10000 of attention_layer() because exp(-10000 - max) is exactly 0 in fp32.  ~3x the GEMM work of the

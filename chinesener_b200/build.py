@@ -1,4 +1,4 @@
-"""Build libner_b200.so (sm_100a only) in-tree with nvcc.
+"""Build libner_b200.so (sm_90a only) in-tree with nvcc.
 
 `python -m chinesener_b200.build` or `__graft_entry__.build()`.  Objects are rebuilt only
 when a source/header is newer; translation units compile in parallel.
@@ -15,7 +15,7 @@ OBJDIR = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libner_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--use_fast_math=false",
 ]
 NVCC_FLAGS = [f for f in NVCC_FLAGS if f != "--use_fast_math=false"]
@@ -82,7 +82,7 @@ def build(verbose=True, force=False):
         res = list(ex.map(lambda s: _compile(s, verbose), sources()))
     objs = [o for o, _ in res]
     if any(c for _, c in res) or not os.path.exists(LIB):
-        cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+        cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
         if verbose:
             print(" ".join(cmd), flush=True)
         subprocess.run(cmd, check=True)

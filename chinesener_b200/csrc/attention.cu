@@ -1,4 +1,4 @@
-// BERT self-attention core for sm_100a:  ctx = softmax(Q K^T * scale + (1-mask)*mask_add) V
+// BERT self-attention core for sm_90a:  ctx = softmax(Q K^T * scale + (1-mask)*mask_add) V
 // per (batch, head), head_dim = 64.  Replaces attention_layer() of bert_base.bert.modeling as
 // executed from reference tools/layer.py:68-77 (semantics: SURVEY.md Appendix A.3).
 //
@@ -6,7 +6,7 @@
 // single pass: one CTA = 64 query rows of one (b, h); K and V of that head are staged once in
 // shared memory with cp.async (row pitch 144 B -> conflict-free fragment loads / ldmatrix),
 // scores and probabilities never leave registers.  (Attention is 2.7 % of the encoder FLOPs;
-// the dense layers run on tcgen05 — see gemm_tc.cu.)
+// the dense layers run on wgmma — see gemm_tc.cu.)
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -219,7 +219,7 @@ extern "C" int ner_bert_attention(const void* qkv_bf16, const int32_t* mask, voi
   if (n_rows < 0 || (!cu_seqlens && n_rows != 0 && n_rows != B * L)) return NER_ERR_INVALID_ARG;
   if (head_dim != D) return NER_ERR_UNSUPPORTED;
   if (keep_prob >= 1.f && attn_variant() != 1) {
-    // inference: tcgen05 kernel (S and O in tensor memory, operands by TMA); packed mode needs the row count of qkv
+    // inference: wgmma kernel (S and O in registers, operands by TMA); packed mode needs the row count of qkv
     const int rows = cu_seqlens ? n_rows : B * L;
     if (rows > 0) {
       const int rc = ner_bert_attention_tc(qkv_bf16, mask, ctx_bf16, B, L, num_heads, head_dim, scale, mask_add, cu_seqlens,

@@ -1,4 +1,4 @@
-// Backward of the BERT self-attention core (sm_100a), head_dim 64, padded layout:
+// Backward of the BERT self-attention core (sm_90a), head_dim 64, padded layout:
 //   given qkv (bf16 [B*L, 3*NH*64]), the forward context O (bf16) and dO (bf16), produce
 //   d_qkv (bf16, same layout as qkv).  This is the gradient tf.gradients derives through
 //   attention_layer() of bert_base.bert.modeling (reference tools/train_utils.py:314).

@@ -1,4 +1,4 @@
-// fp32 self-attention for small heads, with the TENER relative-position term (sm_100a, SIMT).
+// fp32 self-attention for small heads, with the TENER relative-position term (sm_90a, SIMT).
 //
 // Replaces reference tools/transformer/tener.py:12-119 (relative_attention + shift +
 // normalize_attention + weighted value) for model/transformer_tener_crf_bichar.py:

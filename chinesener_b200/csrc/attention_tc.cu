@@ -1,22 +1,22 @@
-// BERT self-attention core on the 5th-gen tensor cores (tcgen05 + TMEM + TMA), sm_100a, inference path:
+// BERT self-attention core on the Hopper tensor cores (wgmma + TMA + mbarrier), sm_90a, inference path:
 //   ctx = softmax(Q K^T * scale + (1 - mask) * mask_add) V     per (sequence, head), head_dim = 64
 // (attention_layer() of bert_base.bert.modeling as executed from reference tools/layer.py:68-77; SURVEY Appendix A.3).
 //
 // One CTA = one (sequence b, head h, tile of 128 query rows); sequences of up to 256 keys are handled in ONE pass:
 //   thread 0   TMA: Q tile, K rows and V rows of the head come from the fused [rows, 3H] QKV matrix as 64-row x 64-column
 //              bf16 boxes (CU_TENSOR_MAP_SWIZZLE_128B) into shared memory, mbarrier transaction counts
-//   thread 0   MMA 1: S[128, Nk] = Q K^T — four tcgen05.mma.kind::f16 (K = 16 each) from K-major SWIZZLE_128B
-//              descriptors, fp32 accumulator in TENSOR MEMORY (Nk <= 256 columns)
-//   4 warps    softmax straight out of TMEM: warp w owns TMEM lanes 32w..32w+31 = query rows, tcgen05.ld 32 columns at a
-//              time, pass 1 row max, pass 2 exp2 / row sum; the unnormalised probabilities go back to shared memory as bf16
-//              in the canonical K-major SWIZZLE_128B A-operand layout (over the space Q and K occupied)
-//   thread 0   MMA 2: O[128, 64] = P V — V stays as TMA delivered it ([key][d], d contiguous) and is consumed as an
-//              MN-MAJOR B operand (instruction-descriptor b_major = 1, 8-key swizzle atoms 1024 B apart), Nk/16 MMAs,
-//              accumulator over TMEM columns 0..63 (S is dead by then)
-//   4 warps    O rows from TMEM, times 1 / row sum, bf16, 128 contiguous bytes per row to ctx
-// Shared memory 48 KB (Nk <= 128) / 96 KB, TMEM 128 / 256 columns -> 4 / 2 CTAs per SM overlap each other's load -> MMA ->
-// softmax -> MMA -> store chains.  Nothing L x L leaves the SM.  Rows of other sequences that ride along in a 64-row box
-// are masked as keys (probability exactly 0, V rows >= L zeroed in shared memory) and never stored as queries.
+//   2 warpgroups, warpgroup w = query rows 64w .. 64w+63:
+//     MMA 1    S[64, N] = Q K^T — four wgmma.m64nNk16 (K = 16 each) from K-major SWIZZLE_128B descriptors, fp32
+//              accumulator in registers; N = the sequence's key count rounded up to 64 (<= NKMAX)
+//     softmax  in registers (row max / sum over the 4 lanes that share a row); the unnormalised probabilities go to
+//              shared memory as bf16 in the canonical K-major SWIZZLE_128B A-operand layout (over the space Q and K
+//              occupied, after both warpgroups finished reading them)
+//     MMA 2    O[64, 64] = P V — V stays as TMA delivered it ([key][d], d contiguous) and is consumed as an MN-MAJOR
+//              ("transposed") B operand (8-key swizzle atoms 1024 B apart), N/16 MMAs
+//     store    O rows times 1 / row sum, bf16, to ctx
+// Shared memory 48 KB (NKMAX 128) / 96 KB (NKMAX 256).  Nothing L x L leaves the SM.  Rows of other sequences that ride
+// along in a 64-row box are masked as keys (probability exactly 0, V rows >= L zeroed in shared memory) and never stored
+// as queries.
 #include <stdlib.h>
 
 #include "tc_common.cuh"
@@ -27,9 +27,10 @@ using namespace tc;
 using nerdev::fast_ex2;
 
 constexpr int D = 64;          // head_dim
-constexpr int QT = 128;        // query rows per CTA (UMMA M)
+constexpr int QT = 128;        // query rows per CTA (two wgmma M = 64 warpgroups)
 constexpr int BOX_ROWS = 64;   // rows per TMA box
 constexpr int BOX_BYTES = BOX_ROWS * D * 2;   // 8 KB
+constexpr int THREADS = 256;
 
 template <int NKMAX>
 struct ACfg {
@@ -37,32 +38,113 @@ struct ACfg {
   static constexpr int P_BYTES = QT * NKMAX * 2;                          // probabilities, bf16
   static constexpr int REGION_A = QK_BYTES > P_BYTES ? QK_BYTES : P_BYTES;
   static constexpr int V_BYTES = NKMAX * D * 2;
-  static constexpr int TMEM_COLS = NKMAX;                                 // S [128, NKMAX] fp32; O aliases columns 0..63
   static constexpr size_t SMEM = (size_t)REGION_A + V_BYTES + 64 + NKMAX * 4;
 };
 
-// MN-major operand, SWIZZLE_128B: 64 contiguous elements (128 B) along N, 8-row groups along K 1024 B apart (SBO);
-// the tile is one swizzle atom wide in N, so the leading-dimension offset is never used.
-__device__ __forceinline__ uint64_t make_smem_desc_sw128_mn(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;                 // LBO (unused: N = 64 = one atom)
-  d |= (uint64_t)(1024 >> 4) << 32;       // SBO: next group of 8 keys
-  d |= (uint64_t)1 << 46;                 // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                 // SWIZZLE_128B
-  return d;
-}
-__device__ __forceinline__ uint32_t idesc_bf16(int M, int N, bool b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (b_mn_major ? (1u << 16) : 0u) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
-}
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
+// S = Q K^T for this warpgroup's 64 rows over N key columns, softmax numerators into the P tile, then O = P V and the
+// normalised store.  r_lo = this thread's first row within the CTA tile (the second is r_lo + 8).  live = this warpgroup
+// has query rows (false for warpgroup 1 when the tile holds <= 64 of them): it then only joins the CTA barriers and the
+// zeroing of V, and issues no MMA.
+template <int N>
+__device__ __forceinline__ void attend(uint8_t* s_q, uint8_t* s_k, uint8_t* s_p, uint8_t* s_v, const float* s_madd, int wg,
+                                       bool live, int r_lo, int L, float sc, uint64_t* v_bar, __nv_bfloat16* ctx,
+                                       size_t out_row0, int HD, int h, int q0) {
+  const int lane = threadIdx.x & 31;
+  constexpr float kLog2e = 1.4426950408889634f;
+  float s[N / 2];
+  float lsum[2] = {0.f, 0.f};
+  if (live) {
+    const uint32_t qa = smem_u32(s_q) + wg * 64 * 128, ka = smem_u32(s_k);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < D / 16; ++k)
+      wgmma_bf16<N, 0, 0>(s, make_wgmma_desc_sw128(qa + k * 32), make_wgmma_desc_sw128(ka + k * 32), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    // scores in the log2 domain: x = s*scale*log2e + madd*log2e; columns >= L (other sequences' or never loaded key rows)
+    // are excluded by a select, so whatever their score holds (NaN included) never reaches the max, the sum or P
+    float mx[2] = {-3.0e38f, -3.0e38f};
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int c = 8 * j + 2 * (lane & 3) + (e & 1);
+        const float x = fmaf(s[4 * j + e], sc, s_madd[c] * kLog2e);
+        s[4 * j + e] = x;
+        if (c < L) mx[e >> 1] = fmaxf(mx[e >> 1], x);
+      }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+    }
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int c = 8 * j + 2 * (lane & 3) + (e & 1);
+        const float p = (c < L) ? fast_ex2(s[4 * j + e] - mx[e >> 1]) : 0.f;
+        s[4 * j + e] = p;
+        lsum[e >> 1] += p;
+      }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      lsum[hh] += __shfl_xor_sync(0xffffffffu, lsum[hh], 1);
+      lsum[hh] += __shfl_xor_sync(0xffffffffu, lsum[hh], 2);
+    }
+  }
+  __syncthreads();                             // both warpgroups are done reading Q and K: P may overwrite them
+  if (live) {
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int r = r_lo + 8 * hh, c = 8 * j + 2 * (lane & 3);
+        uint8_t* blk = s_p + (c >> 6) * (QT * 128) + (r >> 3) * 1024 + (r & 7) * 128;
+        *reinterpret_cast<uint32_t*>(blk + ((((c & 63) >> 3) ^ (r & 7)) << 4) + (c & 7) * 2) =
+            pack_bf16x2(s[4 * j + 2 * hh], s[4 * j + 2 * hh + 1]);
+      }
+  }
+  // V rows [L, N) belong to other sequences (or were never loaded): zero them so that 0 * x stays 0
+  mbar_wait(v_bar, 0);
+  for (int idx = threadIdx.x; idx < (N - L) * 8; idx += THREADS)
+    *reinterpret_cast<uint4*>(s_v + (size_t)(L + (idx >> 3)) * 128 + ((idx & 7) << 4)) = make_uint4(0, 0, 0, 0);
+  fence_proxy_async();                         // P and the zeroed V rows: generic-proxy writes -> visible to wgmma
+  __syncthreads();
+  if (!live) return;
+
+  float o[D / 2];
+  {
+    const uint32_t pa = smem_u32(s_p) + wg * 64 * 128, va = smem_u32(s_v);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < N / 16; ++ks)
+      wgmma_bf16<D, 0, 1>(o, make_wgmma_desc_sw128(pa + (ks >> 2) * (QT * 128) + (ks & 3) * 32),
+                          make_wgmma_desc_sw128(va + ks * 2048), ks > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+  }
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int r = r_lo + 8 * hh;
+    if (q0 + r >= L) continue;
+    const float inv = 1.f / lsum[hh];
+    __nv_bfloat16* orow = ctx + (out_row0 + r) * HD + h * D;
+#pragma unroll
+    for (int j = 0; j < D / 8; ++j)
+      *reinterpret_cast<uint32_t*>(orow + 8 * j + 2 * (lane & 3)) = pack_bf16x2(o[4 * j + 2 * hh] * inv, o[4 * j + 2 * hh + 1] * inv);
+  }
+}
+
 template <int NKMAX>
-__global__ void __launch_bounds__(128)
+__global__ void __launch_bounds__(THREADS)
 bert_attention_tc_kernel(const __grid_constant__ CUtensorMap tma_qkv, const int32_t* __restrict__ mask,
                          __nv_bfloat16* __restrict__ ctx, int Lpad, int NH, float scale, float mask_add,
                          const int32_t* __restrict__ cu_seqlens) {
@@ -74,140 +156,54 @@ bert_attention_tc_kernel(const __grid_constant__ CUtensorMap tma_qkv, const int3
   uint8_t* s_k = smem + QT * D * 2;            // [Nk rows][128 B]
   uint8_t* s_p = smem;                         // [Nk/64 blocks][128 rows][128 B] — written after S is complete
   uint8_t* s_v = smem + C::REGION_A;           // [Nk rows][128 B]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_v + C::V_BYTES);   // qk, v, s, o
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 4);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_v + C::V_BYTES);   // qk, v
   float* s_madd = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 64);
 
   const int b = blockIdx.z, h = blockIdx.y, qt = blockIdx.x;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, wg = tid >> 7;
   const int HD = NH * D;
 
   if (tid == 0) {
     tma_prefetch_desc(&tma_qkv);
-    for (int i = 0; i < 4; ++i) mbar_init(&bars[i], 1);
+    for (int i = 0; i < 2; ++i) mbar_init(&bars[i], 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<C::TMEM_COLS>(tmem_ptr);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   nerdev::pdl_wait();                         // QKV comes from the GEMM just before this kernel in the stream
 
   // padded mode: rows [b*Lpad, (b+1)*Lpad), keys masked by `mask`; packed mode: rows [cu[b], cu[b+1]), all keys valid
   const int row_base = cu_seqlens ? cu_seqlens[b] : b * Lpad;
   const int L = cu_seqlens ? (cu_seqlens[b + 1] - row_base) : Lpad;
   const int q0 = qt * QT;
-  const bool active = q0 < L;                 // uniform over the CTA
-  const int nk = (L + 31) & ~31;              // UMMA N of S = K extent of P V (multiple of 32, <= NKMAX)
-  const int kv_boxes = (L + BOX_ROWS - 1) / BOX_ROWS;
+  if (q0 >= L) return;                        // uniform over the CTA
+  const int n64 = (L + 63) & ~63;             // wgmma N of S = K extent of P V (multiple of 64, <= NKMAX)
+  const int kv_boxes = n64 / BOX_ROWS;
   const int q_rows = min(QT, L - q0);
   const int q_boxes = (q_rows + BOX_ROWS - 1) / BOX_ROWS;
 
-  if (active) {
-    if (tid == 0) {
-      mbar_arrive_expect_tx(&bars[0], (uint32_t)((q_boxes + kv_boxes) * BOX_BYTES));
-      for (int i = 0; i < q_boxes; ++i) tma_load_2d(s_q + i * BOX_BYTES, &tma_qkv, &bars[0], h * D, row_base + q0 + i * BOX_ROWS);
-      for (int i = 0; i < kv_boxes; ++i) tma_load_2d(s_k + i * BOX_BYTES, &tma_qkv, &bars[0], HD + h * D, row_base + i * BOX_ROWS);
-      mbar_arrive_expect_tx(&bars[1], (uint32_t)(kv_boxes * BOX_BYTES));
-      for (int i = 0; i < kv_boxes; ++i) tma_load_2d(s_v + i * BOX_BYTES, &tma_qkv, &bars[1], 2 * HD + h * D, row_base + i * BOX_ROWS);
-    }
-    for (int k = tid; k < nk; k += 128)
-      s_madd[k] = (k < L) ? (cu_seqlens ? 0.f : (1.f - (float)mask[(size_t)b * Lpad + k]) * mask_add) : -1e30f;
-
-    if (tid == 0) {
-      // ---- S = Q K^T
-      mbar_wait(&bars[0], 0);
-      tcgen05_fence_after();
-      const uint32_t idesc = idesc_bf16(QT, nk, false);
-      const uint32_t qa = smem_u32(s_q), ka = smem_u32(s_k);
-#pragma unroll
-      for (int k = 0; k < D / 16; ++k)
-        umma_f16(tmem_base, make_smem_desc_sw128(qa + k * 32), make_smem_desc_sw128(ka + k * 32), idesc, k > 0 ? 1u : 0u);
-      umma_commit(&bars[2]);
-    }
-    __syncthreads();                          // s_madd visible
-
-    // ---- softmax out of TMEM: thread = query row (TMEM lane 32*warp + lane)
-    const int r = warp * 32 + lane;
-    const uint32_t trow = tmem_base + ((uint32_t)(warp * 32) << 16);
-    constexpr float kLog2e = 1.4426950408889634f;
-    const float sc = scale * kLog2e;          // scores kept in the log2 domain: x = s*scale*log2e + madd*log2e
-    mbar_wait(&bars[2], 0);
-    tcgen05_fence_after();
-    float mx = -3.0e38f;
-    for (int c = 0; c < nk; c += 32) {
-      uint32_t ra[32];
-      tmem_ld_32x32(trow + (uint32_t)c, ra);
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 32; ++i) mx = fmaxf(mx, fmaf(__uint_as_float(ra[i]), sc, s_madd[c + i] * kLog2e));
-    }
-    float lsum = 0.f;
-    const int sw = r & 7;
-    uint8_t* prow = s_p + (r >> 3) * 1024 + sw * 128;
-    for (int c = 0; c < nk; c += 32) {
-      uint32_t ra[32];
-      tmem_ld_32x32(trow + (uint32_t)c, ra);
-      tmem_ld_wait();
-      float p[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        // columns >= L carry madd = -1e30: ex2 underflows to exactly 0 whatever the (possibly foreign) key row held;
-        // the select keeps a NaN score of such a column out of the sum
-        const float x = fmaf(__uint_as_float(ra[i]), sc, s_madd[c + i] * kLog2e) - mx;
-        p[i] = (c + i < L) ? fast_ex2(x) : 0.f;
-        lsum += p[i];
-      }
-      uint8_t* blk = prow + (c >> 6) * (QT * 128);        // 64-key block of the P tile
-      const int ch0 = (c & 32) >> 3;                      // first 16-byte chunk of this half block
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        *reinterpret_cast<uint4*>(blk + (((ch0 + j) ^ sw) << 4)) =
-            make_uint4(pack_bf16x2(p[8 * j + 0], p[8 * j + 1]), pack_bf16x2(p[8 * j + 2], p[8 * j + 3]),
-                       pack_bf16x2(p[8 * j + 4], p[8 * j + 5]), pack_bf16x2(p[8 * j + 6], p[8 * j + 7]));
-    }
-    // V rows [L, nk) belong to other sequences (or lie past the matrix): zero them so that 0 * x stays 0
-    mbar_wait(&bars[1], 0);
-    for (int idx = tid; idx < (nk - L) * 8; idx += 128)
-      *reinterpret_cast<uint4*>(s_v + (size_t)(L + (idx >> 3)) * 128 + ((idx & 7) << 4)) = make_uint4(0, 0, 0, 0);
-    fence_proxy_async();                      // P and the zeroed V rows: generic-proxy writes -> visible to the MMA (async proxy)
-    tcgen05_fence_before();
-    __syncthreads();                          // every thread has finished reading S: O may overwrite its columns
-
-    if (tid == 0) {
-      // ---- O = P V   (A = P K-major, B = V MN-major)
-      tcgen05_fence_after();
-      const uint32_t idesc = idesc_bf16(QT, D, true);
-      const uint32_t pa = smem_u32(s_p), va = smem_u32(s_v);
-      for (int ks = 0; ks < nk / 16; ++ks)
-        umma_f16(tmem_base, make_smem_desc_sw128(pa + (ks >> 2) * (QT * 128) + (ks & 3) * 32),
-                 make_smem_desc_sw128_mn(va + ks * 2048), idesc, ks > 0 ? 1u : 0u);
-      umma_commit(&bars[3]);
-    }
-    mbar_wait(&bars[3], 0);
-    tcgen05_fence_after();
-    const float inv = 1.f / lsum;
-    __nv_bfloat16* orow = ctx + (size_t)(row_base + q0 + r) * HD + h * D;
-#pragma unroll
-    for (int half = 0; half < 2; ++half) {
-      uint32_t ra[32];
-      tmem_ld_32x32(trow + (uint32_t)(half * 32), ra);      // warp-collective: every lane executes it, rows >= L only skip the store
-      tmem_ld_wait();
-      if (q0 + r < L) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          *reinterpret_cast<uint4*>(orow + half * 32 + j * 8) =
-              make_uint4(pack_bf16x2(__uint_as_float(ra[8 * j + 0]) * inv, __uint_as_float(ra[8 * j + 1]) * inv),
-                         pack_bf16x2(__uint_as_float(ra[8 * j + 2]) * inv, __uint_as_float(ra[8 * j + 3]) * inv),
-                         pack_bf16x2(__uint_as_float(ra[8 * j + 4]) * inv, __uint_as_float(ra[8 * j + 5]) * inv),
-                         pack_bf16x2(__uint_as_float(ra[8 * j + 6]) * inv, __uint_as_float(ra[8 * j + 7]) * inv));
-      }
-    }
+  if (tid == 0) {
+    mbar_arrive_expect_tx(&bars[0], (uint32_t)((q_boxes + kv_boxes) * BOX_BYTES));
+    for (int i = 0; i < q_boxes; ++i) tma_load_2d(s_q + i * BOX_BYTES, &tma_qkv, &bars[0], h * D, row_base + q0 + i * BOX_ROWS);
+    for (int i = 0; i < kv_boxes; ++i) tma_load_2d(s_k + i * BOX_BYTES, &tma_qkv, &bars[0], HD + h * D, row_base + i * BOX_ROWS);
+    mbar_arrive_expect_tx(&bars[1], (uint32_t)(kv_boxes * BOX_BYTES));
+    for (int i = 0; i < kv_boxes; ++i) tma_load_2d(s_v + i * BOX_BYTES, &tma_qkv, &bars[1], 2 * HD + h * D, row_base + i * BOX_ROWS);
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<C::TMEM_COLS>(tmem_base);
+  for (int k = tid; k < n64; k += THREADS)
+    s_madd[k] = (k < L) ? (cu_seqlens ? 0.f : (1.f - (float)mask[(size_t)b * Lpad + k]) * mask_add) : -1e30f;
+  __syncthreads();                            // s_madd visible
+  mbar_wait(&bars[0], 0);
+
+  constexpr float kLog2e = 1.4426950408889634f;
+  const float sc = scale * kLog2e;
+  const int r_lo = wg * 64 + ((tid >> 5) & 3) * 16 + ((tid & 31) >> 2);
+  const size_t out_row0 = (size_t)row_base + q0;
+  const bool live = wg * 64 < q_rows;         // uniform over the warpgroup
+  if (n64 <= 64) attend<64>(s_q, s_k, s_p, s_v, s_madd, wg, live, r_lo, L, sc, &bars[1], ctx, out_row0, HD, h, q0);
+  else if (n64 <= 128 || NKMAX == 128) attend<128>(s_q, s_k, s_p, s_v, s_madd, wg, live, r_lo, L, sc, &bars[1], ctx, out_row0, HD, h, q0);
+  else if constexpr (NKMAX == 256) {
+    if (n64 <= 192) attend<192>(s_q, s_k, s_p, s_v, s_madd, wg, live, r_lo, L, sc, &bars[1], ctx, out_row0, HD, h, q0);
+    else attend<256>(s_q, s_k, s_p, s_v, s_madd, wg, live, r_lo, L, sc, &bars[1], ctx, out_row0, HD, h, q0);
+  }
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -237,7 +233,7 @@ int launch(const CUtensorMap& map, const int32_t* mask, void* ctx, int B, int L,
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
   dim3 grid((L + QT - 1) / QT, NH, B);
-  e = ner_launch_pdl(kern, grid, dim3(128), smem, st, map, mask, static_cast<__nv_bfloat16*>(ctx), L, NH, scale, mask_add,
+  e = ner_launch_pdl(kern, grid, dim3(THREADS), smem, st, map, mask, static_cast<__nv_bfloat16*>(ctx), L, NH, scale, mask_add,
                      cu_seqlens);
   if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
   return ner_launch_status();
@@ -245,7 +241,7 @@ int launch(const CUtensorMap& map, const int32_t* mask, void* ctx, int B, int L,
 
 }  // namespace
 
-// tcgen05 path of ner_bert_attention (inference: no attention-probs dropout).  NER_ERR_UNSUPPORTED = not applicable
+// wgmma path of ner_bert_attention (inference: no attention-probs dropout).  NER_ERR_UNSUPPORTED = not applicable
 // (caller falls back to the mma.sync kernel): head_dim != 64, sequences longer than 256, misaligned QKV.
 int ner_bert_attention_tc(const void* qkv_bf16, const int32_t* mask, void* ctx_bf16, int B, int L, int num_heads, int head_dim,
                           float scale, float mask_add, const int32_t* cu_seqlens, int n_rows, cudaStream_t st) {

@@ -1,7 +1,7 @@
-// Backward-pass HBM-bound kernels of the encoder (sm_100a): LayerNorm backward (with the residual
+// Backward-pass HBM-bound kernels of the encoder (sm_90a): LayerNorm backward (with the residual
 // recomputed from the saved operands), bf16 transposes for the weight-gradient GEMMs, bias
 // gradients of bf16 tensors, GELU backward, and the embedding scatter-add.  Together with the
-// tcgen05 GEMM (gemm_tc.cu) and attention_bwd.cu they are the gradient that tf.gradients produces
+// wgmma GEMM (gemm_tc.cu) and attention_bwd.cu they are the gradient that tf.gradients produces
 // for bert_base.bert.modeling.BertModel in the reference (tools/train_utils.py:314).
 #include "common.cuh"
 
@@ -168,8 +168,7 @@ transpose_bf16_scalar_kernel(const __nv_bfloat16* __restrict__ src, __nv_bfloat1
 // Same for even N: 2x2 sub-blocks.  A thread loads the words (m, n..n+1) and (m+1, n..n+1), re-pairs them with two
 // PRMTs into (n; m..m+1) and (n+1; m..m+1) and parks those in a [64 n][32 m-pair] word tile (pitch 33: the 16-byte
 // output reads are conflict-free, the parking stores 2-way); output rows leave as 16-byte stores.  Half the
-// memory instructions of the scalar kernel and 4x wider ones on the store side (the wgrad operand transposes
-// were 2.2 ms of an 18 ms TRAIN step).
+// memory instructions of the scalar kernel and 4x wider ones on the store side.
 __global__ void __launch_bounds__(256)
 transpose_bf16_kernel(const __nv_bfloat16* __restrict__ src, __nv_bfloat16* __restrict__ dst, int M, int N, int Mp) {
   __shared__ uint32_t t[64][33];
@@ -251,6 +250,21 @@ colsum_bf16_v8_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ o
   }
 }
 
+// gelu'(v), tanh approximation or erf.  Every operation is an explicitly rounded intrinsic, so the compiler cannot contract
+// it differently in the two kernels below: the fused-bias kernel must reproduce ner_gelu_bwd_bf16 bit for bit.
+__device__ __forceinline__ float gelu_grad(float v, int erf_variant) {
+  if (erf_variant) {
+    const float cdf = __fmul_rn(0.5f, __fadd_rn(1.f, erff(__fmul_rn(v, 0.7071067811865476f))));
+    const float pdf = __expf(__fmul_rn(__fmul_rn(-0.5f, v), v));
+    return __fadd_rn(cdf, __fmul_rn(__fmul_rn(v, 0.3989422804014327f), pdf));
+  }
+  const float v2 = __fmul_rn(v, v);
+  const float u = __fmul_rn(0.7978845608028654f, __fadd_rn(v, __fmul_rn(__fmul_rn(0.044715f, v2), v)));
+  const float t = tanhf(u);
+  const float du = __fmul_rn(0.7978845608028654f, __fadd_rn(1.f, __fmul_rn(3.f * 0.044715f, v2)));
+  return __fadd_rn(__fmul_rn(0.5f, __fadd_rn(1.f, t)), __fmul_rn(__fmul_rn(__fmul_rn(0.5f, v), __fsub_rn(1.f, __fmul_rn(t, t))), du));
+}
+
 // d_pre = d_act * gelu'(pre)   (tanh approximation or erf), all bf16
 __global__ void __launch_bounds__(256)
 gelu_bwd_kernel(const __nv_bfloat16* __restrict__ pre, const __nv_bfloat16* __restrict__ dact,
@@ -260,30 +274,13 @@ gelu_bwd_kernel(const __nv_bfloat16* __restrict__ pre, const __nv_bfloat16* __re
     const float4 x = ld_bf16x4(pre + 4 * i), g = ld_bf16x4(dact + 4 * i);
     float xs[4] = {x.x, x.y, x.z, x.w}, gs[4] = {g.x, g.y, g.z, g.w}, o[4];
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float v = xs[k];
-      float d;
-      if (erf_variant) {
-        d = 0.5f * (1.f + erff(v * 0.7071067811865476f)) + v * 0.3989422804014327f * __expf(-0.5f * v * v);
-      } else {
-        const float u = 0.7978845608028654f * (v + 0.044715f * v * v * v);
-        const float t = tanhf(u);
-        d = 0.5f * (1.f + t) + 0.5f * v * (1.f - t * t) * 0.7978845608028654f * (1.f + 3.f * 0.044715f * v * v);
-      }
-      o[k] = gs[k] * d;
-    }
+    for (int k = 0; k < 4; ++k) o[k] = gs[k] * gelu_grad(xs[k], erf_variant);
     st_bf16x4(dpre + 4 * i, make_float4(o[0], o[1], o[2], o[3]));
   }
 }
 
 // The same with the bias gradient of the dense layer in front of the GELU fused in: d_bias[c] += sum over rows of d_pre[:, c]
 // (2-D tiling of colsum_bf16_v8_kernel: a lane owns 8 consecutive columns, the CTA's 8 warps stride over rows).
-__device__ __forceinline__ float gelu_grad(float v, int erf_variant) {
-  if (erf_variant) return 0.5f * (1.f + erff(v * 0.7071067811865476f)) + v * 0.3989422804014327f * __expf(-0.5f * v * v);
-  const float u = 0.7978845608028654f * (v + 0.044715f * v * v * v);
-  const float t = tanhf(u);
-  return 0.5f * (1.f + t) + 0.5f * v * (1.f - t * t) * 0.7978845608028654f * (1.f + 3.f * 0.044715f * v * v);
-}
 __global__ void __launch_bounds__(256)
 gelu_bwd_bias_kernel(const __nv_bfloat16* __restrict__ pre, const __nv_bfloat16* __restrict__ dact,
                      __nv_bfloat16* __restrict__ dpre, float* __restrict__ dbias, int M, int N, int erf_variant) {
@@ -361,13 +358,13 @@ bert_embed_bwd_kernel(const float* __restrict__ dx, const int32_t* __restrict__ 
 
 int rows_grid(int rows, int per_block) {
   long g = ((long)rows + per_block - 1) / per_block;
-  if (g > 148L * 8) g = 148L * 8;
+  if (g > (long)ner_num_sms() * 8) g = (long)ner_num_sms() * 8;
   if (g < 1) g = 1;
   return (int)g;
 }
 int flat_grid(size_t n) {
   size_t g = (n + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > ner_num_sms() * 16) g = ner_num_sms() * 16;
   if (g < 1) g = 1;
   return (int)g;
 }
@@ -397,8 +394,8 @@ extern "C" int ner_layernorm_dropout_bwd_bias(const void* y, int y_is_bf16, cons
   if (H % 4 != 0 || H > 128 * LN_MAXV) return NER_ERR_UNSUPPORTED;
   const size_t smem = (size_t)8 * 3 * H * 4;   // per-warp column partials
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // two CTAs per SM: rows per CTA sized so that the grid covers 2 x 148 CTA slots once
-  int per_block = ((M + 2 * 148 - 1) / (2 * 148) + 7) / 8 * 8;
+  // two CTAs per SM: rows per CTA sized so that the grid covers 2 x #SMs CTA slots once
+  int per_block = ((M + 2 * ner_num_sms() - 1) / (2 * ner_num_sms()) + 7) / 8 * 8;
   per_block = per_block < 8 ? 8 : (per_block > 64 ? 64 : per_block);
   const int grid = rows_grid(M, per_block);
   const bool drop = keep_prob < 1.f;
@@ -444,7 +441,7 @@ extern "C" int ner_colsum_bf16_add(const void* x_bf16, float* out, int M, int N,
   if (M == 0) return NER_OK;
   if (N % 8 == 0 && (reinterpret_cast<uintptr_t>(x_bf16) & 15) == 0) {
     const int cb = (N + 255) / 256;
-    int gy = (2 * 148 + cb - 1) / cb;          // ~2 CTAs per SM in total
+    int gy = (2 * ner_num_sms() + cb - 1) / cb;          // ~2 CTAs per SM in total
     if (gy > (M + 7) / 8) gy = (M + 7) / 8;
     colsum_bf16_v8_kernel<<<dim3(cb, gy), 256, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<const __nv_bfloat16*>(x_bf16),
                                                                                         out, M, N);
@@ -501,7 +498,7 @@ extern "C" int ner_gelu_bwd_bias_bf16(const void* pre_bf16, const void* dact_bf1
                       reinterpret_cast<uintptr_t>(dpre_bf16)) & 15) != 0)
     return NER_ERR_UNSUPPORTED;
   const int cb = (N + 255) / 256;
-  int gy = (4 * 148 + cb - 1) / cb;
+  int gy = (4 * ner_num_sms() + cb - 1) / cb;
   if (gy > (M + 7) / 8) gy = (M + 7) / 8;
   gelu_bwd_bias_kernel<<<dim3(cb, gy), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(pre_bf16), static_cast<const __nv_bfloat16*>(dact_bf16),

@@ -1,4 +1,4 @@
-// HBM-bound glue kernels of the encoder path (sm_100a): embedding-sum + LayerNorm, LayerNorm,
+// HBM-bound glue kernels of the encoder path (sm_90a): embedding-sum + LayerNorm, LayerNorm,
 // weight packing / casts, and the small-N (label_size) dense projection.
 //
 // Reference call sites: bert_base.bert.modeling (embedding_postprocessor, layer_norm) executed
@@ -371,7 +371,7 @@ split_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ hi,
 
 int grid_for_rows(int rows, int rows_per_block) {
   long g = ((long)rows + rows_per_block - 1) / rows_per_block;
-  if (g > 148L * 16) g = 148L * 16;
+  if (g > (long)ner_num_sms() * 16) g = (long)ner_num_sms() * 16;
   if (g < 1) g = 1;
   return (int)g;
 }
@@ -450,7 +450,7 @@ extern "C" int ner_cast_bf16(const float* src, void* dst_bf16, size_t n, ner_str
   if (!src || !dst_bf16) return n == 0 ? NER_OK : NER_ERR_INVALID_ARG;
   if (n == 0) return NER_OK;
   size_t g = (n + 255) / 256;
-  if (g > 148 * 32) g = 148 * 32;
+  if (g > ner_num_sms() * 32) g = ner_num_sms() * 32;
   cast_bf16_kernel<<<(int)g, 256, 0, static_cast<cudaStream_t>(stream)>>>(src, static_cast<__nv_bfloat16*>(dst_bf16), n);
   return ner_launch_status();
 }
@@ -497,7 +497,7 @@ extern "C" int ner_cast_pad_bf16(const float* src, void* dst_bf16, int M, int D,
   if (M == 0) return NER_OK;
   if (!src || !dst_bf16) return NER_ERR_INVALID_ARG;
   size_t g = ((size_t)M * Dp + 255) / 256;
-  if (g > 148 * 32) g = 148 * 32;
+  if (g > ner_num_sms() * 32) g = ner_num_sms() * 32;
   cast_pad_bf16_kernel<<<(int)g, 256, 0, static_cast<cudaStream_t>(stream)>>>(src, static_cast<__nv_bfloat16*>(dst_bf16), M,
                                                                               D, Dp, ld_src);
   return ner_launch_status();
@@ -524,7 +524,7 @@ extern "C" int ner_split_bf16(const float* src, void* hi_bf16, void* lo_bf16, in
   if (M == 0) return NER_OK;
   if (!src || !hi_bf16 || !lo_bf16) return NER_ERR_INVALID_ARG;
   size_t g = ((size_t)M * Dp + 255) / 256;
-  if (g > 148 * 32) g = 148 * 32;
+  if (g > ner_num_sms() * 32) g = ner_num_sms() * 32;
   split_bf16_kernel<<<(int)g, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       src, static_cast<__nv_bfloat16*>(hi_bf16), static_cast<__nv_bfloat16*>(lo_bf16), M, D, Dp, ld_src);
   return ner_launch_status();

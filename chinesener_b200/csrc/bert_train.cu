@@ -2,8 +2,7 @@
 // with is_training=True as driven from reference tools/layer.py:63-81, gradients as tf.gradients
 // derives them at tools/train_utils.py:314).  The host loops below only enqueue kernels (≈11 per
 // layer forward, ≈27 per layer backward) on the caller's stream: issued from Python the same
-// sequence costs ~20 us of host time per launch and the TRAIN step was launch-bound (19 ms of host
-// time for ~7 ms of device work, profiles/README.md trip 19).
+// sequence costs tens of microseconds of host time per launch, which made the TRAIN step launch-bound.
 //
 // Saved activations (padded layout, rows = B*L), one block per layer:
 //   x32 f32 | x16 bf16 (layer input) | qkv bf16 | ctx bf16 | y1 bf16 | x1_32 f32 | x1_16 bf16 |
@@ -323,7 +322,7 @@ static int train_bwd_impl(const ner_bert_config* cfg, const float* emb_ln_gamma,
       NER_TRY(ner_transpose_bf16(s.x16, xt, rows, H, Rp, stream));
       NER_TRY(ner_transpose_bf16(dqkv, dyt, rows, 3 * H, Rp, stream));
       NER_TRY(ner_gemm_bf16(xt, dyt, nullptr, nullptr, dwqkv, H, 3 * H, Rp, NER_EPI_F32, 0, stream));
-      add_split3_kernel<<<148 * 4, 256, 0, st>>>(dwqkv, g.d_wq, g.d_wk, g.d_wv, H);
+      add_split3_kernel<<<ner_num_sms() * 4, 256, 0, st>>>(dwqkv, g.d_wq, g.d_wk, g.d_wv, H);
       NER_TRY(ner_launch_status());
     }
     float* dprev = (dx1 == dA) ? dB : dA;

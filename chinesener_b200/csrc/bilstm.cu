@@ -1,4 +1,4 @@
-// BiLSTM recurrence as a persistent thread-block-cluster kernel (sm_100a).
+// BiLSTM recurrence as a persistent thread-block-cluster kernel (sm_90a).
 //
 // Replaces tf.nn.bidirectional_dynamic_rnn over tf.nn.rnn_cell.LSTMCell as built by
 // reference tools/layer.py:10-41 (gate order i,j,f,o; forget_bias 1.0; zero initial state;
@@ -6,7 +6,7 @@
 // reverse_sequence(x, seq_len) and is reversed back — SURVEY.md Appendix A.2).
 //
 // The input half of the LSTMCell matmul ([x_t] · kernel[:D]) + bias is hoisted out of the
-// recurrence into ONE tcgen05 GEMM for both directions (xproj [B*L, 8H], gemm_tc.cu).  This
+// recurrence into ONE wgmma GEMM for both directions (xproj [B*L, 8H], gemm_tc.cu).  This
 // kernel runs the sequential half: a cluster of C CTAs owns R batch rows of one direction for
 // all time steps.  Each CTA keeps its slice of the recurrent matrix kernel[D:, :] resident in
 // shared memory for the whole sequence (fp32, [H][4*H/C] laid out so one LDS.128 yields four
@@ -361,12 +361,12 @@ extern "C" int ner_bilstm_recurrence(const float* xproj, const float* wh_fw, con
   const int C = pick_cluster(H);
   if (C == 0) return NER_ERR_UNSUPPORTED;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // rows per cluster: fill the 148 SMs once when the batch is small, amortise W_h reads when large
+  // rows per cluster: fill the SMs once when the batch is small, amortise W_h reads when large
   int R = 1;
-  if ((long)2 * B * C > 148) R = 2;
-  if ((long)2 * ((B + 1) / 2) * C > 2 * 148) R = 4;
+  if ((long)2 * B * C > ner_num_sms()) R = 2;
+  if ((long)2 * ((B + 1) / 2) * C > 2 * ner_num_sms()) R = 4;
   // four stacked PREDICT batches (B = 256): 4 rows per cluster would be 256 CTAs = two waves of the one-CTA-per-SM kernel
-  if (H == 128 && (long)2 * ((B + 3) / 4) * C > 148) R = 8;
+  if (H == 128 && (long)2 * ((B + 3) / 4) * C > ner_num_sms()) R = 8;
   if (const char* e = getenv("NER_BILSTM_ROWS")) {   // tuning hook: rows per cluster (1, 2, 4 or 8)
     const int v = atoi(e);
     if (v == 1 || v == 2 || v == 4 || (v == 8 && H == 128)) R = v;

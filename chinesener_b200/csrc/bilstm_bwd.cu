@@ -1,4 +1,4 @@
-// Back-propagation-through-time of the BiLSTM recurrence (sm_100a), the gradient the reference
+// Back-propagation-through-time of the BiLSTM recurrence (sm_90a), the gradient the reference
 // obtains from tf.gradients through bidirectional_dynamic_rnn (reference tools/train_utils.py:383
 // over tools/layer.py:27-41).
 //
@@ -38,7 +38,7 @@ __device__ __forceinline__ float actf(float x) {
 // WR > 0 (H = 128): the recurrent matrix slice lives in REGISTERS — thread (k, part) = (tid / 4, tid % 4) keeps
 // kernel[D + rank*HU + k, part*WR .. part*WR + WR) and forms dh_prev[r][k] for all R rows from float4 reads of the gathered
 // gate gradients (one address per `part` in a warp -> broadcasts; the per-part padding of 4 floats keeps the four parts on
-// different banks).  The shared-memory walk it replaces issued two LDS per FMA (6.9 us per step at H = 128).
+// different banks).  The shared-memory walk it replaces issued two LDS per FMA.
 template <int R, int ACT, int WR>
 __global__ void __launch_bounds__(WR > 0 ? 256 : 512, 1)
 bilstm_bwd_kernel(const float* __restrict__ d_out, const float* __restrict__ gates, const float* __restrict__ cstate,
@@ -289,7 +289,7 @@ extern "C" int ner_bilstm_recurrence_bwd(const float* d_out, const float* gates,
   if (C == 0 || (H / C) > 256) return NER_ERR_UNSUPPORTED;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   int R = 1;
-  if ((long)2 * B * C > 148) R = 2;
+  if ((long)2 * B * C > ner_num_sms()) R = 2;
   if (2 * (H / C) > 512) R = 1;
 #define GO(RR, WRR)                                                                                                \
   return activation == 1 ? launch_bwd<RR, 1, WRR>(d_out, gates, cstate, wh_fw, wh_bw, seq_len, d_xproj, B, L, H, C, keep_prob, seed, st) \

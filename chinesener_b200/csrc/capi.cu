@@ -7,11 +7,11 @@ extern "C" int ner_abi_version(void) { return 2; }   // 2: ner_bert_attention ta
 #ifndef NER_SOURCE_HASH
 #define NER_SOURCE_HASH "unknown"
 #endif
-// "src=<sha256[:16] of csrc/*.cu, csrc/*.cuh, include/*.h> nvcc=<major.minor> arch=sm_100a": what chinesener_b200/build.py
+// "src=<sha256[:16] of csrc/*.cu, csrc/*.cuh, include/*.h> nvcc=<major.minor> arch=sm_90a": what chinesener_b200/build.py
 // computed over the tree this object was compiled from (build provenance: the .so files are shipped prebuilt).
 extern "C" const char* ner_build_info(void) {
   static char info[128];
-  snprintf(info, sizeof(info), "src=%s nvcc=%d.%d arch=sm_100a", NER_SOURCE_HASH, __CUDACC_VER_MAJOR__, __CUDACC_VER_MINOR__);
+  snprintf(info, sizeof(info), "src=%s nvcc=%d.%d arch=sm_90a", NER_SOURCE_HASH, __CUDACC_VER_MAJOR__, __CUDACC_VER_MINOR__);
   return info;
 }
 
@@ -20,7 +20,7 @@ extern "C" const char* ner_strerror(int status) {
   switch (status) {
     case NER_OK: return "ok";
     case NER_ERR_INVALID_ARG: return "invalid argument (null pointer, bad size, misaligned buffer or bad enum)";
-    case NER_ERR_UNSUPPORTED: return "unsupported configuration for the sm_100a kernels (e.g. K > 32 tags)";
+    case NER_ERR_UNSUPPORTED: return "unsupported configuration for the sm_90a kernels (e.g. K > 32 tags)";
     case NER_ERR_WORKSPACE: return "workspace missing or too small";
     case NER_ERR_NO_DRIVER: return "CUDA driver entry point cuTensorMapEncodeTiled unavailable";
     default: break;

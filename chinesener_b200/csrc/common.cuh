@@ -1,4 +1,4 @@
-// Shared device/host helpers for the ner_b200 kernels (sm_100a only).
+// Shared device/host helpers for the ner_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -7,6 +7,26 @@
 #include "../../include/ner_b200.h"
 
 #define NER_MAX_TAGS 32
+
+// SMs of the current device (132 on an H100 SXM, 114 on an H100 PCIe): grid caps, small-batch / big-batch thresholds and
+// the scratch sized by them are in units of it.  Queried once per device ordinal.
+static inline int ner_num_sms() {
+  static int cache[64];
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) {
+    (void)cudaGetLastError();
+    return 132;
+  }
+  if (cache[dev] == 0) {
+    int n = 0;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
+      (void)cudaGetLastError();
+      n = 132;
+    }
+    cache[dev] = n;
+  }
+  return cache[dev];
+}
 
 // Map the last CUDA launch error onto the C-ABI status space.
 static inline int ner_launch_status() {
@@ -66,37 +86,22 @@ __device__ __forceinline__ float fast_lg2(float x) {
   return y;
 }
 
-// sm_100 packed fp32 pairs (FFMA2 / FMUL2: two FMAs per issued instruction; a scalar packed with
-// itself becomes the instruction's broadcast operand form, no MOV is emitted).
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pk2(float lo, float hi) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
+// fp32 pairs.  Hopper has no packed fp32 instructions, so each pair op is two scalar ops with the same
+// rounding (fma.rn / mul.rn / add.rn per lane); the kernels keep the pair form for their data layout.
+struct f32x2 {
+  float lo, hi;
+};
+__device__ __forceinline__ f32x2 pk2(float lo, float hi) { return f32x2{lo, hi}; }
 __device__ __forceinline__ void upk2(f32x2 v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
+  lo = v.lo;
+  hi = v.hi;
 }
 __device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
+  return f32x2{__fmaf_rn(a.lo, b.lo, c.lo), __fmaf_rn(a.hi, b.hi, c.hi)};
 }
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ float max3(float a, float b, float c) {
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
-}
+__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { return f32x2{__fmul_rn(a.lo, b.lo), __fmul_rn(a.hi, b.hi)}; }
+__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { return f32x2{__fadd_rn(a.lo, b.lo), __fadd_rn(a.hi, b.hi)}; }
+__device__ __forceinline__ float max3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

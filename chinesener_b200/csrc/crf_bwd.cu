@@ -1,5 +1,5 @@
 // Gradient of the CRF log-likelihood w.r.t. emission logits and the transition matrix,
-// sm_100a.  The reference obtains it by tf.gradients through the crf_log_norm while-loop
+// sm_90a.  The reference obtains it by tf.gradients through the crf_log_norm while-loop
 // (reference tools/train_utils.py:314 over tools/layer.py:122-127); here it is the closed
 // form forward-backward:
 //     d ll / d x[t][j]      = 1[y_t = j]              - P(y_t = j | x)
@@ -335,7 +335,7 @@ template <int K>
 int launch_bwd(const float* logits, const int32_t* tags, const int32_t* seq_len, const float* trans,
                const float* alpha_ws, const float* logz, const float* d_ll, float scale, float* d_logits,
                float* d_trans, int B, int L, cudaStream_t st) {
-  if (B > 148 * 64 * 2)
+  if (B > ner_num_sms() * 64 * 2)
     return launch_bwd_nt<K, 64>(logits, tags, seq_len, trans, alpha_ws, logz, d_ll, scale, d_logits, d_trans, B, L, st);
   return launch_bwd_nt<K, 32>(logits, tags, seq_len, trans, alpha_ws, logz, d_ll, scale, d_logits, d_trans, B, L, st);
 }

@@ -1,4 +1,4 @@
-// CRF log-likelihood (gold-path score minus forward-alpha log-partition) for sm_100a —
+// CRF log-likelihood (gold-path score minus forward-alpha log-partition) for sm_90a —
 // replaces tf.contrib.crf.crf_log_likelihood as called at reference tools/layer.py:122-127
 // (crf_sequence_score / crf_log_norm semantics restated in SURVEY.md Appendix A.1).
 //
@@ -339,7 +339,7 @@ int launch_fwd_nt(const float* logits, const int32_t* tags, const int32_t* seq_l
 }
 
 // NER_CRF_FWD_VARIANT=1 selects the previous configuration (8-step chunks, no register cap: 8 warps/SM)
-// so both can be timed by scripts/bench_kernels.py; profiles/README.md records the sweep behind the default.
+// so both can be timed by scripts/bench_kernels.py.
 int fwd_variant() {
   const char* e = getenv("NER_CRF_FWD_VARIANT");   // tuning / test hook, read per call
   return e ? atoi(e) : 0;
@@ -349,7 +349,7 @@ template <int K>
 int launch_fwd(const float* logits, const int32_t* tags, const int32_t* seq_len, const float* trans,
                float* ll, float* logz, float* alpha_ws, int B, int L, int flags, cudaStream_t st) {
   constexpr bool ER = (K <= 10);
-  if (B > 148 * 64 * 2) {
+  if (B > ner_num_sms() * 64 * 2) {
     if (fwd_variant() == 1)
       return launch_fwd_nt<K, 64, T_CHUNK, ER>(logits, tags, seq_len, trans, ll, logz, alpha_ws, B, L, flags, st);
     // 4-step chunks (30 KB smem / CTA) and <= 170 registers: 6 CTAs = 12 warps per SM

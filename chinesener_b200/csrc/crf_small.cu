@@ -1,4 +1,4 @@
-// Latency-oriented CRF kernels for small batches (B below a few thousand sequences), sm_100a.
+// Latency-oriented CRF kernels for small batches (B below a few thousand sequences), sm_90a.
 //
 // The thread-per-sequence kernels (crf_viterbi.cu / crf_loglik.cu) are built for HBM throughput at
 // very large B; at the model's real batch (B = 64) they leave one warp walking a 128-step

@@ -1,4 +1,4 @@
-// CRF Viterbi decode for sm_100a — replaces tf.contrib.crf.crf_decode as called at
+// CRF Viterbi decode for sm_90a — replaces tf.contrib.crf.crf_decode as called at
 // reference tools/layer.py:140-142 (semantics restated in SURVEY.md Appendix A.1).
 //
 // One thread per sequence, K-wide max-plus state in registers, transition matrix in
@@ -407,14 +407,11 @@ __device__ __forceinline__ void sel_all(F& f) {
 // Pipe-balanced variant (K <= 16, L*K % 4 == 0): same one-thread-per-sequence decomposition, four changes.
 //  (1) The per-(i,j) work of the argmax is split over BOTH arithmetic pipes.  The kernels above spend, per pair, one
 //      FADD2 half on the fma pipe and FSETP + FSEL + SEL on the alu pipe: 277 alu vs 60 fma instructions per step at
-//      K = 10.  Here the max over i is a tree of 3-input FMNMX (K/2 alu instructions per tag), and the arg is the
+//      K = 10.  Here the max over i is a tree of max3 (two FMNMX each on sm_90a), and the arg is the
 //      FIRST i whose value equals the max: one FSETP.EQ (alu) and one predicated IMAD of a pre-shifted immediate (fma
 //      pipe) per pair, walking i downwards so the lowest index is the one that sticks.  That is the reference's strict
 //      '>' scan for every non-NaN input (+0 / -0 compare equal in both formulations; the running score may differ in
-//      the sign of a zero, never in value).  Per step at K = 10: ~150 alu + ~150 fma instructions (was 277 + 60).
-//      scripts/ubench/vit_core.cu times this core without memory: 390 cycles per warp-step at 2 warps per scheduler
-//      (465 for the strict '>' scan); FSET + FFMA, sign(v - max) + SHF and predicated-FFMA variants measure the same or
-//      worse, in the model and in this kernel.
+//      the sign of a zero, never in value).
 //  (2) Emission logits arrive by TMA: one cp.async.bulk.tensor per chunk of T steps per warp (box = 32 rows x
 //      (T*K + pad) floats of the [B, L*K] view; the pad keeps the row pitch an odd number of 16-byte units so the
 //      LDS.128 reads are conflict free; out-of-range columns/rows are zero filled) instead of ~18 instructions per
@@ -808,7 +805,7 @@ int launch_viterbi(const float* logits, const int32_t* seq_len, const float* tra
                    int32_t* tags_out, float* best_score, int B, int L, cudaStream_t st) {
   // Large batches: 128 sequences per CTA when the backpointer slab fits; small batches
   // spread over more SMs with 32-sequence CTAs.
-  const bool big = B > 148 * 32 * 2;
+  const bool big = B > ner_num_sms() * 32 * 2;
   if constexpr (K <= 16) {
     if (big && vit_variant() == 0) {   // default: the pipe-balanced TMA kernel (falls through when L*K % 4 != 0 or L is too long)
       const int rc = launch_viterbi_tma<K, 32, 2, 2, 8>(logits, seq_len, trans, tags_out, best_score, B, L, st);

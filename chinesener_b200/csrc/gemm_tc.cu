@@ -1,4 +1,4 @@
-// Dense layers of the encoder on the 5th-gen tensor cores (tcgen05 + TMEM + TMA), sm_100a.
+// Dense layers of the encoder on the Hopper tensor cores (wgmma + TMA + mbarrier), sm_90a.
 //
 //   out[M,N] = epilogue( A[M,K] · Wt[N,K]^T + bias[N] )       A, Wt bf16 (K-major), fp32 accumulate
 //
@@ -6,24 +6,21 @@
 // reference tools/layer.py:68-77 (bert_base.bert.modeling) and model/bert_bilstm_crf.py:26,
 // and the input projection half of the LSTMCell matmul (tools/layer.py:16,35).
 //
-// Kernel shape (persistent, warp-specialised, 320 threads = 10 warps, 1 CTA/SM):
-//   warp 0    TMA producer : cp.async.bulk.tensor 2-D loads of a 128x64 A box and a B box per
-//                            k-block into a STAGES-deep smem ring (SWIZZLE_128B), mbarrier tx
-//   warp 1    MMA issuer   : one thread issues tcgen05.mma.kind::f16 x4 per k-block;
-//                            tcgen05.commit releases smem slots / publishes the accumulator
-//   warps 2-9 epilogue     : tcgen05.ld 32x32b (TMEM lane quarter = warp%4, two warps per quarter
-//                            on alternating 128-byte column groups) -> bias / GELU / residual ->
-//                            swizzled smem staging tile -> cp.async.bulk.tensor (TMA) store
-// Two TMEM accumulator stages (2*BN columns) let the epilogue of tile i overlap the main loop
-// of tile i+1.
+// Kernel shape (persistent, warp-specialised, 384 threads = 3 warpgroups, 1 CTA/SM):
+//   warpgroup 0    TMA producer : one elected thread issues cp.async.bulk.tensor 2-D loads of a 128x64 A box and a
+//                                 BN x 64 B box per k-block into a STAGES-deep smem ring (SWIZZLE_128B), mbarrier tx;
+//                                 it gives its registers to the MMA warpgroups (setmaxnreg)
+//   warpgroups 1-2 MMA + epilogue: warpgroup w owns rows 64(w-1) .. 64(w-1)+63 of the tile; per k-block four
+//                                 wgmma.m64nBNk16 from SWIZZLE_128B descriptors, fp32 accumulator in registers, one
+//                                 wgmma group kept in flight before the previous smem slot is released; then bias /
+//                                 GELU / residual straight from the accumulator fragment to global memory.
+// While the MMA warpgroups run the epilogue of tile i the producer already fills the ring for tile i+1.
 //
 // Two variants:
-//   gemm_bf16_tc_kernel<BN>    cta_group::1, 128 x BN tile per CTA (BN = 64/128/256)
-//   gemm_bf16_tc2_kernel<BN>   cta_group::2: a CTA PAIR (cluster of 2, one per SM of a TPC)
-//                              computes a 256 x BN tile with M=256 MMAs issued by CTA 0; each CTA
-//                              stages its own 128 A rows and HALF of the B tile, so the L2->smem
-//                              bytes per FLOP drop by 1.5x vs the 128x256 single-CTA tile (the
-//                              single-CTA kernel is L2-feed-bound at ~9-10 TB/s, see DESIGN.md).
+//   gemm_bf16_tc_kernel<BN, SK, 1>   128 x BN tile per CTA (BN = 64/128/192/256), optionally stream-K
+//   gemm_bf16_tc_kernel<BN, 0, 2>    a cluster of 2 CTAs computes a 256 x BN tile: each CTA stages its own 128 A rows
+//                                    and loads HALF of the B tile with TMA multicast into both CTAs, so the L2->smem
+//                                    bytes per FLOP drop by 1.5x vs the 128 x BN single-CTA tile.
 #include <stdlib.h>
 
 #include <mutex>
@@ -36,33 +33,21 @@ using namespace tc;
 
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 bf16 = 128 B = one swizzle-128B row
-constexpr int UMMA_K = 16;
-constexpr int NUM_EPI_WARPS = 8;
-// stream-K fixed charge in k-block times: parking + re-reading a 128 KB partial accumulator and the
-// exposed finisher epilogue cost ~6 us (trip 16/17: SK loses on the encoder's forward shapes at M ~ 3150,
-// 24.9 vs 18.8 us for 3150x2304x768); it pays when tiles << SMs and K is long (weight gradients, K = tokens).
+constexpr int MMA_K = 16;
+constexpr int NUM_MMA_WG = 2;
+// stream-K fixed charge in k-block times: parking + re-reading a 128 x 256 fp32 partial accumulator and the
+// exposed finisher epilogue; it pays when tiles << SMs and K is long (weight gradients, K = tokens).
 constexpr float kSkFixupCost = 10.0f;
-constexpr int NUM_THREADS = 64 + 32 * NUM_EPI_WARPS;
-
-constexpr int tmem_cols_for(int n) { return n <= 32 ? 32 : n <= 64 ? 64 : n <= 128 ? 128 : n <= 256 ? 256 : 512; }
+constexpr int NUM_THREADS = 128 * (1 + NUM_MMA_WG);
 
 template <int BN>
 struct Cfg {
-  static constexpr int STAGES = (BN == 256) ? 4 : (BN == 192) ? 4 : ((BN == 128) ? 6 : 8);
+  // 227 KB of shared memory per block: 4 x 48 KB (BN 256), 5 x 40 KB (192), 6 x 32 KB (128), 8 x 24 KB (64)
+  static constexpr int STAGES = (BN == 256) ? 4 : (BN == 192) ? 5 : ((BN == 128) ? 6 : 8);
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
-  static constexpr int TMEM_COLS = tmem_cols_for(2 * BN);
-  // ring + 8 x 4 KB epilogue staging + barriers + bias; the dynamic smem base is 1024-aligned (checked in-kernel)
-  static constexpr size_t SMEM = (size_t)STAGES * (A_BYTES + B_BYTES) + NUM_EPI_WARPS * 4096 + 256 + 2 * BN * 4;
-};
-
-template <int BN>
-struct Cfg2 {  // per CTA of the pair
-  static constexpr int STAGES = 6;
-  static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = (BN / 2) * BK * 2;
-  static constexpr int TMEM_COLS = tmem_cols_for(2 * BN);
-  static constexpr size_t SMEM = (size_t)STAGES * (A_BYTES + B_BYTES) + NUM_EPI_WARPS * 4096 + 256 + 2 * BN * 4;
+  // ring + barriers; the dynamic smem base is 1024-aligned (checked in-kernel)
+  static constexpr size_t SMEM = (size_t)STAGES * (A_BYTES + B_BYTES) + 256;
 };
 
 struct EpiArgs {
@@ -86,78 +71,36 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
-// Fused epilogue math on one 32-column chunk of one accumulator row (values in registers).
-// `sbias` = this chunk's 32 bias values in shared memory (broadcast LDS.128), staged once per tile.
-__device__ __forceinline__ void epilogue_math(float (&v)[32], const uint32_t (&r)[32], const EpiArgs& ep,
-                                              const float* sbias, int row, int col0, int M, int N) {
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-  {
-    const float4* b4 = reinterpret_cast<const float4*>(sbias);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float4 b = b4[i];
-      v[4 * i + 0] += b.x;
-      v[4 * i + 1] += b.y;
-      v[4 * i + 2] += b.z;
-      v[4 * i + 3] += b.w;
-    }
-  }
-  if (ep.mode == NER_EPI_RES_F32 || ep.mode == NER_EPI_RES_RELU_F32) {
-    if (row < M && col0 < N) {
-      const float4* r4 = reinterpret_cast<const float4*>(ep.residual + (size_t)row * N + col0);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float4 b = __ldg(r4 + i);
-        v[4 * i + 0] += b.x;
-        v[4 * i + 1] += b.y;
-        v[4 * i + 2] += b.z;
-        v[4 * i + 3] += b.w;
-      }
-    }
-    if (ep.mode == NER_EPI_RES_RELU_F32) {
-#pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.f);
-    }
-  } else if (ep.mode == NER_EPI_GELU_TANH_BF16) {
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = gelu_tanh(v[i]);
-  } else if (ep.mode == NER_EPI_GELU_ERF_BF16) {
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = gelu_erf(v[i]);
-  } else if (ep.mode == NER_EPI_RELU_BF16) {
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.f);
-  }
-}
-
 // ---------------------------------------------------------------------------------------------
 // Stream-K work split.  With SK the M x N x K iteration space is cut into tiles * num_kb k-block
 // units and CTA c owns the contiguous unit range [c*U/G, (c+1)*U/G): every SM gets the same number
-// of k-blocks whatever tiles/SMs is (the packed M of an MSRA batch gives 1.5 / 2.03 / 0.5 waves on
-// the encoder's GEMMs, i.e. 25-50 % idle SMs with whole-tile scheduling).  A CTA's range is
+// of k-blocks whatever tiles/SMs is (the packed M of an MSRA batch gives fractional waves on
+// the encoder's GEMMs, i.e. idle SMs with whole-tile scheduling).  A CTA's range is
 //   [tail piece of a tile]  [whole tiles]  [head piece of a tile]
 // The CTA holding a tile's HEAD (kb0 == 0) finishes that tile: it adds the fp32 partial sums that
 // the CTAs holding the later k-blocks parked in their workspace slot and runs the normal epilogue.
 // A tail piece is always the FIRST thing its CTA does and the head piece the LAST, so a finisher
 // never waits in practice and no wait cycle can form (all CTAs are co-resident: grid <= #SMs).
 struct SkArgs {
-  float4* ws;   // [grid][BN/32 chunks][8][128 rows] float4: slot c = partial accumulator of CTA c's first segment
+  float4* ws;   // [grid][128 x 256 floats]: slot c = partial accumulator of CTA c's first segment
   int* flags;   // [grid] 0 / 1 = slot c published; reset to 0 by the finisher (all zero between launches)
 };
 
+// Work iterator over tiles (whole-tile round robin) or stream-K unit ranges; `id` / `count` = this CTA (or CTA
+// pair) and the number of them.
 struct SegIter {
   int num_kb, num_tiles, tile, stride;
   long long u, u1;
   bool sk;
-  __device__ SegIter(bool sk_, int num_tiles_, int num_kb_) : num_kb(num_kb_), num_tiles(num_tiles_), sk(sk_) {
+  __device__ SegIter(bool sk_, int num_tiles_, int num_kb_, int id, int count)
+      : num_kb(num_kb_), num_tiles(num_tiles_), sk(sk_) {
     if (sk) {
       const long long U = (long long)num_tiles * num_kb;
-      u = (long long)blockIdx.x * U / gridDim.x;
-      u1 = (long long)(blockIdx.x + 1) * U / gridDim.x;
+      u = (long long)id * U / count;
+      u1 = (long long)(id + 1) * U / count;
     } else {
-      tile = blockIdx.x;
-      stride = gridDim.x;
+      tile = id;
+      stride = count;
     }
   }
   __device__ bool next(int& t, int& kb0, int& kb1) {
@@ -188,302 +131,262 @@ __device__ __forceinline__ void st_release_gpu(int* p, int v) {
   asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
-__device__ __forceinline__ void epi_bar_sync() {  // named barrier 1 over the 8 epilogue warps only
-  asm volatile("bar.sync 1, %0;" ::"n"(32 * NUM_EPI_WARPS) : "memory");
+__device__ __forceinline__ void mma_bar_sync() {  // named barrier 1 over the MMA warpgroups only
+  asm volatile("bar.sync 1, %0;" ::"n"(128 * NUM_MMA_WG) : "memory");
 }
 
-// Stage bias[n0 .. n0+BN) of the coming tile into smem (called by all epilogue threads BEFORE they
-// wait for the accumulator, so the global-load latency hides behind the main loop).
+// Shared-memory ring of one CTA: STAGES slots of {A tile, B tile}, a `full` barrier per slot (TMA transaction
+// bytes) and an `empty` barrier per slot (one arrive per MMA warp of every CTA that reads the slot's bytes).
 template <int BN>
-__device__ __forceinline__ void epilogue_stage_bias(float* sbias, const EpiArgs& ep, int n0, int N) {
-  const int t = (int)threadIdx.x - 64;  // 0 .. 255
-  for (int i = t; i < BN; i += 32 * NUM_EPI_WARPS) {
-    const int col = n0 + i;
-    sbias[i] = (ep.bias != nullptr && col < N) ? __ldg(ep.bias + col) : 0.f;
+struct Ring {
+  uint8_t* a;
+  uint8_t* b;
+  uint64_t* full;
+  uint64_t* empty;
+  __device__ Ring(uint8_t* smem) {
+    using C = Cfg<BN>;
+    a = smem;
+    b = smem + C::STAGES * C::A_BYTES;
+    full = reinterpret_cast<uint64_t*>(smem + C::STAGES * (C::A_BYTES + C::B_BYTES));
+    empty = full + C::STAGES;
   }
-  epi_bar_sync();
+};
+
+struct RingPos {
+  int stage = 0;
+  uint32_t phase = 0;
+  template <int STAGES>
+  __device__ __forceinline__ void advance() {
+    if (++stage == STAGES) {
+      stage = 0;
+      phase ^= 1u;
+    }
+  }
+};
+
+// MMA side of k-blocks [kb0, kb1): this warpgroup's 64 x BN slice of the tile into `acc`.  A and B descriptors for a
+// K-step of 16 are produced by `desc_a(addr, k)` / `desc_b(addr, k)`; TA / TB = operand is MN-major.  The smem slot of
+// k-block i is released once the wgmma group of k-block i+1 is issued and group i has retired.
+template <int BN, int STAGES, int CL, int TA, int TB, typename DA, typename DB>
+__device__ __forceinline__ void mma_kblocks(float (&acc)[BN / 2], const Ring<BN>& ring, RingPos& pos, int kb0, int kb1,
+                                            uint32_t a_off, DA desc_a, DB desc_b, const uint32_t (&empty_peer)[STAGES]) {
+  const int lane = threadIdx.x & 31;
+  int prev = -1;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(&ring.full[pos.stage], pos.phase);
+    const uint32_t a_addr = smem_u32(ring.a + pos.stage * (BM * BK * 2)) + a_off;
+    const uint32_t b_addr = smem_u32(ring.b + pos.stage * (BN * BK * 2));
+    reg_fence(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / MMA_K; ++k)
+      wgmma_bf16<BN, TA, TB>(acc, desc_a(a_addr, k), desc_b(b_addr, k), (kb > kb0 || k > 0) ? 1u : 0u);
+    wgmma_commit();
+    reg_fence(acc);
+    if (prev >= 0) {
+      wgmma_wait<1>();
+      reg_fence(acc);
+      if (lane == 0) {
+        mbar_arrive(&ring.empty[prev]);
+        if constexpr (CL == 2) mbar_arrive_cluster(empty_peer[prev]);
+      }
+    }
+    prev = pos.stage;
+    pos.template advance<STAGES>();
+  }
+  wgmma_wait<0>();
+  reg_fence(acc);
+  if (lane == 0 && prev >= 0) {
+    mbar_arrive(&ring.empty[prev]);
+    if constexpr (CL == 2) mbar_arrive_cluster(empty_peer[prev]);
+  }
 }
 
-// Epilogue of one 128 x BN accumulator.  Each epilogue warp owns a TMEM lane quarter (32 rows) and
-// every other 128-byte column group (64 bf16 or 32 fp32 columns).  Per group: tcgen05.ld -> fused
-// math -> the warp's 32 x 128 B staging tile in shared memory (SWIZZLE_128B: chunk ^ (row & 7),
-// conflict-free STS.128) -> ONE cp.async.bulk.tensor store by lane 0.  The store writes full
-// 128-byte lines and clips rows >= M / columns >= N by itself; direct per-thread stores wrote
-// 16-byte fragments of 32 different lines per instruction and were L2-transaction-bound.
-// Finisher side of a split tile: add the parked partial sums of CTAs [c_first, c_first + n_part) to
-// one 32-column chunk held in registers (same (chunk, i, row) layout the contributors wrote).
+// Fused epilogue of this thread's accumulator fragment (rows r, r + 8; column pairs 8 j + 2 (lane % 4)), written straight
+// to global memory.  `row_w` = first row of this warp's 16-row slice.
 template <int BN>
-__device__ __forceinline__ void add_partials(uint32_t (&r)[32], const float4* ws, int c_first, int n_part, int chunk,
-                                             int row_in_tile) {
-  constexpr size_t SLOT = (size_t)(BN / 32) * 8 * 128;
-  for (int c = 0; c < n_part; ++c) {
-    const float4* p = ws + (size_t)(c_first + c) * SLOT + (size_t)chunk * 8 * 128 + row_in_tile;
+__device__ __forceinline__ void epilogue_regs(const float (&acc)[BN / 2], const EpiArgs& ep, int row_w, int n0, int M,
+                                              int N) {
+  if (ep.mode == NER_EPI_DIAG_DISCARD) return;  // diagnostic: drain the accumulator, store nothing
+  const int lane = threadIdx.x & 31;
+  const bool f32 = ep.mode == NER_EPI_F32 || ep.mode == NER_EPI_RES_F32 || ep.mode == NER_EPI_RES_RELU_F32;
+  const bool res = ep.mode == NER_EPI_RES_F32 || ep.mode == NER_EPI_RES_RELU_F32;
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float4 v = __ldcg(p + i * 128);
-      r[4 * i + 0] = __float_as_uint(__uint_as_float(r[4 * i + 0]) + v.x);
-      r[4 * i + 1] = __float_as_uint(__uint_as_float(r[4 * i + 1]) + v.y);
-      r[4 * i + 2] = __float_as_uint(__uint_as_float(r[4 * i + 2]) + v.z);
-      r[4 * i + 3] = __float_as_uint(__uint_as_float(r[4 * i + 3]) + v.w);
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = n0 + 8 * j + 2 * (lane & 3);
+    if (col >= N) continue;
+    float2 b = make_float2(0.f, 0.f);
+    if (ep.bias != nullptr) b = __ldg(reinterpret_cast<const float2*>(ep.bias + col));
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = row_w + (lane >> 2) + 8 * h;
+      if (row >= M) continue;
+      float v0 = acc[4 * j + 2 * h] + b.x, v1 = acc[4 * j + 2 * h + 1] + b.y;
+      const size_t off = (size_t)row * N + col;
+      if (res) {
+        const float2 r = *reinterpret_cast<const float2*>(ep.residual + off);
+        v0 += r.x;
+        v1 += r.y;
+        if (ep.mode == NER_EPI_RES_RELU_F32) {
+          v0 = fmaxf(v0, 0.f);
+          v1 = fmaxf(v1, 0.f);
+        }
+      } else if (ep.mode == NER_EPI_GELU_TANH_BF16) {
+        v0 = gelu_tanh(v0);
+        v1 = gelu_tanh(v1);
+      } else if (ep.mode == NER_EPI_GELU_ERF_BF16) {
+        v0 = gelu_erf(v0);
+        v1 = gelu_erf(v1);
+      } else if (ep.mode == NER_EPI_RELU_BF16) {
+        v0 = fmaxf(v0, 0.f);
+        v1 = fmaxf(v1, 0.f);
+      }
+      if (f32)
+        *reinterpret_cast<float2*>(static_cast<float*>(ep.out) + off) = make_float2(v0, v1);
+      else
+        *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(ep.out) + off) = pack_bf16x2(v0, v1);
     }
   }
 }
 
-// Contributor side: park the raw fp32 accumulator of this CTA's (partial) first segment in its slot.
-template <int BN>
-__device__ __forceinline__ void park_partial(uint32_t tmem_acc, int warp, int lane, float4* slot) {
-  const int q = warp & 3, half = (warp - 2) >> 2;
-  const uint32_t tbase = tmem_acc + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-  for (int ch = half; ch < BN / 32; ch += 2) {
-    uint32_t ra[32];
-    tmem_ld_32x32(tbase + (uint32_t)(ch * 32), ra);
-    tmem_ld_wait();
-    float4* p = slot + (size_t)ch * 8 * 128 + q * 32 + lane;
-#pragma unroll
-    for (int i = 0; i < 8; ++i)
-      __stcg(p + i * 128, make_float4(__uint_as_float(ra[4 * i]), __uint_as_float(ra[4 * i + 1]),
-                                      __uint_as_float(ra[4 * i + 2]), __uint_as_float(ra[4 * i + 3])));
+// Barrier setup shared by both kernels: full[s] count 1 (+ tx), empty[s] one arrive per MMA warp of each CTA of the
+// cluster that reads slot s.
+template <int BN, int CL>
+__device__ __forceinline__ void init_ring(const Ring<BN>& ring) {
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < Cfg<BN>::STAGES; ++s) {
+      mbar_init(&ring.full[s], 1);
+      mbar_init(&ring.empty[s], 4 * NUM_MMA_WG * CL);
+    }
+    fence_barrier_init();
   }
 }
 
-template <int BN, bool OUT_F32>
-__device__ __forceinline__ void epilogue_tile(uint32_t tmem_acc, int warp, int lane, const EpiArgs& ep,
-                                              const CUtensorMap* tma_c, uint8_t* stage, const float* sbias, int row0,
-                                              int n0, int M, int N, const float4* ws = nullptr, int c_first = 0,
-                                              int n_part = 0) {
-  constexpr int GC = OUT_F32 ? 32 : 64;  // columns per 128-byte group
-  constexpr int NG = BN / GC;            // groups per tile
-  const int q = warp & 3;                // TMEM lane quarter this warp may access
-  const int half = (warp - 2) >> 2;      // 0: even groups, 1: odd groups
-  const int row = row0 + q * 32 + lane;
-  const uint32_t tbase = tmem_acc + ((uint32_t)(q * 32) << 16);
-  uint8_t* my = stage + lane * 128;
-  const int sw = lane & 7;
-#pragma unroll 1
-  for (int g = half; g < NG; g += 2) {
-    const int col0 = n0 + g * GC;
-    uint32_t ra[32];
-    float v[32];
-    uint4 pk[8];
-    tmem_ld_32x32(tbase + (uint32_t)(g * GC), ra);
-    tmem_ld_wait();
-    if (n_part > 0) add_partials<BN>(ra, ws, c_first, n_part, g * GC / 32, q * 32 + lane);
-    epilogue_math(v, ra, ep, sbias + g * GC, row, col0, M, N);
-    if constexpr (OUT_F32) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-        pk[i] = make_uint4(__float_as_uint(v[4 * i]), __float_as_uint(v[4 * i + 1]), __float_as_uint(v[4 * i + 2]),
-                           __float_as_uint(v[4 * i + 3]));
-    } else {
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        pk[i] = make_uint4(pack_bf16x2(v[8 * i + 0], v[8 * i + 1]), pack_bf16x2(v[8 * i + 2], v[8 * i + 3]),
-                           pack_bf16x2(v[8 * i + 4], v[8 * i + 5]), pack_bf16x2(v[8 * i + 6], v[8 * i + 7]));
-      tmem_ld_32x32(tbase + (uint32_t)(g * GC + 32), ra);
-      tmem_ld_wait();
-      if (n_part > 0) add_partials<BN>(ra, ws, c_first, n_part, g * GC / 32 + 1, q * 32 + lane);
-      epilogue_math(v, ra, ep, sbias + g * GC + 32, row, col0 + 32, M, N);
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        pk[4 + i] = make_uint4(pack_bf16x2(v[8 * i + 0], v[8 * i + 1]), pack_bf16x2(v[8 * i + 2], v[8 * i + 3]),
-                               pack_bf16x2(v[8 * i + 4], v[8 * i + 5]), pack_bf16x2(v[8 * i + 6], v[8 * i + 7]));
-    }
-    if (ep.mode == NER_EPI_DIAG_DISCARD) continue;  // diagnostic: drain TMEM, store nothing
-    // the previous bulk store of this warp must have finished reading the staging tile
-    if (lane == 0) tma_store_wait_read<0>();
-    __syncwarp();
-#pragma unroll
-    for (int i = 0; i < 8; ++i) *reinterpret_cast<uint4*>(my + ((i ^ sw) << 4)) = pk[i];
-    fence_proxy_async();
-    __syncwarp();
-    if (lane == 0 && col0 < N && row0 + q * 32 < M) {
-      tma_store_2d(tma_c, stage, col0, row0 + q * 32);
-      tma_store_commit();
-    }
-  }
-}
-
-// ===================================================================== cta_group::1
-template <int BN, bool SK>
+// ===================================================================== main kernel
+template <int BN, bool SK, int CL>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_bf16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
-                    const __grid_constant__ CUtensorMap tma_c, EpiArgs ep, int M, int N, int K, SkArgs skargs) {
+gemm_bf16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, EpiArgs ep,
+                    int M, int N, int K, SkArgs skargs) {
   using C = Cfg<BN>;
   constexpr int STAGES = C::STAGES;
   nerdev::pdl_launch_dependents();   // the next kernel of the stream may start its prologue while this one runs
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw;  // SWIZZLE_128B tiles need 1024-B alignment
-  if ((smem_u32(smem_raw) & 1023u) != 0u) __trap();
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + STAGES * C::A_BYTES;
-  uint8_t* epi_stage = smem + STAGES * (C::A_BYTES + C::B_BYTES);  // [NUM_EPI_WARPS][32 rows][128 B], 1024-aligned
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_stage + NUM_EPI_WARPS * 4096);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  float* sbias = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full_bar) + 256);  // [2][BN]
+  if ((smem_u32(smem_raw) & 1023u) != 0u) __trap();  // SWIZZLE_128B tiles need 1024-B alignment
+  const Ring<BN> ring(smem_raw);
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
+  const uint32_t rank = CL == 2 ? cluster_ctarank() : 0u;
+  const int id = CL == 2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
+  const int count = CL == 2 ? (int)(gridDim.x >> 1) : (int)gridDim.x;
 
-  const int num_m = (M + BM - 1) / BM;
+  const int num_m = (M + CL * BM - 1) / (CL * BM);
   const int num_n = (N + BN - 1) / BN;
   const int num_tiles = num_m * num_n;
   const int num_kb = (K + BK - 1) / BK;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tma_a);
     tma_prefetch_desc(&tma_b);
-    tma_prefetch_desc(&tma_c);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full[s], 1);
-      mbar_init(&tmem_empty[s], NUM_EPI_WARPS);  // one arrive per epilogue warp
-    }
-    fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<C::TMEM_COLS>(tmem_ptr);
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  // barriers, TMEM and descriptor prefetch are set up: everything below touches global memory and must
+  init_ring<BN, CL>(ring);
+  if constexpr (CL == 2) cluster_sync_all();  // barrier inits visible cluster-wide before any multicast / remote arrive
+  else __syncthreads();
+  // barriers and descriptor prefetch are set up: everything below touches global memory and must
   // wait for the previous kernel of the stream (no-op unless launched with the PDL attribute)
   nerdev::pdl_wait();
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      SegIter it(SK, num_tiles, num_kb);
+    setmaxnreg_dec<40>();
+    if (threadIdx.x < 32 && elect_one()) {
+      RingPos pos;
+      SegIter it(SK, num_tiles, num_kb, id, count);
       int tile, kb0, kb1;
       while (it.next(tile, kb0, kb1)) {
         const int m_blk = tile / num_n, n_blk = tile - m_blk * num_n;
+        const int row_a = (m_blk * CL + (int)rank) * BM;
         for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          mbar_arrive_expect_tx(&full_bar[stage], C::A_BYTES + C::B_BYTES);
-          tma_load_2d(smem_a + stage * C::A_BYTES, &tma_a, &full_bar[stage], kb * BK, m_blk * BM);
-          tma_load_2d(smem_b + stage * C::B_BYTES, &tma_b, &full_bar[stage], kb * BK, n_blk * BN);
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (single thread) =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      SegIter it(SK, num_tiles, num_kb);
-      int tile, kb0, kb1;
-      while (it.next(tile, kb0, kb1)) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1u);
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tcgen05_fence_after();
-          const uint32_t a_addr = smem_u32(smem_a + stage * C::A_BYTES);
-          const uint32_t b_addr = smem_u32(smem_b + stage * C::B_BYTES);
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            const uint64_t da = make_smem_desc_sw128(a_addr + k * UMMA_K * 2);
-            const uint64_t db = make_smem_desc_sw128(b_addr + k * UMMA_K * 2);
-            umma_f16(d_tmem, da, db, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);  // smem slot free once these MMAs retire
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-        umma_commit(&tmem_full[acc]);  // accumulator complete
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1u;
+          mbar_wait(&ring.empty[pos.stage], pos.phase ^ 1u);
+          mbar_arrive_expect_tx(&ring.full[pos.stage], C::A_BYTES + C::B_BYTES);
+          tma_load_2d(ring.a + pos.stage * C::A_BYTES, &tma_a, &ring.full[pos.stage], kb * BK, row_a);
+          if constexpr (CL == 2)
+            tma_load_2d_mc(ring.b + pos.stage * C::B_BYTES + rank * (C::B_BYTES / 2), &tma_b, &ring.full[pos.stage],
+                           kb * BK, n_blk * BN + (int)rank * (BN / 2), (uint16_t)0x3);
+          else
+            tma_load_2d(ring.b + pos.stage * C::B_BYTES, &tma_b, &ring.full[pos.stage], kb * BK, n_blk * BN);
+          pos.advance<STAGES>();
         }
       }
     }
   } else {
-    // ===================== epilogue warps (2..9) =====================
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    constexpr size_t SLOT = (size_t)(BN / 32) * 8 * 128;
-    SegIter it(SK, num_tiles, num_kb);
+    // ===================== MMA + epilogue warpgroups =====================
+    setmaxnreg_inc<232>();
+    const int mw = wg - 1;                      // 64-row slice of the tile
+    const int ctid = threadIdx.x - 128;         // 0 .. 255
+    const int row_in_tile = mw * 64 + ((threadIdx.x >> 5) & 3) * 16;
+    uint32_t empty_peer[STAGES];
+#pragma unroll
+    for (int s = 0; s < STAGES; ++s) empty_peer[s] = CL == 2 ? mapa_u32(smem_u32(&ring.empty[s]), rank ^ 1u) : 0u;
+    auto da = [](uint32_t addr, int k) { return make_wgmma_desc_sw128(addr + k * MMA_K * 2); };
+    constexpr size_t SLOT = (size_t)BN * BM / 2;   // float2 per CTA slot
+    float2* ws = reinterpret_cast<float2*>(skargs.ws);
+    RingPos pos;
+    SegIter it(SK, num_tiles, num_kb, id, count);
     int tile, kb0, kb1;
+    float acc[BN / 2];
     while (it.next(tile, kb0, kb1)) {
       const int m_blk = tile / num_n, n_blk = tile - m_blk * num_n;
-      const bool contributor = SK && kb0 > 0;
-      if (!contributor) epilogue_stage_bias<BN>(sbias + acc * BN, ep, n_blk * BN, N);
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tcgen05_fence_after();
-      if (contributor) {
-        park_partial<BN>(tmem_base + (uint32_t)(acc * BN), warp, lane, skargs.ws + (size_t)blockIdx.x * SLOT);
+      const int row0 = (m_blk * CL + (int)rank) * BM;
+      mma_kblocks<BN, STAGES, CL, 0, 0>(acc, ring, pos, kb0, kb1, (uint32_t)(mw * 64 * BK * 2), da, da, empty_peer);
+      if (SK && kb0 > 0) {
+        // contributor: park the raw partial accumulator of this CTA's first segment in its slot
+        float2* p = ws + (size_t)blockIdx.x * SLOT + ctid;
+#pragma unroll
+        for (int i = 0; i < BN / 4; ++i) __stcg(p + (size_t)i * 256, make_float2(acc[2 * i], acc[2 * i + 1]));
         __threadfence();
-        epi_bar_sync();
-        if (warp == 2 && lane == 0) st_release_gpu(skargs.flags + blockIdx.x, 1);
-      } else {
-        int c_first = 0, n_part = 0;
-        if (SK && kb1 < num_kb) {
-          // finisher: the following CTAs whose ranges start inside this tile hold its later k-blocks
-          const long long U = (long long)num_tiles * num_kb, tile_end = (long long)(tile + 1) * num_kb;
-          c_first = blockIdx.x + 1;
-          for (int c = c_first; c < (int)gridDim.x; ++c) {
-            const long long c0 = (long long)c * U / gridDim.x, c1 = (long long)(c + 1) * U / gridDim.x;
-            if (c0 >= tile_end) break;
-            if (c1 > c0) ++n_part; else if (n_part == 0) ++c_first;   // (empty ranges only occur when U < grid)
-          }
-          if (warp == 2 && lane == 0) {
-            for (int c = 0; c < n_part; ++c) {
-              unsigned spins = 0;
-              while (ld_acquire_gpu(skargs.flags + c_first + c) == 0)
-                if (++spins > (1u << 28)) __trap();   // never hang the GPU on a protocol bug
-            }
-          }
-          epi_bar_sync();
-          __threadfence();
+        mma_bar_sync();
+        if (ctid == 0) st_release_gpu(skargs.flags + blockIdx.x, 1);
+        continue;
+      }
+      int c_first = 0, n_part = 0;
+      if (SK && kb1 < num_kb) {
+        // finisher: the following CTAs whose ranges start inside this tile hold its later k-blocks
+        const long long U = (long long)num_tiles * num_kb, tile_end = (long long)(tile + 1) * num_kb;
+        c_first = blockIdx.x + 1;
+        for (int c = c_first; c < (int)gridDim.x; ++c) {
+          const long long c0 = (long long)c * U / gridDim.x, c1 = (long long)(c + 1) * U / gridDim.x;
+          if (c0 >= tile_end) break;
+          if (c1 > c0) ++n_part; else if (n_part == 0) ++c_first;   // (empty ranges only occur when U < grid)
         }
-        if (ep.mode == NER_EPI_F32 || ep.mode == NER_EPI_RES_F32 || ep.mode == NER_EPI_RES_RELU_F32)
-          epilogue_tile<BN, true>(tmem_base + (uint32_t)(acc * BN), warp, lane, ep, &tma_c, epi_stage + (warp - 2) * 4096,
-                                  sbias + acc * BN, m_blk * BM, n_blk * BN, M, N, skargs.ws, c_first, n_part);
-        else
-          epilogue_tile<BN, false>(tmem_base + (uint32_t)(acc * BN), warp, lane, ep, &tma_c, epi_stage + (warp - 2) * 4096,
-                                   sbias + acc * BN, m_blk * BM, n_blk * BN, M, N, skargs.ws, c_first, n_part);
-        if (n_part > 0) {
-          epi_bar_sync();   // every epilogue thread has consumed the parked partials
-          if (warp == 2)
-            for (int c = lane; c < n_part; c += 32) skargs.flags[c_first + c] = 0;
+        if (ctid == 0) {
+          for (int c = 0; c < n_part; ++c) {
+            unsigned spins = 0;
+            while (ld_acquire_gpu(skargs.flags + c_first + c) == 0)
+              if (++spins > (1u << 28)) __trap();   // never hang the GPU on a protocol bug
+          }
+        }
+        mma_bar_sync();
+        __threadfence();
+        for (int c = 0; c < n_part; ++c) {
+          const float2* p = ws + (size_t)(c_first + c) * SLOT + ctid;
+#pragma unroll
+          for (int i = 0; i < BN / 4; ++i) {
+            const float2 v = __ldcg(p + (size_t)i * 256);
+            acc[2 * i] += v.x;
+            acc[2 * i + 1] += v.y;
+          }
         }
       }
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1u;
+      epilogue_regs<BN>(acc, ep, row0 + row_in_tile, n_blk * BN, M, N);
+      if (n_part > 0) {
+        mma_bar_sync();   // every MMA thread has consumed the parked partials
+        if (ctid < 32)
+          for (int c = ctid; c < n_part; c += 32) skargs.flags[c_first + c] = 0;
       }
     }
   }
-
-  if (warp >= 2 && lane == 0) tma_store_wait_read<0>();  // staging tiles fully read before the CTA exits
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc<C::TMEM_COLS>(tmem_base);
-  }
+  if constexpr (CL == 2) cluster_sync_all();  // no CTA leaves while its peer may still multicast into it / arrive on it
 }
 
 // ===================================================================== grouped weight gradients
@@ -491,34 +394,21 @@ gemm_bf16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
 // ONE persistent launch: the tiles of all problems form one list (128 x 256 output tiles), so the 18..72 tiles of the single
 // GEMMs (K = tokens: 50 k-blocks, a quarter to a half of the SMs idle per launch) become 216 per layer.
 // Both operands are read AS THEY LIE in memory — X [R, k_in] and dY [R, n_out] are token-major, i.e. M / N contiguous and
-// K (tokens) strided: "MN-major" operands of tcgen05.mma (instruction-descriptor bits 15/16).  A k-block is 64 tokens; the A
-// tile arrives as two and the B tile as four {64 columns x 64 tokens} TMA boxes (SWIZZLE_128B), which is the canonical MN-major
-// layout: 64-element blocks along M/N 8 KB apart (leading byte offset), 8-token groups 1 KB apart (stride byte offset); one
-// MMA (K = 16) spans two token groups, consecutive MMAs advance the start address by 2 KB.  No bf16 transposes, no padded
-// copies: TMA zero-fills the token rows past R.  Epilogue = the GEMM's fp32 accumulate-into-gradient path (RES_F32).
+// K (tokens) strided: "MN-major" (transposed) operands of wgmma.  A k-block is 64 tokens; the A tile arrives as two and the
+// B tile as four {64 columns x 64 tokens} TMA boxes (SWIZZLE_128B), which is the canonical MN-major layout: 64-element
+// blocks along M/N 8 KB apart (leading byte offset), 8-token groups 1 KB apart (stride byte offset); one MMA (K = 16) spans
+// two token groups, consecutive MMAs advance the start address by 2 KB.  Each MMA warpgroup's 64 rows of A are one box.
+// No bf16 transposes, no padded copies: TMA zero-fills the token rows past R.  Epilogue = fp32 accumulate-into-gradient (RES_F32).
 constexpr int WG_MAXP = 6;
 constexpr int WG_BN = 256;
 
 struct WgradGroup {
-  CUtensorMap a[WG_MAXP], b[WG_MAXP], c[WG_MAXP];
+  CUtensorMap a[WG_MAXP], b[WG_MAXP];
   float* dw[WG_MAXP];
   int m[WG_MAXP], n[WG_MAXP], b_col0[WG_MAXP];
   int tile_start[WG_MAXP + 1];
   int count, rows;
 };
-
-__device__ __forceinline__ uint64_t make_smem_desc_sw128_mn(uint32_t smem_addr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;   // next 64-element block along M / N
-  d |= (uint64_t)(1024 >> 4) << 32;                   // next group of 8 tokens along K
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;                             // SWIZZLE_128B
-  return d;
-}
-__host__ __device__ constexpr uint32_t make_idesc_bf16_mn(int M, int N) {
-  return make_idesc_bf16(M, N) | (1u << 15) | (1u << 16);   // a_major = b_major = MN
-}
 
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_wgrad_group_kernel(const __grid_constant__ WgradGroup grp) {
@@ -529,38 +419,15 @@ gemm_wgrad_group_kernel(const __grid_constant__ WgradGroup grp) {
   nerdev::pdl_launch_dependents();
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw;
   if ((smem_u32(smem_raw) & 1023u) != 0u) __trap();
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + STAGES * C::A_BYTES;
-  uint8_t* epi_stage = smem + STAGES * (C::A_BYTES + C::B_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_stage + NUM_EPI_WARPS * 4096);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  float* sbias = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full_bar) + 256);
+  const Ring<BN> ring(smem_raw);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
   const int num_tiles = grp.tile_start[grp.count];
   const int num_kb = (grp.rows + BK - 1) / BK;
 
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full[s], 1);
-      mbar_init(&tmem_empty[s], NUM_EPI_WARPS);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc<C::TMEM_COLS>(tmem_ptr);
-  tcgen05_fence_before();
+  init_ring<BN, 1>(ring);
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   nerdev::pdl_wait();
 
   auto locate = [&](int tile, int& p, int& m_blk, int& n_blk) {
@@ -571,242 +438,43 @@ gemm_wgrad_group_kernel(const __grid_constant__ WgradGroup grp) {
     n_blk = t - m_blk * num_n;
   };
 
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x < 32 && elect_one()) {
+      RingPos pos;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         int p, m_blk, n_blk;
         locate(tile, p, m_blk, n_blk);
         for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          mbar_arrive_expect_tx(&full_bar[stage], C::A_BYTES + C::B_BYTES);
+          mbar_wait(&ring.empty[pos.stage], pos.phase ^ 1u);
+          mbar_arrive_expect_tx(&ring.full[pos.stage], C::A_BYTES + C::B_BYTES);
 #pragma unroll
           for (int i = 0; i < BM / 64; ++i)
-            tma_load_2d(smem_a + stage * C::A_BYTES + i * BOX, &grp.a[p], &full_bar[stage], m_blk * BM + i * 64, kb * BK);
+            tma_load_2d(ring.a + pos.stage * C::A_BYTES + i * BOX, &grp.a[p], &ring.full[pos.stage], m_blk * BM + i * 64, kb * BK);
 #pragma unroll
           for (int i = 0; i < BN / 64; ++i)
-            tma_load_2d(smem_b + stage * C::B_BYTES + i * BOX, &grp.b[p], &full_bar[stage], grp.b_col0[p] + n_blk * BN + i * 64,
-                        kb * BK);
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16_mn(BM, BN);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1u);
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tcgen05_fence_after();
-          const uint32_t a_addr = smem_u32(smem_a + stage * C::A_BYTES);
-          const uint32_t b_addr = smem_u32(smem_b + stage * C::B_BYTES);
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k)
-            umma_f16(d_tmem, make_smem_desc_sw128_mn(a_addr + k * 2048, BOX), make_smem_desc_sw128_mn(b_addr + k * 2048, BOX), idesc,
-                     (kb > 0 || k > 0) ? 1u : 0u);
-          umma_commit(&empty_bar[stage]);
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-        umma_commit(&tmem_full[acc]);
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1u;
+            tma_load_2d(ring.b + pos.stage * C::B_BYTES + i * BOX, &grp.b[p], &ring.full[pos.stage],
+                        grp.b_col0[p] + n_blk * BN + i * 64, kb * BK);
+          pos.advance<STAGES>();
         }
       }
     }
   } else {
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    setmaxnreg_inc<232>();
+    const int mw = wg - 1;
+    const int row_in_tile = mw * 64 + ((threadIdx.x >> 5) & 3) * 16;
+    const uint32_t no_peer[STAGES] = {};
+    auto da = [](uint32_t addr, int k) { return make_wgmma_desc_sw128(addr + k * 2048); };
+    auto db = [](uint32_t addr, int k) { return make_wgmma_desc_sw128(addr + k * 2048, BOX); };
+    RingPos pos;
+    float acc[BN / 2];
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int p, m_blk, n_blk;
       locate(tile, p, m_blk, n_blk);
-      EpiArgs ep{nullptr, grp.dw[p], grp.dw[p], NER_EPI_RES_F32};
-      epilogue_stage_bias<BN>(sbias + acc * BN, ep, n_blk * BN, grp.n[p]);
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tcgen05_fence_after();
-      epilogue_tile<BN, true>(tmem_base + (uint32_t)(acc * BN), warp, lane, ep, &grp.c[p], epi_stage + (warp - 2) * 4096,
-                              sbias + acc * BN, m_blk * BM, n_blk * BN, grp.m[p], grp.n[p]);
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1u;
-      }
+      mma_kblocks<BN, STAGES, 1, 1, 1>(acc, ring, pos, 0, num_kb, (uint32_t)(mw * BOX), da, db, no_peer);
+      const EpiArgs ep{nullptr, grp.dw[p], grp.dw[p], NER_EPI_RES_F32};
+      epilogue_regs<BN>(acc, ep, m_blk * BM + row_in_tile, n_blk * BN, grp.m[p], grp.n[p]);
     }
-  }
-
-  if (warp >= 2 && lane == 0) tma_store_wait_read<0>();
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc<C::TMEM_COLS>(tmem_base);
-  }
-}
-
-// ===================================================================== cta_group::2 (CTA pair)
-// Protocol (s = smem stage, a = accumulator stage):
-//   full[s]        lives in CTA 0, count 1: CTA 0's producer arrive.expect_tx's the bytes of BOTH CTAs;
-//                  both CTAs' TMA loads complete_tx on it (peer-bit-masked barrier address).
-//   empty[s]       one per CTA, count 1: the MMA thread's multicast commit arrives on both.
-//   tmem_full[a]   one per CTA, count 1: multicast commit after the last k-block.
-//   tmem_empty[a]  lives in CTA 0, count 2*NUM_EPI_WARPS: every epilogue warp of both CTAs arrives
-//                  (CTA 1 through its shared::cluster address).
-template <int BN>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NUM_THREADS, 1)
-gemm_bf16_tc2_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
-                     const __grid_constant__ CUtensorMap tma_c, EpiArgs ep, int M, int N, int K) {
-  using C = Cfg2<BN>;
-  constexpr int STAGES = C::STAGES;
-
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw;
-  if ((smem_u32(smem_raw) & 1023u) != 0u) __trap();
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + STAGES * C::A_BYTES;
-  uint8_t* epi_stage = smem + STAGES * (C::A_BYTES + C::B_BYTES);  // [NUM_EPI_WARPS][32 rows][128 B], 1024-aligned
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_stage + NUM_EPI_WARPS * 4096);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  float* sbias = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full_bar) + 256);  // [2][BN]
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int pair = blockIdx.x >> 1;
-  const int num_pairs = gridDim.x >> 1;
-
-  const int num_m = (M + 2 * BM - 1) / (2 * BM);  // 256-row tiles
-  const int num_n = (N + BN - 1) / BN;
-  const int num_tiles = num_m * num_n;
-  const int num_kb = (K + BK - 1) / BK;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tma_a);
-    tma_prefetch_desc(&tma_b);
-    tma_prefetch_desc(&tma_c);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full[s], 1);
-      mbar_init(&tmem_empty[s], 2 * NUM_EPI_WARPS);
-    }
-    fence_barrier_init();
-  }
-  cluster_sync_all();  // barrier inits visible cluster-wide before any remote arrive / TMA complete_tx
-  if (warp == 1) tmem_alloc_2sm<C::TMEM_COLS>(tmem_ptr);
-  tcgen05_fence_before();
-  cluster_sync_all();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-        const int m_blk = tile / num_n, n_blk = tile - m_blk * num_n;
-        const int row_a = m_blk * 2 * BM + (int)rank * BM;
-        const int row_b = n_blk * BN + (int)rank * (BN / 2);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          if (rank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2 * (C::A_BYTES + C::B_BYTES));
-          tma_load_2d_2sm(smem_a + stage * C::A_BYTES, &tma_a, &full_bar[stage], kb * BK, row_a);
-          tma_load_2d_2sm(smem_b + stage * C::B_BYTES, &tma_b, &full_bar[stage], kb * BK, row_b);
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (one thread of CTA 0) =====================
-    if (rank == 0 && lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(2 * BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1u);
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tcgen05_fence_after();
-          const uint32_t a_addr = smem_u32(smem_a + stage * C::A_BYTES);
-          const uint32_t b_addr = smem_u32(smem_b + stage * C::B_BYTES);
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            const uint64_t da = make_smem_desc_sw128(a_addr + k * UMMA_K * 2);
-            const uint64_t db = make_smem_desc_sw128(b_addr + k * UMMA_K * 2);
-            umma_f16_2sm(d_tmem, da, db, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit_2sm(&empty_bar[stage], 0b11);
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-        umma_commit_2sm(&tmem_full[acc], 0b11);
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1u;
-        }
-      }
-    }
-  } else {
-    // ===================== epilogue warps (2..9), both CTAs =====================
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    const uint32_t empty_remote0 = mapa_u32(smem_u32(&tmem_empty[0]), 0);
-    const uint32_t empty_remote1 = mapa_u32(smem_u32(&tmem_empty[1]), 0);
-    for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-      const int m_blk = tile / num_n, n_blk = tile - m_blk * num_n;
-      epilogue_stage_bias<BN>(sbias + acc * BN, ep, n_blk * BN, N);
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tcgen05_fence_after();
-      if (ep.mode == NER_EPI_F32 || ep.mode == NER_EPI_RES_F32 || ep.mode == NER_EPI_RES_RELU_F32)
-        epilogue_tile<BN, true>(tmem_base + (uint32_t)(acc * BN), warp, lane, ep, &tma_c, epi_stage + (warp - 2) * 4096,
-                                sbias + acc * BN, m_blk * 2 * BM + (int)rank * BM, n_blk * BN, M, N);
-      else
-        epilogue_tile<BN, false>(tmem_base + (uint32_t)(acc * BN), warp, lane, ep, &tma_c, epi_stage + (warp - 2) * 4096,
-                                 sbias + acc * BN, m_blk * 2 * BM + (int)rank * BM, n_blk * BN, M, N);
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(acc == 0 ? empty_remote0 : empty_remote1);
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1u;
-      }
-    }
-  }
-
-  if (warp >= 2 && lane == 0) tma_store_wait_read<0>();
-  tcgen05_fence_before();
-  cluster_sync_all();  // both CTAs done with TMEM / remote barriers
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc_2sm<C::TMEM_COLS>(tmem_base);
   }
 }
 
@@ -844,20 +512,6 @@ int make_map_bf16_2d(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t 
   return r == CUDA_SUCCESS ? NER_OK : NER_ERR_INVALID_ARG;
 }
 
-// output [M, N] (bf16 or f32) with a {128 bytes of columns, 32 rows} box, 128-byte swizzle
-int make_map_out(CUtensorMap* map, void* ptr, uint64_t rows, uint64_t cols, bool f32) {
-  EncodeTiledFn fn = get_encode_fn();
-  if (fn == nullptr) return NER_ERR_NO_DRIVER;
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {cols * (f32 ? 4 : 2)};
-  cuuint32_t box[2] = {(cuuint32_t)(f32 ? 32 : 64), 32};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(map, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, ptr, dims, strides, box,
-                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? NER_OK : NER_ERR_INVALID_ARG;
-}
-
 // NER_GEMM_POLICY=1: "auto" picks the 128x256 tile whenever N allows instead of fitting waves (tuning hook).
 int gemm_auto_policy() {
   static int v = -1;
@@ -868,18 +522,7 @@ int gemm_auto_policy() {
   return v;
 }
 
-bool epi_is_f32(int mode) { return mode == NER_EPI_F32 || mode == NER_EPI_RES_F32 || mode == NER_EPI_RES_RELU_F32; }
-
-int sm_count() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
-  }
-  return n;
-}
+int sm_count() { return ner_num_sms(); }
 
 // Stream-K scratch: one slot of 128 x 256 fp32 per CTA + one flag per CTA, per (device, stream) so
 // that GEMMs running concurrently on different streams never share slots.  Allocated on first use
@@ -930,57 +573,54 @@ bool sk_scratch(cudaStream_t st, SkArgs* out) {
   return true;
 }
 
-template <int BN>
+// Launch with PDL and, for CL = 2, clusters of two CTAs along x.
+template <typename... KArgs, typename... Args>
+cudaError_t launch_ex(void (*kern)(KArgs...), int grid, size_t smem, cudaStream_t st, int cl, Args... args) {
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(NUM_THREADS);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[2];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  attr[1].id = cudaLaunchAttributeClusterDimension;
+  attr[1].val.clusterDim.x = cl;
+  attr[1].val.clusterDim.y = 1;
+  attr[1].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 2;
+  return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
+}
+
+template <int BN, int CL>
 int launch_gemm(const void* A, const void* Wt, EpiArgs ep, int M, int N, int K, cudaStream_t st, bool sk = false) {
   CUtensorMap ma, mb;
   int rc = make_map_bf16_2d(&ma, A, (uint64_t)M, (uint64_t)K, BM);
   if (rc != NER_OK) return rc;
-  rc = make_map_bf16_2d(&mb, Wt, (uint64_t)N, (uint64_t)K, BN);
-  if (rc != NER_OK) return rc;
-  CUtensorMap mc;
-  rc = make_map_out(&mc, ep.out, (uint64_t)M, (uint64_t)N, epi_is_f32(ep.mode));
+  rc = make_map_bf16_2d(&mb, Wt, (uint64_t)N, (uint64_t)K, BN / CL);
   if (rc != NER_OK) return rc;
   const size_t smem = Cfg<BN>::SMEM;
-  const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
+  const int tiles = ((M + CL * BM - 1) / (CL * BM)) * ((N + BN - 1) / BN);
   const int num_kb = (K + BK - 1) / BK;
   SkArgs ska{nullptr, nullptr};
-  // stream-K needs every CTA co-resident (grid = #SMs) and at least one k-block unit per CTA
-  sk = sk && (long long)tiles * num_kb >= sm_count() && ep.mode != NER_EPI_DIAG_DISCARD && sk_scratch(st, &ska);
-  if (sk) {
-    auto kern = gemm_bf16_tc_kernel<BN, true>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
-    e = ner_launch_pdl(kern, dim3(sm_count()), dim3(NUM_THREADS), smem, st, ma, mb, mc, ep, M, N, K, ska);
-    if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
-    return ner_launch_status();
+  cudaError_t e;
+  if constexpr (CL == 1) {
+    // stream-K needs every CTA co-resident (grid = #SMs) and at least one k-block unit per CTA
+    sk = sk && (long long)tiles * num_kb >= sm_count() && ep.mode != NER_EPI_DIAG_DISCARD && sk_scratch(st, &ska);
+    if (sk)
+      e = launch_ex(gemm_bf16_tc_kernel<BN, true, 1>, sm_count(), smem, st, 1, ma, mb, ep, M, N, K, ska);
+    else
+      e = launch_ex(gemm_bf16_tc_kernel<BN, false, 1>, tiles < sm_count() ? tiles : sm_count(), smem, st, 1, ma, mb, ep,
+                    M, N, K, ska);
+  } else {
+    const int max_pairs = sm_count() / 2;
+    const int pairs = tiles < max_pairs ? tiles : max_pairs;
+    e = launch_ex(gemm_bf16_tc_kernel<BN, false, 2>, 2 * pairs, smem, st, 2, ma, mb, ep, M, N, K, ska);
   }
-  auto kern = gemm_bf16_tc_kernel<BN, false>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
-  const int grid = tiles < sm_count() ? tiles : sm_count();
-  e = ner_launch_pdl(kern, dim3(grid), dim3(NUM_THREADS), smem, st, ma, mb, mc, ep, M, N, K, ska);
-  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
-  return ner_launch_status();
-}
-
-template <int BN>
-int launch_gemm2(const void* A, const void* Wt, EpiArgs ep, int M, int N, int K, cudaStream_t st) {
-  CUtensorMap ma, mb;
-  int rc = make_map_bf16_2d(&ma, A, (uint64_t)M, (uint64_t)K, BM);
-  if (rc != NER_OK) return rc;
-  rc = make_map_bf16_2d(&mb, Wt, (uint64_t)N, (uint64_t)K, BN / 2);
-  if (rc != NER_OK) return rc;
-  CUtensorMap mc;
-  rc = make_map_out(&mc, ep.out, (uint64_t)M, (uint64_t)N, epi_is_f32(ep.mode));
-  if (rc != NER_OK) return rc;
-  auto kern = gemm_bf16_tc2_kernel<BN>;
-  const size_t smem = Cfg2<BN>::SMEM;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
-  const int tiles = ((M + 2 * BM - 1) / (2 * BM)) * ((N + BN - 1) / BN);
-  const int max_pairs = sm_count() / 2;
-  const int pairs = tiles < max_pairs ? tiles : max_pairs;
-  kern<<<2 * pairs, NUM_THREADS, smem, st>>>(ma, mb, mc, ep, M, N, K);
   return ner_launch_status();
 }
 
@@ -1022,8 +662,6 @@ extern "C" int ner_wgrad_group_bf16(const ner_wgrad_problem* problems_host, int 
     if (rc != NER_OK) return rc;
     rc = make_map_bf16_box64(&g.b[p], q.dy_bf16, (uint64_t)rows, (uint64_t)q.ld_dy);
     if (rc != NER_OK) return rc;
-    rc = make_map_out(&g.c[p], q.dw, (uint64_t)q.k_in, (uint64_t)q.n_out, true);
-    if (rc != NER_OK) return rc;
     g.dw[p] = q.dw;
     g.m[p] = q.k_in;
     g.n[p] = q.n_out;
@@ -1031,17 +669,13 @@ extern "C" int ner_wgrad_group_bf16(const ner_wgrad_problem* problems_host, int 
     g.tile_start[p + 1] = g.tile_start[p] + (q.k_in / BM) * (q.n_out / WG_BN);
   }
   for (int p = count; p < WG_MAXP; ++p) {
-    g.a[p] = g.a[0]; g.b[p] = g.b[0]; g.c[p] = g.c[0];
+    g.a[p] = g.a[0]; g.b[p] = g.b[0];
     g.dw[p] = nullptr; g.m[p] = g.n[p] = g.b_col0[p] = 0;
     g.tile_start[p + 1] = g.tile_start[count];
   }
-  const size_t smem = Cfg<WG_BN>::SMEM;
-  auto kern = gemm_wgrad_group_kernel;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
   const int tiles = g.tile_start[count];
   const int grid = tiles < sm_count() ? tiles : sm_count();
-  e = ner_launch_pdl(kern, dim3(grid), dim3(NUM_THREADS), smem, static_cast<cudaStream_t>(stream), g);
+  cudaError_t e = launch_ex(gemm_wgrad_group_kernel, grid, Cfg<WG_BN>::SMEM, static_cast<cudaStream_t>(stream), 1, g);
   if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
   return ner_launch_status();
 }
@@ -1057,6 +691,8 @@ extern "C" int ner_gemm_bf16(const void* A, const void* Wt, const float* bias, c
   if ((reinterpret_cast<uintptr_t>(A) & 15) || (reinterpret_cast<uintptr_t>(Wt) & 15) ||
       (reinterpret_cast<uintptr_t>(out) & 15))
     return NER_ERR_INVALID_ARG;
+  // the epilogue reads bias and residual as float2 column pairs
+  if ((reinterpret_cast<uintptr_t>(bias) & 7) || (reinterpret_cast<uintptr_t>(residual) & 7)) return NER_ERR_INVALID_ARG;
   EpiArgs ep{bias, residual, out, epilogue};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   int bn = tile_n;
@@ -1070,8 +706,8 @@ extern "C" int ner_gemm_bf16(const void* A, const void* Wt, const float* bias, c
   }
   if (bn == 0) {
     // Cost model in units of one 128x256 k-block per CTA.  Whole-tile scheduling: ceil(tiles/SMs) waves
-    // of num_kb k-blocks, the relative tile costs measured on B200 (profiles/): the 128-wide tile is
-    // smem-bandwidth-bound.  Stream-K (128x256 tiles): every CTA gets ceil(tiles*num_kb/SMs) k-blocks
+    // of num_kb k-blocks times the relative k-block cost of the tile width (narrower tiles re-read the A
+    // tile more often per FLOP).  Stream-K (128x256 tiles): every CTA gets ceil(tiles*num_kb/SMs) k-blocks
     // plus a fixed charge for parking / adding one partial accumulator.
     const int mt = (M + BM - 1) / BM, sms = sm_count(), num_kb = (K + BK - 1) / BK;
     const int cand[3] = {256, 192, 128};
@@ -1097,12 +733,12 @@ extern "C" int ner_gemm_bf16(const void* A, const void* Wt, const float* bias, c
     }
   }
   switch (bn) {
-    case 256: return launch_gemm<256>(A, Wt, ep, M, N, K, st, sk);
-    case 192: return launch_gemm<192>(A, Wt, ep, M, N, K, st);
-    case 128: return launch_gemm<128>(A, Wt, ep, M, N, K, st, sk);
-    case 64: return launch_gemm<64>(A, Wt, ep, M, N, K, st);
-    case NER_TILE_2CTA_256: return launch_gemm2<256>(A, Wt, ep, M, N, K, st);
-    case NER_TILE_2CTA_128: return launch_gemm2<128>(A, Wt, ep, M, N, K, st);
+    case 256: return launch_gemm<256, 1>(A, Wt, ep, M, N, K, st, sk);
+    case 192: return launch_gemm<192, 1>(A, Wt, ep, M, N, K, st);
+    case 128: return launch_gemm<128, 1>(A, Wt, ep, M, N, K, st, sk);
+    case 64: return launch_gemm<64, 1>(A, Wt, ep, M, N, K, st);
+    case NER_TILE_2CTA_256: return launch_gemm<256, 2>(A, Wt, ep, M, N, K, st);
+    case NER_TILE_2CTA_128: return launch_gemm<128, 2>(A, Wt, ep, M, N, K, st);
     default: return NER_ERR_INVALID_ARG;
   }
 }

@@ -1,7 +1,7 @@
 // One C-ABI call for the whole PREDICT step of the bert_bilstm_crf plugin (reference
 // model/bert_bilstm_crf.py:8-34 in PREDICT mode: pretrain_bert_embedding -> bilstm -> dense(logits) ->
 // crf_decode; the log-likelihood of crf_layer is not fetched by PREDICT, tools/train_utils.py:181-185).
-// The host enqueues: packing plan, packed BERT encoder, LSTM input projection (tcgen05 GEMM), the
+// The host enqueues: packing plan, packed BERT encoder, LSTM input projection (wgmma GEMM), the
 // bidirectional recurrence, the label projection and Viterbi — the same kernels the layer functions of
 // chinesener_b200/tools/layer.py launch one by one, in the same order, on the caller's stream.  It exists to
 // take the ~20 Python-level calls of a step off the host's critical path when eight 4-stream pipelines share

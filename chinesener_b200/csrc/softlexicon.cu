@@ -1,4 +1,4 @@
-// SoftLexicon B/M/E/S gather-and-pool (sm_100a), forward and backward.
+// SoftLexicon B/M/E/S gather-and-pool (sm_90a), forward and backward.
 //
 // Replaces the embedding_lookup * weight -> reshape -> reduce_sum block of reference
 // model/bilstm_crf_softlexicon.py:37-44 (same block in bert_bilstm_crf_softlexicon.py):
@@ -100,7 +100,7 @@ extern "C" int ner_softlexicon_pool_fwd(const float* table, const int32_t* ids, 
   if (!table || !ids || !weights || !out) return NER_ERR_INVALID_ARG;
   if (G * S > 64 || E > 32 * MAXE_PER_LANE) return NER_ERR_UNSUPPORTED;
   long grid = ((long)n_tok + 7) / 8;
-  if (grid > 148L * 32) grid = 148L * 32;
+  if (grid > (long)ner_num_sms() * 32) grid = (long)ner_num_sms() * 32;
   softlexicon_pool_fwd_kernel<<<(int)grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(table, ids, weights, out, n_tok,
                                                                                         G, S, E, V, ld_out);
   return ner_launch_status();
@@ -112,7 +112,7 @@ extern "C" int ner_softlexicon_pool_bwd(float* d_table, const int32_t* ids, cons
   if (n_tok == 0) return NER_OK;
   if (!d_table || !ids || !weights || !d_out) return NER_ERR_INVALID_ARG;
   long grid = ((long)n_tok + 7) / 8;
-  if (grid > 148L * 32) grid = 148L * 32;
+  if (grid > (long)ner_num_sms() * 32) grid = (long)ner_num_sms() * 32;
   softlexicon_pool_bwd_kernel<<<(int)grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(d_table, ids, weights, d_out,
                                                                                         n_tok, G, S, E, V);
   return ner_launch_status();

@@ -1,4 +1,4 @@
-// Training-side HBM-bound kernels (sm_100a): operand transposes for the weight-gradient GEMMs,
+// Training-side HBM-bound kernels (sm_90a): operand transposes for the weight-gradient GEMMs,
 // bias gradients, label-projection backward, dropout, and the two optimizer steps of the reference
 // (tools/train_utils.py:246-390): AdamWeightDecayOptimizer (no bias correction, decoupled weight
 // decay, global-norm clipping) and tf.train.AdamOptimizer (bias-corrected, clip-by-value).
@@ -268,7 +268,7 @@ move_rows_kernel(const uint4* __restrict__ src, const int32_t* __restrict__ idx,
 
 int flat_grid(size_t n) {
   size_t g = (n + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > ner_num_sms() * 16) g = ner_num_sms() * 16;
   if (g < 1) g = 1;
   return (int)g;
 }
@@ -301,7 +301,7 @@ extern "C" int ner_dense_small_n_bwd(const float* x, const float* W, const float
   const size_t smem = (size_t)2 * F * N * 4;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   long g = ((long)M + 63) / 64;
-  if (g > 148 * 2) g = 148 * 2;
+  if (g > ner_num_sms() * 2) g = ner_num_sms() * 2;
   cudaError_t e;
   if (N <= 16) {
     auto kern = dense_small_n_bwd_kernel<16>;
@@ -373,7 +373,7 @@ extern "C" int ner_dropout(const float* x, float* y, size_t n, float keep_prob, 
   return ner_launch_status();
 }
 
-extern "C" size_t ner_sumsq_scratch_floats(void) { return (size_t)148 * 16; }
+extern "C" size_t ner_sumsq_scratch_floats(void) { return (size_t)ner_num_sms() * 16; }
 
 extern "C" int ner_sumsq_add(const float* g, size_t n, float* out, float* scratch, ner_stream_t stream) {
   if (!g || !out || !scratch) return n == 0 ? NER_OK : NER_ERR_INVALID_ARG;

@@ -115,8 +115,8 @@ class Estimator:
         8(e)), so the SMs a kernel of one call leaves idle are taken by the other call's kernels.
         group > 1: `group` consecutive host batches are stacked into one device batch per call (sentences are
         independent, so the tags are those of the separate calls): the packed token count of a 64-sentence MSRA batch
-        (~3.2 k rows) fills 0.5 / 1.5 / 2.0 waves of 128x256 GEMM tiles on 148 SMs, two batches (~6.3 k rows) fill
-        1.0 / 3.0 / 4.0 — the tensor-core tiles stop idling in partial waves without relying on stream overlap."""
+        (~3.2 k rows) fills 0.6 / 1.7 / 2.3 waves of 128x256 GEMM tiles on 132 SMs, two batches (~6.3 k rows) fill
+        1.1 / 3.4 / 4.5 — the tensor-core tiles stop idling in partial waves without relying on stream overlap."""
         from . import ops
         ring, inflight = {}, []
         depth = max(depth, streams + 1) if streams > 1 else depth

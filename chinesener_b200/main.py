@@ -14,7 +14,7 @@ What `singletask_train` does, in the reference's order (main.py:14-62):
   * PREDICT over the `predict` split with the LAST checkpoint's weights; the list of per-sentence dicts
     {'pred_ids' int32[L], 'label_ids' int32[L], 'tokens' bytes[L]} is pickled to `<data_dir>/<model>_predict.pkl`
     (main.py:52-55) — the file evaluation.py scores.
-The Estimator's own evaluation cadence is time based (throttle_secs=60, the hook polls every 60 s); on a B200 a whole
+The Estimator's own evaluation cadence is time based (throttle_secs=60, the hook polls every 60 s); on an H100 a whole
 epoch takes seconds, so the cadence here is the step-based one those timers converge to on the reference's hardware:
 evaluate at every checkpoint.  Exporting a SavedModel (main.py:57-60) has no counterpart: the in-process InferHelper
 serves from the checkpoint.
@@ -228,7 +228,7 @@ def build_parser():
     parser.add_argument('--model_name', type=str, help='model_name[bert_bilstm_crf, bert_crf, bilstm_crf ...]', required=True)
     parser.add_argument('--clear_model', type=int, help='Whether to clear existing model', required=False, default=0)
     parser.add_argument('--data', type=str, help='which data to use[msra, people_daily]', required=False, default='msra')
-    parser.add_argument('--gpu', type=int, help='kept for compatibility: the sm_100a path always runs on the GPU', required=False, default=1)
+    parser.add_argument('--gpu', type=int, help='kept for compatibility: the sm_90a path always runs on the GPU', required=False, default=1)
     parser.add_argument('--device', type=int, help='which gpu to use', required=False, default=-1)
     parser.add_argument('--rename', type=str, help='Allow rename model with special parameter', required=False, default='')
     parser.add_argument('--export_only', type=int, help='kept for compatibility (no SavedModel export: InferHelper serves in-process)',

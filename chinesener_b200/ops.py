@@ -48,7 +48,7 @@ def crf_loglik_fwd(logits, tags, seq_len, trans, want_alpha=False, exact=False):
     return ll, logz, alpha
 
 
-# --------------------------------------------------------------------------- dense (tcgen05)
+# --------------------------------------------------------------------------- dense (wgmma)
 def gemm_bf16(a, wt, bias=None, residual=None, epilogue=EPI_BF16, tile_n=None, out=None):
     """out[M,N] = epilogue(a[M,K] @ wt[N,K]^T + bias).  a, wt bf16; see ner_gemm_bf16.  tile_n None = DEFAULT_TILE."""
     if tile_n is None:
@@ -277,7 +277,7 @@ def split_bf16(x2d, Dp=None):
 
 def gemm_split_f32(a_hi, a_lo, w_hi, w_lo, bias=None, residual=None, relu=False, out=None):
     """out f32 [M,N] = [relu](A·W^T + bias [+ residual]) at ~fp32 accuracy: A_hi·W_hi + A_hi·W_lo + A_lo·W_hi
-    as three tcgen05 launches chained through the f32 residual epilogue."""
+    as three wgmma launches chained through the f32 residual epilogue."""
     M, N = a_hi.shape[0], w_hi.shape[0]
     if out is None:
         out = torch.empty((M, N), dtype=torch.float32, device=a_hi.device)

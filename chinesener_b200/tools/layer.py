@@ -15,7 +15,7 @@ from .. import ops, variables
 PACK_SEQUENCES = os.environ.get("NER_B200_PACK", "1") != "0"
 # TRAIN mode of BertModel on the packed layout too (ner_bert_encoder_train_fwd_packed / _bwd_packed)
 TRAIN_PACK = os.environ.get("NER_B200_TRAIN_PACK", "1") != "0"
-# 'bf16': bf16 tcgen05 operands (BASELINE config 3, the benchmark path); 'fp32': fp32-accurate encoder (config 2's
+# 'bf16': bf16 wgmma operands (BASELINE config 3, the benchmark path); 'fp32': fp32-accurate encoder (config 2's
 # "fp32": split-bf16 dense + fp32 attention, emission logits within 1e-3 of the reference).  Estimator sets it from
 # params['bert_precision'] around build_graph.
 BERT_PRECISION = os.environ.get("NER_B200_BERT_PRECISION", "bf16")
@@ -100,7 +100,7 @@ def bilstm(embedding, cell_type, activation, hidden_units_list, keep_prob_list, 
     if is_training:
         return _bilstm_train(embedding, activation, hidden_units_list, keep_prob_list, cell_size, seq_len)
     if cell_type.lower() != 'lstm':
-        raise Exception('Only lstm is built on the sm_100a path (reference models all use cell_type=lstm)')
+        raise Exception('Only lstm is built on the sm_90a path (reference models all use cell_type=lstm)')
     if cell_size != 1:
         raise Exception('cell_size must be 1 (every reference model uses a single LSTM layer)')
     pack = getattr(embedding, "pack", None)

@@ -92,7 +92,7 @@ def _backward_order(name):
 class GradExchange(object):
     """The data-parallel gradient exchange of one TRAIN step, overlapped with the backward pass (SURVEY 8e).
 
-    The reference is single device; the B200 engine shards sentences over ranks and sums gradients.  Instead of one
+    The reference is single device; this engine shards sentences over ranks and sums gradients.  Instead of one
     all-reduce after the whole backward, the flat gradient buffer (laid out in backward-completion order, FlatState) is
     cut into contiguous buckets — the dense kernels of each encoder layer, 11 first ... 0, then the rest (embeddings,
     LayerNorm / bias ranges, the layers above BertModel) — and a layer bucket is all-reduced on a side stream as soon as the event recorded behind its last

@@ -1,6 +1,6 @@
 # -*-coding:utf-8 -*-
 """Transformer building blocks with the reference's surface (reference tools/transformer/modules.py),
-executed at fp32 accuracy: dense layers run as three split-bf16 tcgen05 products (ops.gemm_split_f32),
+executed at fp32 accuracy: dense layers run as three split-bf16 wgmma products (ops.gemm_split_f32),
 LayerNorm / attention in fp32."""
 import numpy as np
 import torch

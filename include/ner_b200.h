@@ -1,5 +1,5 @@
 /*
- * ner_b200.h — C-ABI of libner_b200.so: the sm_100a kernels behind the
+ * ner_b200.h — C-ABI of libner_b200.so: the sm_90a kernels behind the
  * bert_bilstm_crf hot path of DSXiangLi/ChineseNER.
  *
  * Every entry point mirrors one reference call site (cited per function,
@@ -35,7 +35,7 @@ typedef void* ner_stream_t; /* cudaStream_t */
 const char* ner_strerror(int status);
 /* Library/ABI version; bumps when a signature changes. */
 int ner_abi_version(void);
-/* Build provenance: "src=<hash of the sources this library was compiled from> nvcc=<version> arch=sm_100a"; the hash is
+/* Build provenance: "src=<hash of the sources this library was compiled from> nvcc=<version> arch=sm_90a"; the hash is
  * chinesener_b200.build.source_hash() of the tree at compile time. */
 const char* ner_build_info(void);
 
@@ -77,7 +77,7 @@ int ner_crf_loglik_bwd(const float* logits, const int32_t* tags, const int32_t* 
 
 
 /* ------------------------------------------------------------------------ *
- * Dense layers on tcgen05 tensor cores — replaces tf.layers.dense /
+ * Dense layers on wgmma tensor cores — replaces tf.layers.dense /
  * modeling.dense_layer inside BertModel (tools/layer.py:68-77), the logits
  * projection's big-M cousins and the LSTM input projection (tools/layer.py:35)
  * ------------------------------------------------------------------------ */
@@ -88,11 +88,11 @@ int ner_crf_loglik_bwd(const float* logits, const int32_t* tags, const int32_t* 
 #define NER_EPI_RELU_BF16 4      /* out bf16 = relu(acc + bias)              */
 #define NER_EPI_RES_F32 5        /* out f32  = acc + bias + residual (f32)   */
 #define NER_EPI_RES_RELU_F32 6   /* out f32  = relu(acc + bias + residual)   */
-#define NER_EPI_DIAG_DISCARD 99  /* diagnostic only: accumulate, drain TMEM, store nothing */
+#define NER_EPI_DIAG_DISCARD 99  /* diagnostic only: accumulate, store nothing */
 
 /* tile_n selectors of ner_gemm_bf16: 64/128/192/256 = one CTA per 128 x tile_n tile
- * (cta_group::1), whole tiles round-robin over the SMs; the 2CTA values = a CTA pair per 256 x N
- * tile (cta_group::2); the SK values = 128 x tile_n tiles with stream-K scheduling (every SM gets
+ * (one CTA), whole tiles round-robin over the SMs; the 2CTA values = a cluster of two CTAs per 256 x N
+ * tile (B tile TMA-multicast to both); the SK values = 128 x tile_n tiles with stream-K scheduling (every SM gets
  * the same number of k-blocks; split tiles are summed through an internal fp32 scratch). */
 #define NER_TILE_2CTA_128 1128
 #define NER_TILE_2CTA_256 1256
@@ -106,6 +106,7 @@ int ner_crf_loglik_bwd(const float* logits, const int32_t* tags, const int32_t* 
 /* out[M,N] = epilogue(A[M,K] · Wt[N,K]^T + bias[N]).  A and Wt are bf16,
  * K contiguous (Wt is the TF kernel [K,N] transposed once by
  * ner_pack_weight_bf16).  bias may be NULL.  K % 8 == 0, N % 32 == 0.
+ * A, Wt, out 16-byte aligned; bias, residual 8-byte aligned (NER_ERR_INVALID_ARG otherwise).
  * tile_n: 0 = auto, or one of the selectors above. */
 int ner_gemm_bf16(const void* A, const void* Wt, const float* bias, const float* residual,
                   void* out, int M, int N, int K, int epilogue, int tile_n,
@@ -212,7 +213,7 @@ int ner_layernorm_dropout(const void* y, int y_is_bf16, const float* residual, c
  * keep_prob < 1: attention_probs dropout of BertModel in training (probabilities scaled by
  * keep(seed; b, head, q, k) / keep_prob after the softmax); keep_prob = 1: inference.
  * n_rows: rows of qkv / ctx — the packed token count in packed mode (0 = unknown), B*L or 0 in padded mode.
- * keep_prob = 1 with known n_rows and L <= 256 runs on tcgen05 (S = Q K^T and O = P V accumulate in tensor memory, Q/K/V
+ * keep_prob = 1 with known n_rows and L <= 256 runs on wgmma (S = Q K^T and O = P V accumulate in registers, Q/K/V
  * tiles arrive by TMA, V is consumed as an MN-major operand); otherwise a warp-level mma.sync kernel (ABI version 2). */
 int ner_bert_attention(const void* qkv_bf16, const int32_t* mask, void* ctx_bf16, int B, int L,
                        int num_heads, int head_dim, float scale, float mask_add,
@@ -502,7 +503,7 @@ int ner_bert_attention_bwd_packed(const void* qkv_bf16, const int32_t* cu_seqlen
 /* Weight gradients of several dense layers in ONE launch (tools/train_utils.py:314 `tf.gradients` w.r.t. the dense kernels):
  *   dw_p[k_in, n_out] (f32, accumulated into) += x_p^T . dy_p[:, dy_col0 : dy_col0 + n_out]
  * x_p bf16 [rows, ld_x] (the layer's input activations, first k_in columns used), dy_p bf16 [rows, ld_dy] (gradient w.r.t. the
- * layer's output).  Both are consumed as they lie (token-major = MN-major tcgen05 operands, 64 x 64 TMA boxes): no transposed
+ * layer's output).  Both are consumed as they lie (token-major = MN-major wgmma operands, 64 x 64 TMA boxes): no transposed
  * copies.  k_in % 128 == 0, n_out % 256 == 0, dy_col0 % 64 == 0, ld % 8 == 0; at most 6 problems per call. */
 typedef struct {
   const void* x_bf16;

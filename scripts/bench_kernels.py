@@ -85,7 +85,7 @@ if __name__ == "__main__":
 
 
 def bench_attention():
-    """tcgen05 attention vs the mma.sync kernel at the bench shapes: one MSRA-shaped 64-sentence batch and four stacked."""
+    """wgmma attention vs the mma.sync kernel at the bench shapes: one MSRA-shaped 64-sentence batch and four stacked."""
     import os
     from chinesener_b200 import synthetic
     import numpy as np
@@ -96,7 +96,7 @@ def bench_attention():
         T = int(lens.sum())
         qkv = torch.randn(T, 3 * NH * D, device="cuda").to(torch.bfloat16)
         cu = torch.tensor([0] + list(np.cumsum(lens)), dtype=torch.int32, device="cuda")
-        for name, var in (("tcgen05", None), ("mma_sync", "1")):
+        for name, var in (("wgmma", None), ("mma_sync", "1")):
             if var:
                 os.environ["NER_ATTN_VARIANT"] = var
             med, best = timeit(lambda: ops.bert_attention(qkv, None, B, 128, NH, D, cu_seqlens=cu), iters=30)

@@ -1,12 +1,12 @@
 """Summarise an ncu launch list (`--metrics gpu__time_duration.sum --csv`): time per kernel family and its share.
-usage: python scripts/launch_shares.py profiles/r01_ncu_launches_*.csv [first_row last_row]"""
+usage: python scripts/launch_shares.py <launches.csv> [first_row last_row]"""
 import csv
 import re
 import sys
 from collections import OrderedDict
 
 FAMILIES = OrderedDict([
-    ("gemm (tcgen05)", r"gemm_bf16_tc"), ("attention", r"attention"), ("bilstm recurrence", r"bilstm"),
+    ("gemm (wgmma)", r"gemm_bf16_tc"), ("attention", r"attention"), ("bilstm recurrence", r"bilstm"),
     ("layernorm / embed", r"layernorm|embed"), ("crf", r"crf_"), ("label projection", r"dense_small"),
     ("cast / pack / gelu / misc", r".*"),
 ])

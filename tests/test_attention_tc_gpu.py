@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 attention kernel (csrc/attention_tc.cu — S = Q K^T and O = P V in tensor memory, TMA operand loads, V as
+"""GPU: the wgmma attention kernel (csrc/attention_tc.cu — S = Q K^T and O = P V in registers, TMA operand loads, V as
 an MN-major operand) against a plain PyTorch fp32 softmax(QK^T)V of the same bf16 inputs, against the warp-level mma.sync
 kernel it replaces on the inference path, on ragged packed batches, and with hostile neighbours (rows of other sequences
 that ride along in a TMA box must never leak into a result)."""

@@ -1,5 +1,5 @@
 """GPU: TRAIN mode of the bert_crf plugin (BASELINE config 2's model) — the full encoder backward
-(dense dgrad/wgrad on tcgen05, attention backward, LayerNorm/GELU/embedding backward) against
+(dense dgrad/wgrad on wgmma, attention backward, LayerNorm/GELU/embedding backward) against
 autograd of the float64 oracle, and a short AdamW run."""
 import json
 

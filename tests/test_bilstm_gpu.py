@@ -1,4 +1,4 @@
-"""GPU: persistent cluster BiLSTM recurrence (+ tcgen05 input projection) vs the CPU oracle."""
+"""GPU: persistent cluster BiLSTM recurrence (+ wgmma input projection) vs the CPU oracle."""
 import pytest
 import torch
 

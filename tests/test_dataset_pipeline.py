@@ -3,7 +3,6 @@
 Golden fixtures (tests/golden/make_msra_sample_golden.py, make_variables_index_golden.py): the reference's own featurisation
 of its MSRA test split, recovered from the tokens / label_ids inside `data/msra/bilstm_crf_predict.pkl`; its
 `data_params.pkl`; the `variables.index` tables of its four serving checkpoints."""
-import hashlib
 import json
 import os
 import pickle
@@ -66,22 +65,6 @@ def test_data_params_match_the_shipped_pickle(tmp_path):
     assert dp["n_sample"] == 16 and dp["embedding"].shape[1] == 50
     ds = records.NerDataset(out, batch_size=5, epoch_size=3, model_name="bilstm_crf")
     assert ds.params["step_per_epoch"] == 3 and ds.params["num_train_steps"] == 9              # dataset.py:62-63
-
-
-@pytest.mark.skipif(not os.path.exists(os.path.join(os.path.dirname(GOLD), "..", "datasets", "msra", "giga_predict.nerrec")),
-                    reason="datasets/msra not generated (python -m chinesener_b200.data.preprocess ...)")
-def test_full_test_split_digest_matches_the_reference_pickle():
-    rec = records.RecordFile(os.path.join(os.path.dirname(GOLD), "..", "datasets", "msra", "giga_predict.nerrec"))
-    assert rec.n == SAMPLE["n_test"]
-    b = rec.batch(slice(0, rec.n))
-    h = hashlib.sha256()
-    for row in b["tokens"]:
-        h.update("\x1f".join(row).encode("utf-8") + b"\n")
-    assert h.hexdigest() == SAMPLE["tokens_sha256"]
-    h = hashlib.sha256()
-    for row in b["label_ids"].numpy():
-        h.update(bytes(int(x) for x in row))
-    assert h.hexdigest() == SAMPLE["label_ids_sha256"]
 
 
 def test_record_file_round_trip_with_optional_features(tmp_path):

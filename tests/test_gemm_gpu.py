@@ -1,4 +1,4 @@
-"""GPU: tcgen05/TMA dense kernel vs a plain PyTorch fp32 matmul of the same bf16 operands."""
+"""GPU: wgmma/TMA dense kernel vs a plain PyTorch fp32 matmul of the same bf16 operands."""
 import pytest
 import torch
 
@@ -56,6 +56,20 @@ def test_gemm_epilogues(epi, tile_n):
         torch.testing.assert_close(out, ref, rtol=1e-4, atol=1e-3)
 
 
+def test_gemm_rejects_misaligned_bias_and_residual():
+    """The epilogue reads bias and residual as 8-byte column pairs: a view starting at an odd float is refused, not read."""
+    M, N, K = 128, 128, 64
+    a = torch.randn(M, K).to(torch.bfloat16).cuda()
+    wt = torch.randn(N, K).to(torch.bfloat16).cuda()
+    buf = torch.randn(M * N + 1).cuda()
+    with pytest.raises(ops.NerB200Error):
+        ops.gemm_bf16(a, wt, buf[1:N + 1], epilogue=ops.EPI_F32)
+    with pytest.raises(ops.NerB200Error):
+        ops.gemm_bf16(a, wt, None, residual=buf[1:].view(M, N), epilogue=ops.EPI_RES_F32)
+    out = ops.gemm_bf16(a, wt, buf[2:N + 2], residual=buf[:M * N].view(M, N), epilogue=ops.EPI_RES_F32)
+    torch.testing.assert_close(out, _ref(a, wt, buf[2:N + 2], buf[:M * N].view(M, N), ops.EPI_RES_F32), rtol=1e-4, atol=1e-3)
+
+
 def test_gemm_auto_tile_and_no_bias():
     M, N, K = 8192, 1024, 768
     g = torch.Generator().manual_seed(1)
@@ -106,7 +120,7 @@ def test_gemm_stream_k_on_a_second_stream():
 @pytest.mark.parametrize("rows", [3150, 64, 1, 200, 4097])
 def test_grouped_mn_major_weight_gradients(rows):
     """ner_wgrad_group_bf16: dW += X^T dY for a group of problems in one launch, operands consumed token-major (MN-major
-    tcgen05 descriptors, no transposed copies) — vs fp32 matmuls of the same bf16 operands; accumulation into dW, column
+    wgmma descriptors, no transposed copies) — vs fp32 matmuls of the same bf16 operands; accumulation into dW, column
     slices of a fused dY (the Q/K/V gradients), rows that are not a multiple of the 64-token k-block."""
     g = torch.Generator().manual_seed(rows)
     H, I = 768, 3072

@@ -1,4 +1,4 @@
-"""GPU: fp32-accurate dense (split-bf16 tcgen05), fp32 TENER attention and the TENER plugin vs the oracle."""
+"""GPU: fp32-accurate dense (split-bf16 wgmma), fp32 TENER attention and the TENER plugin vs the oracle."""
 import numpy as np
 import pytest
 import torch

@@ -9,7 +9,7 @@
 
 Parity is "unpinned" in the sense of SURVEY 8(c): no reference artefact holds logits; the oracle restates TF 1.14 /
 bert-base 0.0.9 semantics and is itself checked against HuggingFace BertModel / torch.nn.LSTM / brute force.
-Tolerances are written at each assert.  The measured errors are printed (pytest -s) and copied to profiles/README.md.
+Tolerances are written at each assert.  The measured errors are printed (pytest -s).
 """
 import json
 
