@@ -48,6 +48,8 @@ SIGNATURES = {
     "ner_dropout_bf16": (_i, [_vp, _vp, _c.c_size_t, _c.c_float, _c.c_uint64, _vp]),
     "ner_sumsq_add": (_i, [_vp, _c.c_size_t, _vp, _vp, _vp]),
     "ner_sumsq_scratch_floats": (_c.c_size_t, []),
+    "ner_token_xent": (_i, [_vp] * 6 + [_c.c_float, _vp, _i, _i, _i, _vp]),
+    "ner_token_xent_scratch_floats": (_c.c_size_t, []),
     "ner_layernorm_bwd": (_i, [_vp, _i] + [_vp] * 7 + [_i, _i, _c.c_float, _vp]),
     "ner_layernorm_dropout_bwd": (_i, [_vp, _i] + [_vp] * 7 + [_i, _i, _c.c_float, _c.c_float, _c.c_uint64, _vp]),
     "ner_layernorm_dropout_bwd_bias": (_i, [_vp, _i] + [_vp] * 8 + [_i, _i, _c.c_float, _c.c_float, _c.c_uint64, _vp]),

@@ -427,6 +427,16 @@ int ner_reduce_max_time_bwd(const float* x, const float* y, const float* dy, flo
  * loss[b]; dlogits (nullable) = scale * (softmax - onehot). */
 int ner_softmax_xent(const float* logits, const int32_t* labels, float* loss, float* dlogits, int B, int N,
                      float scale, ner_stream_t stream);
+/* model/bert_ce.py + tools/loss.py: cross_entropy_loss and tf.argmax(logits, -1) in one pass over logits [B,L,K] f32.
+ * pred_ids [B,L] i32 (nullable): first argmax at EVERY t < L (not masked).  labels [B,L] i32 (nullable: no loss).
+ * loss [1] f32 (nullable) = sum_{t<len_b} (lse - z[y]) / N,  N = sum_b clamp(len_b, 0, L), 0 when N = 0.
+ * d_logits [B,L,K] f32 (nullable, fully written) = d_loss / N * (softmax - onehot) for t < len_b, 0 elsewhere.
+ * Deterministic: per-CTA partials in scratch (>= ner_token_xent_scratch_floats()), summed in index order; no float
+ * atomics.  N is computed on the device from seq_len (no host synchronisation).  K <= 32; labels in [0, K) for t < len_b.
+ * seq_len and scratch are required with labels; loss / d_logits without labels is NER_ERR_INVALID_ARG.  B * L < 2^31. */
+size_t ner_token_xent_scratch_floats(void);
+int ner_token_xent(const float* logits, const int32_t* labels, const int32_t* seq_len, int32_t* pred_ids, float* loss,
+                   float* d_logits, float d_loss, float* scratch, int B, int L, int K, ner_stream_t stream);
 /* dst[i] += a * src[i]. */
 int ner_axpy_f32(float* dst, const float* src, size_t n, float a, ner_stream_t stream);
 /* out[0] += sum(g^2)  (tf.clip_by_global_norm, tools/train_utils.py:315).  Deterministic (no float atomics): per-CTA partial
