@@ -1,5 +1,7 @@
-// Softmax token head of the bert_ce plugin (model/bert_ce.py + tools/loss.py): masked token cross-entropy, its gradient
-// and the first-maximum argmax, in one pass over the logits [B, L, K <= 32] f32 (sm_90a).  Softmax is never stored.
+// Softmax token heads of the bert_ce and bert_dice plugins (model/bert_ce.py, model/bert_dice.py + tools/loss.py): a masked
+// token loss, its gradient and the first-maximum argmax, in one pass over the logits [B, L, K <= 32] f32 (sm_90a).  The
+// softmax is never stored.  Two losses share the pass: cross-entropy (ner_token_xent) and the self-adjusting Dice loss
+// (ner_token_dice); each is a row functor (XentLoss, DiceLoss) of the one kernel template.
 //
 // HBM-bound.  A CTA stages a tile of 256 rows (256 * K contiguous floats) through shared memory with coalesced loads, one
 // thread then owns one row (the shared rows are laid out with an odd stride, K | 1, so the per-row reads are free of bank
@@ -7,6 +9,8 @@
 // float atomics: one partial per CTA, summed in index order by a one-CTA finaliser, so identical inputs give a
 // bit-identical loss.  The token count N is summed on the device from seq_len before the main pass, which needs it to
 // scale the gradient.
+#include <cmath>
+
 #include "common.cuh"
 
 namespace {
@@ -41,12 +45,88 @@ __device__ __forceinline__ int tile_slot(int e, bool pad, uint32_t k_magic) {
   return pad ? e + (int)__umulhi((uint32_t)e, k_magic) : e;
 }
 
+// A row functor adds the loss of one valid row z[0..K) (in shared memory; m = max, arg = first argmax, y = label) to acc
+// and, when GRAD, overwrites z with scale * d loss / d z.  kGradTiles: shared tiles its GRAD pass needs; the row w[0..K)
+// of the second one is free for per-class intermediates.
+
+// Cross-entropy: logsumexp(z) - z[y]; gradient softmax - onehot.
+struct XentLoss {
+  static constexpr int kGradTiles = 1;
+  template <bool GRAD>
+  __device__ __forceinline__ void row(float* z, float* /*w*/, int K, int y, float m, int /*arg*/, float scale,
+                                      float& acc) const {
+    const float zy = z[y];
+    float s = 0.f;
+    for (int j = 0; j < K; ++j) {
+      const float ej = expf(z[j] - m);
+      s += ej;
+      if (GRAD) z[j] = ej;
+    }
+    acc += (m - zy) + logf(s);
+    if (GRAD) {
+      const float inv = scale / s;
+      for (int j = 0; j < K; ++j) z[j] = z[j] * inv - (j == y ? scale : 0.f);
+    }
+  }
+};
+
+// Self-adjusting Dice loss (Li et al., ACL 2020) summed over the K classes; formula and gradient in ner_b200.h.  With
+// e_k = exp(z_k - m) and s = sum e, u_k = 1 - p_k is computed as s_{-k} / s: s - e_k is accurate for k != arg (s_{-k} >= 1
+// there), s_{-arg} is summed directly because s - e_arg cancels to 0 as soon as p_arg rounds to 1.
+struct DiceLoss {
+  static constexpr int kGradTiles = 2;
+  float alpha, gamma;
+
+  // Class k from e = e_k, sm = s_{-k}, inv_s = 1 / s: returns l_k and sets c = c_k, r = c_k / s_{-k} (0 when s_{-k} = 0,
+  // where c_k is 0 too).
+  __device__ __forceinline__ float term(float e, float sm, float inv_s, bool is_y, float& c, float& r) const {
+    const float p = e * inv_s, u = sm * inv_s;
+    const float ua = alpha == 1.f ? u : powf(u, alpha);    // powf(u, 0) = 1 at u = 0 too
+    const float q = ua * p;
+    const float inv = 1.f / (q + (is_y ? 1.f + gamma : gamma));
+    c = (is_y ? -(2.f + gamma) : gamma) * inv * inv * p * ua * (u - alpha * p);
+    r = sm > 0.f ? c / sm : 0.f;
+    return (is_y ? 1.f - q : q) * inv;
+  }
+
+  // z holds e_k after the first loop, w the c_k of the second (GRAD).  R - r_arg is summed directly as well:
+  // r_arg = c_arg / s_{-arg} grows like u_arg^(alpha-1) on a confident row and would swamp the other r_k in R.
+  template <bool GRAD>
+  __device__ __forceinline__ void row(float* z, float* w, int K, int y, float m, int arg, float scale, float& acc) const {
+    float s = 0.f, s_arg = 0.f;
+    for (int j = 0; j < K; ++j) {
+      const float ej = expf(z[j] - m);
+      s += ej;
+      if (j != arg) s_arg += ej;
+      z[j] = ej;
+    }
+    const float inv_s = 1.f / s;
+    float l = 0.f, r_arg = 0.f, R_arg = 0.f, c, r;
+    for (int j = 0; j < K; ++j) {
+      const float ej = z[j];
+      l += term(ej, j == arg ? s_arg : s - ej, inv_s, j == y, c, r);
+      if (GRAD) w[j] = c;
+      if (j == arg) r_arg = r;
+      else R_arg += r;
+    }
+    if (GRAD) {
+      const float R = r_arg + R_arg;
+      for (int j = 0; j < K; ++j) {
+        const float ej = z[j], cj = w[j];
+        const float rest = j == arg ? R_arg : R - cj / (s - ej);         // R - r_j; s - e_j >= e_arg = 1
+        z[j] = scale * (cj - ej * rest);
+      }
+    }
+    acc += l;
+  }
+};
+
 // LABELS: labels / seq_len present, per-CTA loss partials written to scratch.  GRAD: d_logits written (every row).
-template <bool LABELS, bool GRAD>
+template <class Loss, bool LABELS, bool GRAD>
 __global__ void __launch_bounds__(kRows)
-token_xent_kernel(const float* __restrict__ logits, const int32_t* __restrict__ labels, const int32_t* __restrict__ seq_len,
+token_head_kernel(const float* __restrict__ logits, const int32_t* __restrict__ labels, const int32_t* __restrict__ seq_len,
                   int32_t* __restrict__ pred_ids, float* __restrict__ d_logits, float* __restrict__ scratch, int rows,
-                  int L, int K, uint32_t k_magic) {
+                  int L, int K, uint32_t k_magic, Loss fn) {
   extern __shared__ float tile[];
   const int Kp = K | 1;
   const bool pad = (K & 1) == 0;
@@ -75,19 +155,7 @@ token_xent_kernel(const float* __restrict__ logits, const int32_t* __restrict__ 
       if (LABELS) {
         const int b = row / L, t = row - b * L;
         if (t < __ldg(seq_len + b)) {
-          const int y = __ldcs(labels + row);
-          const float zy = z[y];
-          float s = 0.f;
-          for (int j = 0; j < K; ++j) {
-            const float ej = expf(z[j] - m);
-            s += ej;
-            if (GRAD) z[j] = ej;
-          }
-          acc += (m - zy) + logf(s);
-          if (GRAD) {
-            const float inv = scale / s;
-            for (int j = 0; j < K; ++j) z[j] = z[j] * inv - (j == y ? scale : 0.f);
-          }
+          fn.template row<GRAD>(z, z + kRows * Kp, K, __ldcs(labels + row), m, arg, scale, acc);
         } else if (GRAD) {
           for (int j = 0; j < K; ++j) z[j] = 0.f;
         }
@@ -115,7 +183,7 @@ token_xent_kernel(const float* __restrict__ logits, const int32_t* __restrict__ 
 
 // loss[0] = (sum of the partials, in index order) / N, 0 when N = 0.
 __global__ void __launch_bounds__(256)
-token_xent_final_kernel(const float* __restrict__ scratch, int n_part, float* __restrict__ loss) {
+token_loss_final_kernel(const float* __restrict__ scratch, int n_part, float* __restrict__ loss) {
   __shared__ double part[256];
   double acc = 0.0;
   for (int i = threadIdx.x; i < n_part; i += 256) acc += (double)scratch[kScratchHead + i];
@@ -131,11 +199,52 @@ token_xent_final_kernel(const float* __restrict__ scratch, int n_part, float* __
   }
 }
 
-template <bool LABELS, bool GRAD>
-void launch_main(int grid, size_t smem, cudaStream_t st, const float* logits, const int32_t* labels, const int32_t* seq_len,
-                 int32_t* pred_ids, float* d_logits, float* scratch, int rows, int L, int K, uint32_t k_magic) {
-  token_xent_kernel<LABELS, GRAD><<<grid, kRows, smem, st>>>(logits, labels, seq_len, pred_ids, d_logits, scratch, rows, L,
-                                                             K, k_magic);
+template <class Loss, bool LABELS, bool GRAD>
+void launch_main(const Loss& fn, int grid, cudaStream_t st, const float* logits, const int32_t* labels,
+                 const int32_t* seq_len, int32_t* pred_ids, float* d_logits, float* scratch, int rows, int L, int K,
+                 uint32_t k_magic) {
+  const size_t smem = (size_t)(GRAD ? Loss::kGradTiles : 1) * kRows * (K | 1) * sizeof(float);
+  if (smem > 48 * 1024)       // above the default dynamic shared-memory limit (two tiles at K > 23)
+    cudaFuncSetAttribute(token_head_kernel<Loss, LABELS, GRAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  token_head_kernel<Loss, LABELS, GRAD><<<grid, kRows, smem, st>>>(logits, labels, seq_len, pred_ids, d_logits, scratch,
+                                                                   rows, L, K, k_magic, fn);
+}
+
+// Both entry points: validation in the order ner_b200.h documents, then the launches.  need_labels: the loss has no
+// argmax-only mode (ner_token_dice).
+template <class Loss>
+int token_head(const Loss& fn, bool need_labels, const float* logits, const int32_t* labels, const int32_t* seq_len,
+               int32_t* pred_ids, float* loss, float* d_logits, float d_loss, float* scratch, int B, int L, int K,
+               ner_stream_t stream) {
+  if (B < 0 || L < 1 || K < 1) return NER_ERR_INVALID_ARG;
+  if (K > NER_MAX_TAGS) return NER_ERR_UNSUPPORTED;
+  if ((long long)B * L > 0x7fffffffLL) return NER_ERR_UNSUPPORTED;
+  if (B == 0) return NER_OK;
+  if (!logits) return NER_ERR_INVALID_ARG;
+  const bool with_labels = labels != nullptr;
+  if (need_labels && !with_labels) return NER_ERR_INVALID_ARG;
+  if (!with_labels && (loss || d_logits)) return NER_ERR_INVALID_ARG;      // no labels: argmax only
+  if (with_labels && (!seq_len || !scratch)) return NER_ERR_INVALID_ARG;
+  if (!pred_ids && !loss && !d_logits) return NER_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int rows = B * L;
+  const int tiles = (rows + kRows - 1) / kRows;
+  const int grid = min(tiles, ner_num_sms() * kCtasPerSm);
+  const uint32_t k_magic = K > 1 ? 0xffffffffu / (uint32_t)K + 1u : 0u;
+  if (!with_labels) {
+    launch_main<XentLoss, false, false>(XentLoss{}, grid, st, logits, nullptr, nullptr, pred_ids, nullptr, nullptr,
+                                        rows, L, K, k_magic);
+    return ner_launch_status();
+  }
+  token_count_kernel<<<1, 1024, 0, st>>>(seq_len, B, L, d_loss, scratch);
+  if (d_logits)
+    launch_main<Loss, true, true>(fn, grid, st, logits, labels, seq_len, pred_ids, d_logits, scratch, rows, L, K,
+                                  k_magic);
+  else
+    launch_main<Loss, true, false>(fn, grid, st, logits, labels, seq_len, pred_ids, nullptr, scratch, rows, L, K,
+                                   k_magic);
+  if (loss) token_loss_final_kernel<<<1, 256, 0, st>>>(scratch, grid, loss);
+  return ner_launch_status();
 }
 
 }  // namespace
@@ -145,30 +254,13 @@ extern "C" size_t ner_token_xent_scratch_floats(void) { return (size_t)kScratchH
 extern "C" int ner_token_xent(const float* logits, const int32_t* labels, const int32_t* seq_len, int32_t* pred_ids,
                               float* loss, float* d_logits, float d_loss, float* scratch, int B, int L, int K,
                               ner_stream_t stream) {
-  if (B < 0 || L < 1 || K < 1) return NER_ERR_INVALID_ARG;
-  if (K > NER_MAX_TAGS) return NER_ERR_UNSUPPORTED;
-  if ((long long)B * L > 0x7fffffffLL) return NER_ERR_UNSUPPORTED;
-  if (B == 0) return NER_OK;
-  if (!logits) return NER_ERR_INVALID_ARG;
-  const bool with_labels = labels != nullptr;
-  if (!with_labels && (loss || d_logits)) return NER_ERR_INVALID_ARG;      // no labels: argmax only
-  if (with_labels && (!seq_len || !scratch)) return NER_ERR_INVALID_ARG;
-  if (!pred_ids && !loss && !d_logits) return NER_OK;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int rows = B * L;
-  const int tiles = (rows + kRows - 1) / kRows;
-  const int grid = min(tiles, ner_num_sms() * kCtasPerSm);
-  const size_t smem = (size_t)kRows * (K | 1) * sizeof(float);
-  const uint32_t k_magic = K > 1 ? 0xffffffffu / (uint32_t)K + 1u : 0u;
-  if (!with_labels) {
-    launch_main<false, false>(grid, smem, st, logits, nullptr, nullptr, pred_ids, nullptr, nullptr, rows, L, K, k_magic);
-    return ner_launch_status();
-  }
-  token_count_kernel<<<1, 1024, 0, st>>>(seq_len, B, L, d_loss, scratch);
-  if (d_logits)
-    launch_main<true, true>(grid, smem, st, logits, labels, seq_len, pred_ids, d_logits, scratch, rows, L, K, k_magic);
-  else
-    launch_main<true, false>(grid, smem, st, logits, labels, seq_len, pred_ids, nullptr, scratch, rows, L, K, k_magic);
-  if (loss) token_xent_final_kernel<<<1, 256, 0, st>>>(scratch, grid, loss);
-  return ner_launch_status();
+  return token_head(XentLoss{}, false, logits, labels, seq_len, pred_ids, loss, d_logits, d_loss, scratch, B, L, K, stream);
+}
+
+extern "C" int ner_token_dice(const float* logits, const int32_t* labels, const int32_t* seq_len, int32_t* pred_ids,
+                              float* loss, float* d_logits, float d_loss, float alpha, float gamma, float* scratch, int B,
+                              int L, int K, ner_stream_t stream) {
+  if (!(std::isfinite(alpha) && alpha >= 0.f && std::isfinite(gamma) && gamma > 0.f)) return NER_ERR_INVALID_ARG;
+  return token_head(DiceLoss{alpha, gamma}, true, logits, labels, seq_len, pred_ids, loss, d_logits, d_loss, scratch, B, L,
+                    K, stream);
 }

@@ -370,6 +370,16 @@ def softmax_xent(logits, labels, scale=1.0, want_grad=False):
 _token_xent_scratch = {}
 
 
+def _token_head_scratch(dev):
+    """The loss-partials buffer of ner_token_xent / ner_token_dice: one per (device, stream)."""
+    key = (dev.index, stream())
+    scratch = _token_xent_scratch.get(key)
+    if scratch is None:
+        scratch = _token_xent_scratch[key] = torch.empty(int(lib().ner_token_xent_scratch_floats()), dtype=torch.float32,
+                                                         device=dev)
+    return scratch
+
+
 def token_xent(logits, labels=None, seq_len=None, want_pred=True, want_loss=True, want_grad=False, d_loss=1.0):
     """Masked token cross-entropy + first argmax over logits [B, L, K<=32] f32 in one pass (ner_token_xent).
     -> (pred_ids [B,L] int32 | None, loss [] f32 | None, d_logits [B,L,K] | None).  labels None: argmax only.
@@ -386,15 +396,32 @@ def token_xent(logits, labels=None, seq_len=None, want_pred=True, want_loss=True
     pred = torch.empty((B, L), dtype=torch.int32, device=dev) if want_pred else None
     loss = torch.empty((), dtype=torch.float32, device=dev) if want_loss else None
     dz = torch.empty_like(logits) if want_grad else None
-    scratch = None
-    if labels is not None:
-        key = (dev.index, stream())
-        scratch = _token_xent_scratch.get(key)
-        if scratch is None:
-            scratch = _token_xent_scratch[key] = torch.empty(int(lib().ner_token_xent_scratch_floats()), dtype=torch.float32,
-                                                             device=dev)
+    scratch = _token_head_scratch(dev) if labels is not None else None
     check(lib().ner_token_xent(ptr(logits), ptr(labels), ptr(seq_len), ptr(pred), ptr(loss), ptr(dz), float(d_loss),
                                ptr(scratch), B, L, K, stream()))
+    if B == 0 and loss is not None:
+        loss.zero_()
+    if B == 0 and dz is not None:
+        dz.zero_()
+    return pred, loss, dz
+
+
+def token_dice(logits, labels, seq_len, alpha=1.0, gamma=1.0, want_pred=True, want_loss=True, want_grad=False, d_loss=1.0):
+    """Masked token self-adjusting Dice loss + first argmax over logits [B, L, K<=32] f32 in one pass (ner_token_dice).
+    -> (pred_ids [B,L] int32 | None, loss [] f32 | None, d_logits [B,L,K] | None), as token_xent.
+    loss = mean over t < seq_len of sum_k dice_k(softmax(z), label; alpha, gamma); d_logits = d_loss * its gradient, 0
+    past seq_len.  alpha >= 0, gamma > 0."""
+    require_cuda(logits, labels, seq_len)
+    assert logits.dtype == torch.float32 and logits.dim() == 3
+    B, L, K = logits.shape
+    dev = logits.device
+    labels, seq_len = _i32(labels), _i32(seq_len)
+    assert tuple(labels.shape) == (B, L) and tuple(seq_len.shape) == (B,)
+    pred = torch.empty((B, L), dtype=torch.int32, device=dev) if want_pred else None
+    loss = torch.empty((), dtype=torch.float32, device=dev) if want_loss else None
+    dz = torch.empty_like(logits) if want_grad else None
+    check(lib().ner_token_dice(ptr(logits), ptr(labels), ptr(seq_len), ptr(pred), ptr(loss), ptr(dz), float(d_loss),
+                               float(alpha), float(gamma), ptr(_token_head_scratch(dev)), B, L, K, stream()))
     if B == 0 and loss is not None:
         loss.zero_()
     if B == 0 and dz is not None:

@@ -437,6 +437,22 @@ int ner_softmax_xent(const float* logits, const int32_t* labels, float* loss, fl
 size_t ner_token_xent_scratch_floats(void);
 int ner_token_xent(const float* logits, const int32_t* labels, const int32_t* seq_len, int32_t* pred_ids, float* loss,
                    float* d_logits, float d_loss, float* scratch, int B, int L, int K, ner_stream_t stream);
+/* model/bert_dice.py + tools/loss.py: dice_loss and tf.argmax(logits, -1) in one pass over logits [B,L,K] f32, the same
+ * pass as ner_token_xent with the self-adjusting Dice loss (Li et al., "Dice Loss for Data-imbalanced NLP Tasks", ACL 2020)
+ * applied to every class of every token t < len_b.  With p = softmax(z), u_k = 1 - p_k, q_k = u_k^alpha * p_k (u^0 = 1):
+ *   l = sum_k l_k,  l_y = (1 - q_y) / (q_y + 1 + gamma),  l_k = q_k / (q_k + gamma) for k != y
+ *     (= 1 - (2 q_k [k=y] + gamma) / (q_k + [k=y] + gamma), the paper's form)
+ * loss [1] f32 (nullable) = sum_{t<len_b} l / N,  N = sum_b clamp(len_b, 0, L), 0 when N = 0.
+ * d_logits [B,L,K] f32 (nullable, fully written) = d_loss / N * d l / d z for t < len_b, 0 elsewhere, computed as
+ *   c_k = d l_k / d q_k * p_k * u_k^alpha * (u_k - alpha p_k),  r_k = c_k / s_{-k},  d l / d z_j = c_j - e_j (sum_k r_k - r_j)
+ * with e = exp(z - max z), s_{-k} = sum_{i != k} e_i and u_k = s_{-k} / sum e (never 1 - p_k, which is 0 in fp32 on a
+ * confident row).  pred_ids (nullable) as ner_token_xent.  labels, seq_len and scratch (ner_token_xent_scratch_floats())
+ * are required; alpha >= 0 and gamma > 0 finite, else NER_ERR_INVALID_ARG; otherwise the checks of ner_token_xent.
+ * Deterministic like ner_token_xent.  The reference's tools/loss.py is not in this repository: the loss, its token-mean
+ * reduction and the plugin's defaults alpha = gamma = 1 are a restatement of the paper, not pinned to the reference. */
+int ner_token_dice(const float* logits, const int32_t* labels, const int32_t* seq_len, int32_t* pred_ids, float* loss,
+                   float* d_logits, float d_loss, float alpha, float gamma, float* scratch, int B, int L, int K,
+                   ner_stream_t stream);
 /* dst[i] += a * src[i]. */
 int ner_axpy_f32(float* dst, const float* src, size_t n, float a, ner_stream_t stream);
 /* out[0] += sum(g^2)  (tf.clip_by_global_norm, tools/train_utils.py:315).  Deterministic (no float atomics): per-CTA partial
