@@ -13,14 +13,17 @@
 //   warpgroups 1-2 MMA + epilogue: warpgroup w owns rows 64(w-1) .. 64(w-1)+63 of the tile; per k-block four
 //                                 wgmma.m64nBNk16 from SWIZZLE_128B descriptors, fp32 accumulator in registers, one
 //                                 wgmma group kept in flight before the previous smem slot is released; then bias /
-//                                 GELU / residual straight from the accumulator fragment to global memory.
+//                                 GELU / residual in registers, the slice written in 8 KB column chunks (64 bf16 or
+//                                 32 fp32 columns x 64 rows) to a double-buffered SWIZZLE_128B staging buffer and
+//                                 stored by TMA (cp.async.bulk.tensor, bulk groups).  The warpgroup goes on to the
+//                                 next tile's k-blocks while the stores drain; TMA clips the M tail and N past the end.
 // While the MMA warpgroups run the epilogue of tile i the producer already fills the ring for tile i+1.
 //
-// Two variants:
-//   gemm_bf16_tc_kernel<BN, SK, 1>   128 x BN tile per CTA (BN = 64/128/192/256), optionally stream-K
-//   gemm_bf16_tc_kernel<BN, 0, 2>    a cluster of 2 CTAs computes a 256 x BN tile: each CTA stages its own 128 A rows
-//                                    and loads HALF of the B tile with TMA multicast into both CTAs, so the L2->smem
-//                                    bytes per FLOP drop by 1.5x vs the 128 x BN single-CTA tile.
+// Variants (EPI = the NER_EPI_* mode, a template parameter: no per-element mode test):
+//   gemm_bf16_tc_kernel<BN, SK, 1, EPI>   128 x BN tile per CTA (BN = 64/128/192/256), optionally stream-K
+//   gemm_bf16_tc_kernel<BN, 0, 2, EPI>    a cluster of 2 CTAs computes a 256 x BN tile: each CTA stages its own 128 A
+//                                         rows and loads HALF of the B tile with TMA multicast into both CTAs, so the
+//                                         L2->smem bytes per FLOP drop by 1.5x vs the 128 x BN single-CTA tile.
 #include <stdlib.h>
 
 #include <mutex>
@@ -40,22 +43,31 @@ constexpr int NUM_MMA_WG = 2;
 constexpr float kSkFixupCost = 10.0f;
 constexpr int NUM_THREADS = 128 * (1 + NUM_MMA_WG);
 
+// Output staging: per MMA warpgroup two 8 KB chunk buffers (64 rows of 128 B), so a chunk is written while the TMA store
+// of the previous one still reads its buffer.
+constexpr int OUT_CHUNK_BYTES = 64 * 128;
+constexpr int OUT_STAGE_BYTES = NUM_MMA_WG * 2 * OUT_CHUNK_BYTES;
+
 template <int BN>
 struct Cfg {
-  // 227 KB of shared memory per block: 4 x 48 KB (BN 256), 5 x 40 KB (192), 6 x 32 KB (128), 8 x 24 KB (64)
-  static constexpr int STAGES = (BN == 256) ? 4 : (BN == 192) ? 5 : ((BN == 128) ? 6 : 8);
+  // 227 KB of shared memory per block = ring + 32 KB output staging + barriers:
+  // 4 x 48 KB (BN 256), 4 x 40 KB (192: five stages would not leave room for the staging), 6 x 32 KB (128), 8 x 24 KB (64)
+  static constexpr int STAGES = (BN == 256 || BN == 192) ? 4 : ((BN == 128) ? 6 : 8);
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
-  // ring + barriers; the dynamic smem base is 1024-aligned (checked in-kernel)
-  static constexpr size_t SMEM = (size_t)STAGES * (A_BYTES + B_BYTES) + 256;
+  static constexpr int RING_BYTES = STAGES * (A_BYTES + B_BYTES);
+  // ring + staging + barriers; the dynamic smem base is 1024-aligned (checked in-kernel)
+  static constexpr size_t SMEM = (size_t)RING_BYTES + OUT_STAGE_BYTES + 256;
+  static_assert(SMEM <= 227 * 1024, "shared memory per block");
 };
 
 struct EpiArgs {
   const float* bias;      // [N] or null
-  const float* residual;  // [M,N] fp32 or null (EPI_RES_F32)
-  void* out;              // [M,N] bf16 or fp32
-  int mode;
+  const float* residual;  // [M,N] fp32 or null (EPI_RES_F32 / EPI_RES_RELU_F32)
 };
+
+template <int EPI>
+__host__ __device__ constexpr bool epi_f32() { return EPI == NER_EPI_F32 || EPI == NER_EPI_RES_F32 || EPI == NER_EPI_RES_RELU_F32; }
 
 __device__ __forceinline__ float gelu_tanh(float x) {
   // 0.5x(1+tanh(sqrt(2/pi)(x+0.044715x^3)))  (google-research/bert modeling.gelu).
@@ -141,13 +153,15 @@ template <int BN>
 struct Ring {
   uint8_t* a;
   uint8_t* b;
+  uint8_t* out;   // output staging, OUT_STAGE_BYTES (1024-aligned)
   uint64_t* full;
   uint64_t* empty;
   __device__ Ring(uint8_t* smem) {
     using C = Cfg<BN>;
     a = smem;
     b = smem + C::STAGES * C::A_BYTES;
-    full = reinterpret_cast<uint64_t*>(smem + C::STAGES * (C::A_BYTES + C::B_BYTES));
+    out = smem + C::RING_BYTES;
+    full = reinterpret_cast<uint64_t*>(out + OUT_STAGE_BYTES);
     empty = full + C::STAGES;
   }
 };
@@ -202,49 +216,114 @@ __device__ __forceinline__ void mma_kblocks(float (&acc)[BN / 2], const Ring<BN>
   }
 }
 
-// Fused epilogue of this thread's accumulator fragment (rows r, r + 8; column pairs 8 j + 2 (lane % 4)), written straight
-// to global memory.  `row_w` = first row of this warp's 16-row slice.
+// Activation of the epilogue, applied after bias (and residual) are added.
+template <int EPI>
+__device__ __forceinline__ float epi_act(float v) {
+  if constexpr (EPI == NER_EPI_GELU_TANH_BF16) return gelu_tanh(v);
+  else if constexpr (EPI == NER_EPI_GELU_ERF_BF16) return gelu_erf(v);
+  else if constexpr (EPI == NER_EPI_RELU_BF16 || EPI == NER_EPI_RES_RELU_F32) return fmaxf(v, 0.f);
+  else return v;
+}
+
+__device__ __forceinline__ void wg_bar_sync(int id) {  // named barrier `id` over the 128 threads of one warpgroup
+  asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory");
+}
+
+// Fused epilogue of one MMA warpgroup's 64 x BN slice (rows row_wg .., columns n0 ..) through shared memory and TMA.
+// Thread fragment: rows r, r + 8 (r = 16 warp + lane / 4), column pairs 8 j + 2 (lane % 4).  Chunk c of the slice (CW
+// columns, 64 rows, 128-B rows in the SWIZZLE_128B layout the store's tensor map expects: 16-B unit u of row r sits at
+// unit u ^ (r % 8)) is written into staging buffer `buf`, then one thread issues its TMA store as one bulk group.  A
+// buffer is rewritten only after the store issued from it two chunks earlier has finished reading it.
+template <int BN, int EPI>
+__device__ __forceinline__ void epilogue_tma(const float (&acc)[BN / 2], const EpiArgs& ep, const CUtensorMap* tma_out,
+                                             uint8_t* stage, uint32_t& buf, int row_wg, int n0, int M, int N) {
+  constexpr bool F32 = epi_f32<EPI>();
+  constexpr bool RES = EPI == NER_EPI_RES_F32 || EPI == NER_EPI_RES_RELU_F32;
+  constexpr int CW = F32 ? 32 : 64;   // columns per 8 KB chunk
+  constexpr int JPC = CW / 8;         // fragment column groups per chunk
+  const int t = threadIdx.x & 127, lane = t & 31, warp = t >> 5;
+  const int bar = 1 + (threadIdx.x >> 7);   // 2, 3 (1 = both MMA warpgroups)
+  const int r0 = 16 * warp + (lane >> 2);
+  if (row_wg >= M) return;   // the whole slice lies past M (tail of a 2-CTA tile)
+#pragma unroll
+  for (int c = 0; c < BN / CW; ++c) {
+    const int col0 = n0 + c * CW;
+    if (col0 >= N) break;
+    uint8_t* sb = stage + buf * OUT_CHUNK_BYTES;
+    if (t == 0) tma_store_wait_read<1>();
+    wg_bar_sync(bar);
+    float2 b[JPC];
+#pragma unroll
+    for (int jj = 0; jj < JPC; ++jj) {
+      const int col = col0 + 8 * jj + 2 * (lane & 3);
+      b[jj] = (ep.bias != nullptr && col < N) ? __ldg(reinterpret_cast<const float2*>(ep.bias + col)) : make_float2(0.f, 0.f);
+    }
+    if constexpr (F32) {
+#pragma unroll
+      for (int jj = 0; jj < JPC; ++jj) {
+        const int j = c * JPC + jj, col = col0 + 8 * jj + 2 * (lane & 3);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = r0 + 8 * h;
+          float v0 = acc[4 * j + 2 * h] + b[jj].x, v1 = acc[4 * j + 2 * h + 1] + b[jj].y;
+          if constexpr (RES) {
+            const int row = row_wg + r;
+            if (row < M && col < N) {
+              const float2 rv = *reinterpret_cast<const float2*>(ep.residual + (size_t)row * N + col);
+              v0 += rv.x;
+              v1 += rv.y;
+            }
+          }
+          v0 = epi_act<EPI>(v0);
+          v1 = epi_act<EPI>(v1);
+          const int unit = (2 * jj + ((lane & 3) >> 1)) ^ (r & 7);
+          *reinterpret_cast<float2*>(sb + r * 128 + unit * 16 + 8 * (lane & 1)) = make_float2(v0, v1);
+        }
+      }
+    } else {
+      // stmatrix x4: matrices (jj, rows r0), (jj, r0 + 8), (jj + 1, r0), (jj + 1, r0 + 8); lane gives a row of matrix lane / 8
+      const int i = lane >> 3, r = 16 * warp + 8 * (i & 1) + (lane & 7);
+      const uint32_t row_addr = smem_u32(sb) + r * 128;
+#pragma unroll
+      for (int jj = 0; jj < JPC; jj += 2) {
+        const int j = c * JPC + jj;
+        uint32_t p[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int jq = j + (q >> 1), h = q & 1;
+          const float2 bq = b[jj + (q >> 1)];
+          p[q] = pack_bf16x2(epi_act<EPI>(acc[4 * jq + 2 * h] + bq.x), epi_act<EPI>(acc[4 * jq + 2 * h + 1] + bq.y));
+        }
+        stmatrix_x4(row_addr + (((jj + (i >> 1)) ^ (r & 7)) << 4), p[0], p[1], p[2], p[3]);
+      }
+    }
+    fence_proxy_async();   // this thread's smem writes -> visible to the async proxy (the TMA store)
+    wg_bar_sync(bar);
+    if (t == 0) {
+      tma_store_2d(tma_out, sb, col0, row_wg);
+      tma_store_commit();
+    }
+    buf ^= 1u;
+  }
+}
+
+// dW += acc: the weight-gradient kernel's accumulate-into-gradient epilogue, straight from the accumulator fragment
+// (rows r, r + 8; column pairs 8 j + 2 (lane % 4)) to global memory.  `row_w` = first row of this warp's 16-row slice.
 template <int BN>
-__device__ __forceinline__ void epilogue_regs(const float (&acc)[BN / 2], const EpiArgs& ep, int row_w, int n0, int M,
-                                              int N) {
-  if (ep.mode == NER_EPI_DIAG_DISCARD) return;  // diagnostic: drain the accumulator, store nothing
+__device__ __forceinline__ void epilogue_accumulate(const float (&acc)[BN / 2], float* dw, int row_w, int n0, int M,
+                                                    int N) {
   const int lane = threadIdx.x & 31;
-  const bool f32 = ep.mode == NER_EPI_F32 || ep.mode == NER_EPI_RES_F32 || ep.mode == NER_EPI_RES_RELU_F32;
-  const bool res = ep.mode == NER_EPI_RES_F32 || ep.mode == NER_EPI_RES_RELU_F32;
 #pragma unroll
   for (int j = 0; j < BN / 8; ++j) {
     const int col = n0 + 8 * j + 2 * (lane & 3);
     if (col >= N) continue;
-    float2 b = make_float2(0.f, 0.f);
-    if (ep.bias != nullptr) b = __ldg(reinterpret_cast<const float2*>(ep.bias + col));
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int row = row_w + (lane >> 2) + 8 * h;
       if (row >= M) continue;
-      float v0 = acc[4 * j + 2 * h] + b.x, v1 = acc[4 * j + 2 * h + 1] + b.y;
-      const size_t off = (size_t)row * N + col;
-      if (res) {
-        const float2 r = *reinterpret_cast<const float2*>(ep.residual + off);
-        v0 += r.x;
-        v1 += r.y;
-        if (ep.mode == NER_EPI_RES_RELU_F32) {
-          v0 = fmaxf(v0, 0.f);
-          v1 = fmaxf(v1, 0.f);
-        }
-      } else if (ep.mode == NER_EPI_GELU_TANH_BF16) {
-        v0 = gelu_tanh(v0);
-        v1 = gelu_tanh(v1);
-      } else if (ep.mode == NER_EPI_GELU_ERF_BF16) {
-        v0 = gelu_erf(v0);
-        v1 = gelu_erf(v1);
-      } else if (ep.mode == NER_EPI_RELU_BF16) {
-        v0 = fmaxf(v0, 0.f);
-        v1 = fmaxf(v1, 0.f);
-      }
-      if (f32)
-        *reinterpret_cast<float2*>(static_cast<float*>(ep.out) + off) = make_float2(v0, v1);
-      else
-        *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(ep.out) + off) = pack_bf16x2(v0, v1);
+      float2* p = reinterpret_cast<float2*>(dw + (size_t)row * N + col);
+      const float2 r = *p;
+      *p = make_float2(acc[4 * j + 2 * h] + 0.f + r.x, acc[4 * j + 2 * h + 1] + 0.f + r.y);
     }
   }
 }
@@ -263,10 +342,10 @@ __device__ __forceinline__ void init_ring(const Ring<BN>& ring) {
 }
 
 // ===================================================================== main kernel
-template <int BN, bool SK, int CL>
+template <int BN, bool SK, int CL, int EPI>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_bf16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, EpiArgs ep,
-                    int M, int N, int K, SkArgs skargs) {
+gemm_bf16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
+                    const __grid_constant__ CUtensorMap tma_out, EpiArgs ep, int M, int N, int K, SkArgs skargs) {
   using C = Cfg<BN>;
   constexpr int STAGES = C::STAGES;
   nerdev::pdl_launch_dependents();   // the next kernel of the stream may start its prologue while this one runs
@@ -288,6 +367,7 @@ gemm_bf16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tma_a);
     tma_prefetch_desc(&tma_b);
+    tma_prefetch_desc(&tma_out);
   }
   init_ring<BN, CL>(ring);
   if constexpr (CL == 2) cluster_sync_all();  // barrier inits visible cluster-wide before any multicast / remote arrive
@@ -324,7 +404,8 @@ gemm_bf16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
     setmaxnreg_inc<232>();
     const int mw = wg - 1;                      // 64-row slice of the tile
     const int ctid = threadIdx.x - 128;         // 0 .. 255
-    const int row_in_tile = mw * 64 + ((threadIdx.x >> 5) & 3) * 16;
+    uint8_t* stage = ring.out + mw * 2 * OUT_CHUNK_BYTES;
+    uint32_t buf = 0;
     uint32_t empty_peer[STAGES];
 #pragma unroll
     for (int s = 0; s < STAGES; ++s) empty_peer[s] = CL == 2 ? mapa_u32(smem_u32(&ring.empty[s]), rank ^ 1u) : 0u;
@@ -378,13 +459,24 @@ gemm_bf16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
           }
         }
       }
-      epilogue_regs<BN>(acc, ep, row0 + row_in_tile, n_blk * BN, M, N);
+      if constexpr (EPI == NER_EPI_DIAG_DISCARD) {
+        // diagnostic mode: store nothing, yet keep the accumulator live, or the compiler drops the wgmma of this
+        // instantiation and the mode would time the loads only.  The smem write is under a condition no launch meets
+        // (M >= 1 is checked on the host) but which the compiler cannot rule out.
+        if (M < 0) {
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) reinterpret_cast<float*>(ring.a)[i * 256 + ctid] = acc[i];
+        }
+      } else {
+        epilogue_tma<BN, EPI>(acc, ep, &tma_out, stage, buf, row0 + mw * 64, n_blk * BN, M, N);
+      }
       if (n_part > 0) {
         mma_bar_sync();   // every MMA thread has consumed the parked partials
         if (ctid < 32)
           for (int c = ctid; c < n_part; c += 32) skargs.flags[c_first + c] = 0;
       }
     }
+    if ((threadIdx.x & 127) == 0) tma_store_wait_all();   // staging stays valid until this warpgroup's stores are done
   }
   if constexpr (CL == 2) cluster_sync_all();  // no CTA leaves while its peer may still multicast into it / arrive on it
 }
@@ -472,8 +564,7 @@ gemm_wgrad_group_kernel(const __grid_constant__ WgradGroup grp) {
       int p, m_blk, n_blk;
       locate(tile, p, m_blk, n_blk);
       mma_kblocks<BN, STAGES, 1, 1, 1>(acc, ring, pos, 0, num_kb, (uint32_t)(mw * BOX), da, db, no_peer);
-      const EpiArgs ep{nullptr, grp.dw[p], grp.dw[p], NER_EPI_RES_F32};
-      epilogue_regs<BN>(acc, ep, m_blk * BM + row_in_tile, n_blk * BN, grp.m[p], grp.n[p]);
+      epilogue_accumulate<BN>(acc, grp.dw[p], m_blk * BM + row_in_tile, n_blk * BN, grp.m[p], grp.n[p]);
     }
   }
 }
@@ -498,17 +589,18 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// bf16 row-major [rows, cols] with a {64, box_rows} box, 128-byte swizzle.
-int make_map_bf16_2d(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+// Row-major [rows, cols] of bf16 (f32 = false) or fp32 with a {box_cols, box_rows} box of 128-B rows, 128-byte swizzle.
+int make_map_2d(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows, bool f32 = false) {
   EncodeTiledFn fn = get_encode_fn();
   if (fn == nullptr) return NER_ERR_NO_DRIVER;
+  const uint32_t esz = f32 ? 4 : 2;
   cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {cols * 2};
-  cuuint32_t box[2] = {(cuuint32_t)BK, box_rows};
+  cuuint64_t strides[1] = {cols * esz};
+  cuuint32_t box[2] = {128 / esz, box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = fn(map, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr),
+                  dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? NER_OK : NER_ERR_INVALID_ARG;
 }
 
@@ -595,12 +687,14 @@ cudaError_t launch_ex(void (*kern)(KArgs...), int grid, size_t smem, cudaStream_
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 
-template <int BN, int CL>
-int launch_gemm(const void* A, const void* Wt, EpiArgs ep, int M, int N, int K, cudaStream_t st, bool sk = false) {
-  CUtensorMap ma, mb;
-  int rc = make_map_bf16_2d(&ma, A, (uint64_t)M, (uint64_t)K, BM);
+template <int BN, int CL, int EPI>
+int launch_gemm(const void* A, const void* Wt, EpiArgs ep, void* out, int M, int N, int K, cudaStream_t st, bool sk) {
+  CUtensorMap ma, mb, mo;
+  int rc = make_map_2d(&ma, A, (uint64_t)M, (uint64_t)K, BM);
   if (rc != NER_OK) return rc;
-  rc = make_map_bf16_2d(&mb, Wt, (uint64_t)N, (uint64_t)K, BN / CL);
+  rc = make_map_2d(&mb, Wt, (uint64_t)N, (uint64_t)K, BN / CL);
+  if (rc != NER_OK) return rc;
+  rc = make_map_2d(&mo, out, (uint64_t)M, (uint64_t)N, 64, epi_f32<EPI>());   // one warpgroup's 64-row chunk
   if (rc != NER_OK) return rc;
   const size_t smem = Cfg<BN>::SMEM;
   const int tiles = ((M + CL * BM - 1) / (CL * BM)) * ((N + BN - 1) / BN);
@@ -608,36 +702,47 @@ int launch_gemm(const void* A, const void* Wt, EpiArgs ep, int M, int N, int K, 
   SkArgs ska{nullptr, nullptr};
   cudaError_t e;
   if constexpr (CL == 1) {
-    // stream-K needs every CTA co-resident (grid = #SMs) and at least one k-block unit per CTA
-    sk = sk && (long long)tiles * num_kb >= sm_count() && ep.mode != NER_EPI_DIAG_DISCARD && sk_scratch(st, &ska);
-    if (sk)
-      e = launch_ex(gemm_bf16_tc_kernel<BN, true, 1>, sm_count(), smem, st, 1, ma, mb, ep, M, N, K, ska);
-    else
-      e = launch_ex(gemm_bf16_tc_kernel<BN, false, 1>, tiles < sm_count() ? tiles : sm_count(), smem, st, 1, ma, mb, ep,
-                    M, N, K, ska);
+    // stream-K (128 x 128 / 128 x 256 tiles) needs every CTA co-resident (grid = #SMs) and at least one k-block unit per CTA
+    if constexpr ((BN == 256 || BN == 128) && EPI != NER_EPI_DIAG_DISCARD) {
+      if (sk && (long long)tiles * num_kb >= sm_count() && sk_scratch(st, &ska)) {
+        e = launch_ex(gemm_bf16_tc_kernel<BN, true, 1, EPI>, sm_count(), smem, st, 1, ma, mb, mo, ep, M, N, K, ska);
+        if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
+        return ner_launch_status();
+      }
+    }
+    e = launch_ex(gemm_bf16_tc_kernel<BN, false, 1, EPI>, tiles < sm_count() ? tiles : sm_count(), smem, st, 1, ma, mb, mo,
+                  ep, M, N, K, ska);
   } else {
     const int max_pairs = sm_count() / 2;
     const int pairs = tiles < max_pairs ? tiles : max_pairs;
-    e = launch_ex(gemm_bf16_tc_kernel<BN, false, 2>, 2 * pairs, smem, st, 2, ma, mb, ep, M, N, K, ska);
+    e = launch_ex(gemm_bf16_tc_kernel<BN, false, 2, EPI>, 2 * pairs, smem, st, 2, ma, mb, mo, ep, M, N, K, ska);
   }
   if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
   return ner_launch_status();
+}
+
+// The epilogue mode is a template parameter of the kernel: one instantiation per (tile, mode).
+template <int BN, int CL>
+int launch_gemm(const void* A, const void* Wt, EpiArgs ep, void* out, int M, int N, int K, int epilogue, cudaStream_t st,
+                bool sk = false) {
+  switch (epilogue) {
+    case NER_EPI_F32: return launch_gemm<BN, CL, NER_EPI_F32>(A, Wt, ep, out, M, N, K, st, sk);
+    case NER_EPI_BF16: return launch_gemm<BN, CL, NER_EPI_BF16>(A, Wt, ep, out, M, N, K, st, sk);
+    case NER_EPI_GELU_TANH_BF16: return launch_gemm<BN, CL, NER_EPI_GELU_TANH_BF16>(A, Wt, ep, out, M, N, K, st, sk);
+    case NER_EPI_GELU_ERF_BF16: return launch_gemm<BN, CL, NER_EPI_GELU_ERF_BF16>(A, Wt, ep, out, M, N, K, st, sk);
+    case NER_EPI_RELU_BF16: return launch_gemm<BN, CL, NER_EPI_RELU_BF16>(A, Wt, ep, out, M, N, K, st, sk);
+    case NER_EPI_RES_F32: return launch_gemm<BN, CL, NER_EPI_RES_F32>(A, Wt, ep, out, M, N, K, st, sk);
+    case NER_EPI_RES_RELU_F32: return launch_gemm<BN, CL, NER_EPI_RES_RELU_F32>(A, Wt, ep, out, M, N, K, st, sk);
+    case NER_EPI_DIAG_DISCARD: return launch_gemm<BN, CL, NER_EPI_DIAG_DISCARD>(A, Wt, ep, out, M, N, K, st, sk);
+    default: return NER_ERR_INVALID_ARG;
+  }
 }
 
 }  // namespace
 
 // bf16 row-major [rows, cols] with a {64 columns, 64 rows} box, 128-byte swizzle (MN-major operand tiles).
 static int make_map_bf16_box64(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols) {
-  EncodeTiledFn fn = get_encode_fn();
-  if (fn == nullptr) return NER_ERR_NO_DRIVER;
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {cols * 2};
-  cuuint32_t box[2] = {64, 64};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? NER_OK : NER_ERR_INVALID_ARG;
+  return make_map_2d(map, ptr, rows, cols, 64);
 }
 
 extern "C" int ner_wgrad_group_bf16(const ner_wgrad_problem* problems_host, int count, int rows, ner_stream_t stream) {
@@ -693,7 +798,7 @@ extern "C" int ner_gemm_bf16(const void* A, const void* Wt, const float* bias, c
     return NER_ERR_INVALID_ARG;
   // the epilogue reads bias and residual as float2 column pairs
   if ((reinterpret_cast<uintptr_t>(bias) & 7) || (reinterpret_cast<uintptr_t>(residual) & 7)) return NER_ERR_INVALID_ARG;
-  EpiArgs ep{bias, residual, out, epilogue};
+  EpiArgs ep{bias, residual};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   int bn = tile_n;
   bool sk = false;
@@ -708,7 +813,10 @@ extern "C" int ner_gemm_bf16(const void* A, const void* Wt, const float* bias, c
     // Cost model in units of one 128x256 k-block per CTA.  Whole-tile scheduling: ceil(tiles/SMs) waves
     // of num_kb k-blocks times the relative k-block cost of the tile width (narrower tiles re-read the A
     // tile more often per FLOP).  Stream-K (128x256 tiles): every CTA gets ceil(tiles*num_kb/SMs) k-blocks
-    // plus a fixed charge for parking / adding one partial accumulator.
+    // plus a fixed charge for parking / adding one partial accumulator.  Re-checked on an H100 SXM (400 W limit) with the
+    // TMA-store epilogue over the encoder shapes at 3549 and 12202 rows (scripts/bench_kernels.py gemm): it picks the
+    // fastest of 128 / 192 / 256 within 3 % (the run-to-run spread) in all ten, and stream-K, 15-72 % slower there, is
+    // never chosen.
     const int mt = (M + BM - 1) / BM, sms = sm_count(), num_kb = (K + BK - 1) / BK;
     const int cand[3] = {256, 192, 128};
     const float cost[3] = {1.00f, 0.80f, 0.64f};
@@ -733,12 +841,12 @@ extern "C" int ner_gemm_bf16(const void* A, const void* Wt, const float* bias, c
     }
   }
   switch (bn) {
-    case 256: return launch_gemm<256, 1>(A, Wt, ep, M, N, K, st, sk);
-    case 192: return launch_gemm<192, 1>(A, Wt, ep, M, N, K, st);
-    case 128: return launch_gemm<128, 1>(A, Wt, ep, M, N, K, st, sk);
-    case 64: return launch_gemm<64, 1>(A, Wt, ep, M, N, K, st);
-    case NER_TILE_2CTA_256: return launch_gemm<256, 2>(A, Wt, ep, M, N, K, st);
-    case NER_TILE_2CTA_128: return launch_gemm<128, 2>(A, Wt, ep, M, N, K, st);
+    case 256: return launch_gemm<256, 1>(A, Wt, ep, out, M, N, K, epilogue, st, sk);
+    case 192: return launch_gemm<192, 1>(A, Wt, ep, out, M, N, K, epilogue, st);
+    case 128: return launch_gemm<128, 1>(A, Wt, ep, out, M, N, K, epilogue, st, sk);
+    case 64: return launch_gemm<64, 1>(A, Wt, ep, out, M, N, K, epilogue, st);
+    case NER_TILE_2CTA_256: return launch_gemm<256, 2>(A, Wt, ep, out, M, N, K, epilogue, st);
+    case NER_TILE_2CTA_128: return launch_gemm<128, 2>(A, Wt, ep, out, M, N, K, epilogue, st);
     default: return NER_ERR_INVALID_ARG;
   }
 }

@@ -92,6 +92,16 @@ template <int N>
 __device__ __forceinline__ void tma_store_wait_read() {
   asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
+// all bulk groups of this thread have completed (their global writes are performed)
+__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
+// Four 8x8 b16 matrices to shared memory; lanes 8i .. 8i+7 give the row addresses of matrix i, register i holds this
+// thread's pair of matrix i (row lane / 4, columns 2 (lane % 4) + {0, 1}) — the layout of a wgmma accumulator 8x8 block.
+__device__ __forceinline__ void stmatrix_x4(uint32_t smem_addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(smem_addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
+}
 
 // ---------------------------------------------------------------- TMA multicast (cluster)
 // 2-D tiled load delivered to the same smem offset in every CTA of `cta_mask`; each destination CTA's barrier at the
