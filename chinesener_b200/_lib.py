@@ -72,6 +72,9 @@ SIGNATURES = {
     "ner_split_bf16": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "ner_attention_f32": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _c.c_float, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "ner_softlexicon_pool_bwd": (_i, [_vp] * 4 + [_i] * 5 + [_vp]),
+    "ner_multihot_embed_fwd": (_i, [_vp] * 3 + [_i] * 4 + [_vp]),
+    "ner_small_table_grad_scratch_floats": (_c.c_size_t, [_i, _i]),
+    "ner_small_table_grad": (_i, [_vp] * 4 + [_i] * 4 + [_vp, _vp]),
 }
 
 

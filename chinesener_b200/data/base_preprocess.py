@@ -24,16 +24,17 @@ def extract_prefix_surfix(model_name):
 
 
 def get_instance(tokenizer_type, max_seq_len, tag2idx, tokenizer, word_enhance=None, **kwargs):
-    """reference :75-93 — the processor class for a word-enhance method.  Only the methods whose plugins are in scope
-    are built (None -> BasicProc, softlexicon -> SoftLexiconProc); the tokenizer object is passed in instead of being
+    """reference :75-93 — the processor class for a word-enhance method (None -> BasicProc, softlexicon ->
+    SoftLexiconProc(vocab), bichar -> BiCharProc(bichar_tokenizer), softword -> SoftWordProc(cut), ex_softword ->
+    ExSoftWordProc(vocab)); the tokenizer object and the method's keyword arguments are passed in instead of being
     looked up by name because vocabularies / vectors live wherever the caller keeps them."""
     assert word_enhance in [None] + WordEnhanceMethod, 'word_enhance must in {}'.format(','.join(WordEnhanceMethod))
     if word_enhance is None:
         return BasicProc(tokenizer_type, max_seq_len, tag2idx, tokenizer)
-    if word_enhance == SoftLexicon:
-        from .word_enhance import SoftLexiconProc
-        return SoftLexiconProc(tokenizer_type, max_seq_len, tag2idx, tokenizer, **kwargs)
-    raise NotImplementedError('word_enhance={} plugins are out of scope (SURVEY 8)'.format(word_enhance))
+    from . import word_enhance as we
+    cls = {SoftLexicon: we.SoftLexiconProc, BiChar: we.BiCharProc, SoftWord: we.SoftWordProc,
+           ExSoftWord: we.ExSoftWordProc}[word_enhance]
+    return cls(tokenizer_type, max_seq_len, tag2idx, tokenizer, **kwargs)
 
 
 class BasicProc(object):

@@ -9,14 +9,17 @@ TFRecords.
 
     python -m chinesener_b200.data.preprocess --src <dir with train/ val/ test/> --out datasets/msra \
         --tokenizer giga --giga_vec <gigaword .vec>  [--bert_vocab <vocab.txt>]
+        [--word_enhance bichar --bichar_vec <bigram .vec> | --word_enhance ex_softword --word_vec <word .vec>
+         | --word_enhance softword]
 """
 import argparse
 import os
 import pickle
 
-from .base_preprocess import get_instance
+from .base_preprocess import BiChar, ExSoftWord, SoftWord, get_instance
 from .records import write_records
-from .tokenizer import TokenizerBert, TokenizerGiga, get_bert_tokenizer, get_giga_tokenizer
+from .tokenizer import TextVectors, TokenizerBert, TokenizerGiga, get_bert_tokenizer, get_giga_tokenizer
+from .word_enhance import WordVocab
 
 # data/msra/preprocess.py:7-27 (people_daily uses the same tag set and length)
 MSRA_TAG2IDX = {'[PAD]': 0, 'O': 1, 'B-ORG': 2, 'I-ORG': 3, 'B-PER': 4, 'I-PER': 5, 'B-LOC': 6, 'I-LOC': 7, '[CLS]': 8, '[SEP]': 9}
@@ -63,9 +66,10 @@ def load_data(data_dir, file_name):
 
 
 def dump_records(proc, src_dir, out_dir, file_name, mapping=MAPPING, word_enhance=None, embedding=None, verbose=True,
-                 load_data=None):
+                 load_data=None, bichar_embedding=None):
     """One split through `proc.build_feature` -> `<out_dir>/<tokenizer>_<renamed>[_<enhance>].nerrec`; the train split
-    also writes `<tokenizer>[_<enhance>]_data_params.pkl` (data/base_preprocess.py:206-227, 247-253)."""
+    also writes `<tokenizer>[_<enhance>]_data_params.pkl` (data/base_preprocess.py:206-227, 247-253), with the bigram
+    table as `bichar_embedding` when one is given."""
     sentences, tags = (load_data or globals()['load_data'])(src_dir, file_name)
     feats, n_invalid = [], 0
     for sentence, tag in zip(sentences, tags):
@@ -84,12 +88,14 @@ def dump_records(proc, src_dir, out_dir, file_name, mapping=MAPPING, word_enhanc
         params = proc.build_data_params(len(feats))
         if proc.tokenizer_type == TokenizerGiga and embedding is not None:
             params['embedding'] = embedding
+        if bichar_embedding is not None:
+            params['bichar_embedding'] = bichar_embedding
         with open(os.path.join(out_dir, '_'.join(filter(None, [proc.tokenizer_type, word_enhance, 'data_params.pkl']))), 'wb') as f:
             pickle.dump(params, f)
     return len(feats), n_invalid
 
 
-def main():
+def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument('--src', required=True, help='directory holding train/ val/ test/ with sentences.txt + tags.txt')
     ap.add_argument('--out', required=True)
@@ -99,18 +105,32 @@ def main():
     ap.add_argument('--max_seq_len', type=int, default=MSRA_MAX_SEQ_LEN)
     ap.add_argument('--seed', type=int, default=1234, help='seed of the two add-on embedding rows ([PAD], [UNK])')
     ap.add_argument('--format', default='ner', choices=['ner', 'msr'], help="'msr': word-segmented msr_<split>.utf8 files (CWS tags)")
-    args = ap.parse_args()
+    ap.add_argument('--word_enhance', default=None, choices=[BiChar, SoftWord, ExSoftWord],
+                    help='extra input of the bilstm_crf_<word_enhance> plugins (giga tokenizer); softword segments with jieba')
+    ap.add_argument('--bichar_vec', default='./pretrain_model/giga/gigaword_chn.all.a2b.bi.ite50.vec',
+                    help='bigram vectors (giga .vec format) for --word_enhance bichar')
+    ap.add_argument('--word_vec', default='./pretrain_model/ctb50/ctb.50d.vec',
+                    help='word vectors (giga .vec format) whose vocabulary is the lexicon of --word_enhance ex_softword')
+    args = ap.parse_args(argv)
     if args.tokenizer == TokenizerGiga:
         tok = get_giga_tokenizer(args.giga_vec)
         emb = tok.embedding(args.seed)
     else:
         tok, emb = get_bert_tokenizer(args.bert_dir), None
     msr = args.format == 'msr'
-    proc = get_instance(args.tokenizer, args.max_seq_len, MSR_TAG2IDX if msr else MSRA_TAG2IDX, tok)
+    kwargs, bichar_emb = {}, None
+    if args.word_enhance == BiChar:
+        kwargs['bichar_tokenizer'] = get_giga_tokenizer(args.bichar_vec)
+        bichar_emb = kwargs['bichar_tokenizer'].embedding(args.seed)
+    elif args.word_enhance == ExSoftWord:
+        words = TextVectors(args.word_vec).index2word
+        kwargs['vocab'] = WordVocab(words, dict.fromkeys(words, 1))
+    proc = get_instance(args.tokenizer, args.max_seq_len, MSR_TAG2IDX if msr else MSRA_TAG2IDX, tok,
+                        word_enhance=args.word_enhance, **kwargs)
     for file in (MSR_MAPPING if msr else MAPPING):
         print('Dumping records for {} tokenizer = {}'.format(file, args.tokenizer))
         dump_records(proc, args.src, args.out, file, mapping=MSR_MAPPING if msr else MAPPING, embedding=emb,
-                     load_data=load_msr_data if msr else None)
+                     load_data=load_msr_data if msr else None, word_enhance=args.word_enhance, bichar_embedding=bichar_emb)
 
 
 if __name__ == '__main__':

@@ -1,5 +1,13 @@
 # -*-coding:utf-8 -*-
-"""SoftLexicon host side (SURVEY §8(f) rank 3) — the step just before the gather-and-pool kernel (ner_softlexicon_pool_fwd).
+"""Word-enhance featurisation of the giga character models: SoftLexicon, and the BiChar / Softword / ExSoftword inputs.
+
+BiChar / Softword / ExSoftword (`BiCharProc`, `SoftWordProc`, `ExSoftWordProc`, after Ma et al., "Simplify the Usage of
+Lexicon in Chinese NER", ACL 2020, and the bigram input of TENER) are restatements: the reference's own
+data/word_enhance.py is not in this repository, so the bigram end marker, the segmentation label-to-id maps and the
+ExSoftword multi-hot layout below are this project's choices, not pinned to it.  All three follow the giga tokenizer's
+characters (whitespace dropped); word-piece alignment for the BERT tokenizer is not built.
+
+SoftLexicon host side (SURVEY §8(f) rank 3) — the step just before the gather-and-pool kernel (ner_softlexicon_pool_fwd).
 
 The matching itself (reference data/word_enhance.py:302-337 build_soft_lexicon, :89-119 align_with_token, :163-205
 postproc_soft_lexicon, data/base_preprocess.py:397-412 format_soft_seq) runs in C++ behind the C-ABI
@@ -122,3 +130,116 @@ class SoftLexiconProc(BasicProc):
         params = super(SoftLexiconProc, self).build_data_params(n_sample)
         params.update({'word_enhance_dim': len(SoftKeys), 'max_lexicon_len': MaxLexiconLen, 'vocab2idx': self.vocab.vocab2idx})
         return params
+
+
+# ----------------------------------------------------------------------------- BiChar / Softword / ExSoftword
+BiCharEnd = '-null-'                 # pairs with the last character (the end key of the giga bigram vectors' convention)
+SoftWordIds = {'B': 1, 'M': 2, 'E': 3, 'S': 4}        # softword_ids; 0 = no label / [PAD]
+ExSoftWordKeys = SoftKeys + ('None',)                   # ex_softword_ids columns
+
+
+def giga_chars(sentence):
+    """The characters the giga tokenizer keeps (whitespace dropped), full-width folded as TokenizerAdapter does."""
+    from .tokenizer import TokenizerAdapter
+    return [TokenizerAdapter.full2half(c) for c in sentence if c.strip()]
+
+
+def _reject_bert(tokenizer_type, name):
+    if tokenizer_type == TokenizerBert:
+        raise ValueError('{} follows the giga tokenizer\'s characters; BERT word-piece alignment is not built'.format(name))
+
+
+class BiCharProc(BasicProc):
+    """BasicProc + bichar_ids [L] int32: character j's bigram is c_j c_{j+1}, the last character's is c_n + '-null-'.
+    `bichar_tokenizer` is a TokenizerAdapter over bigram vectors (get_giga_tokenizer(<bigram .vec>)): out-of-vocabulary
+    bigrams are [UNK], positions past seq_len [PAD].  The caller stores the bigram table as params['bichar_embedding']."""
+
+    def __init__(self, tokenizer_type, max_seq_len, tag2idx, tokenizer, bichar_tokenizer):
+        _reject_bert(tokenizer_type, 'BiCharProc')
+        super(BiCharProc, self).__init__(tokenizer_type, max_seq_len, tag2idx, tokenizer)
+        self.bichar_tokenizer = bichar_tokenizer
+        self.word_enhance = 'bichar'
+
+    def bigrams(self, sentence):
+        chars = giga_chars(sentence)
+        vocab = self.bichar_tokenizer.vocab2idx
+        grams = [a + b for a, b in zip(chars, chars[1:] + [BiCharEnd])]
+        return [g if g in vocab else '[UNK]' for g in grams]
+
+    def build_seq_feature(self, sentence):
+        f = super(BiCharProc, self).build_seq_feature(sentence)
+        grams, _ = self.format_sequence(self.bigrams(sentence))
+        f['bichar_ids'] = self.bichar_tokenizer.convert_tokens_to_ids(grams)
+        return f
+
+
+def ex_softword_from_lexicon(ids, seq_len, none_id, max_seq_len):
+    """NativeLexicon.build ids [n, L * 40] -> ex_softword_ids float32 [n, L * 5]: per character the multi-hot of the
+    B/M/E/S sets its lexicon match holds (a set is non-empty when its first slot is not <None>), None when all four are
+    empty; rows at or past seq_len are zero."""
+    n = ids.shape[0]
+    first = ids.reshape(n, max_seq_len, len(SoftKeys), MaxLexiconLen)[..., 0]          # [n, L, 4]
+    out = np.zeros((n, max_seq_len, len(ExSoftWordKeys)), np.float32)
+    out[..., :len(SoftKeys)] = first != none_id
+    out[..., len(SoftKeys)] = ~out[..., :len(SoftKeys)].any(-1)
+    out[np.arange(max_seq_len)[None, :] >= np.asarray(seq_len)[:, None]] = 0
+    return out.reshape(n, -1)
+
+
+class ExSoftWordProc(BasicProc):
+    """BasicProc + ex_softword_ids [L * 5] float32 (ExSoftword: the multi-hot B/M/E/S/None label set of every character,
+    from the SoftLexicon match against `vocab`, a WordVocab)."""
+
+    def __init__(self, tokenizer_type, max_seq_len, tag2idx, tokenizer, vocab, vocabfreq=None):
+        _reject_bert(tokenizer_type, 'ExSoftWordProc')
+        super(ExSoftWordProc, self).__init__(tokenizer_type, max_seq_len, tag2idx, tokenizer)
+        self.vocab, self.word_enhance = vocab, 'ex_softword'
+        self.lexicon = NativeLexicon(vocab, vocabfreq)
+
+    def build_seq_features(self, sentences, n_threads=0):
+        feats = [super(ExSoftWordProc, self).build_seq_feature(s) for s in sentences]
+        ids, _ = self.lexicon.build(sentences, self.max_seq_len, False, None, n_threads)
+        ex = ex_softword_from_lexicon(ids, [f['seq_len'] for f in feats], self.vocab.vocab2idx[WordVocab.none_token],
+                                      self.max_seq_len)
+        for f, x in zip(feats, ex):
+            f['ex_softword_ids'] = x.tolist()
+        return feats
+
+    def build_seq_feature(self, sentence):
+        return self.build_seq_features([sentence], n_threads=1)[0]
+
+
+def softword_labels(words):
+    """Segmented words -> one B/M/E/S id per character (SoftWordIds)."""
+    out = []
+    for w in words:
+        n = len(w)
+        out += [SoftWordIds['S']] if n == 1 else [SoftWordIds['B']] + [SoftWordIds['M']] * (n - 2) + [SoftWordIds['E']]
+    return out
+
+
+class SoftWordProc(BasicProc):
+    """BasicProc + softword_ids [L] int32: the B/M/E/S label (SoftWordIds) a word segmenter gives each character.
+    `cut(sentence) -> iterable of words` segments the whitespace-stripped sentence; without one, jieba.cut is used when
+    jieba is installed."""
+
+    def __init__(self, tokenizer_type, max_seq_len, tag2idx, tokenizer, cut=None):
+        _reject_bert(tokenizer_type, 'SoftWordProc')
+        super(SoftWordProc, self).__init__(tokenizer_type, max_seq_len, tag2idx, tokenizer)
+        if cut is None:
+            try:
+                import jieba
+            except ImportError:
+                raise ImportError('SoftWordProc needs a word segmenter: pass cut=<sentence -> words> or install jieba')
+            cut = jieba.cut
+        self.cut, self.word_enhance = cut, 'softword'
+
+    def build_seq_feature(self, sentence):
+        f = super(SoftWordProc, self).build_seq_feature(sentence)
+        text = ''.join(c for c in sentence if c.strip())
+        words = [w for w in self.cut(text) if w]
+        if sum(len(w) for w in words) != len(text):
+            raise ValueError('segmenter output does not cover the sentence {}...'.format(text[:10]))
+        labels = softword_labels(words)[:self.max_seq_len]
+        f['softword_ids'] = labels + [0] * (self.max_seq_len - len(labels))
+        return f

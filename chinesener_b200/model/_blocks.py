@@ -1,10 +1,15 @@
 """Shared pieces of the plugin graphs.  Every plugin keeps the reference contract — `build_graph(features, labels, params,
 is_training) -> (loss, pred_ids)` plus a module-level `TRAIN_PARAMS` — and composes these blocks; the blocks call the
 reference-shaped layer functions of `tools/layer.py`, which hold the kernels."""
+import numpy as np
 import torch
 
+from .. import autodiff, ops, variables
 from ..config import TRAIN_PARAMS as BASE_TRAIN_PARAMS
 from ..tools import layer as L
+
+SOFTWORD_TABLE = 'word_enhance/softword_embedding'
+SOFTWORD_LABELS = 5                  # softword: none/[PAD], B, M, E, S; ex_softword: B, M, E, S, None
 
 
 def hyper(*groups, **overrides):
@@ -42,6 +47,41 @@ def recurrent(x, features, params, is_training):
     """The bidirectional LSTM block configured by the plugin's RNN hyper-parameters."""
     return L.bilstm(x, params['cell_type'], params['rnn_activation'], params['hidden_units_list'], params['keep_prob_list'],
                     params['cell_size'], features['seq_len'], params['dtype'], is_training)
+
+
+def bilstm_crf_tail(embedding, features, params, is_training):
+    """bilstm_crf's graph after the embedding: dropout -> BiLSTM -> dropout -> label projection -> CRF."""
+    rate = params['embedding_dropout']
+    hidden = recurrent(L.dropout(embedding, rate=rate, is_training=is_training, seed=1234), features, params, is_training)
+    hidden = L.dropout(hidden, rate=rate, is_training=is_training, seed=1234)
+    return crf_head(hidden, features, params, is_training)
+
+
+def segmentation_embedding(features, params, is_training, ids=None, weights=None):
+    """[W[ids] (softword) or weights @ W (ex_softword) | frozen character embedding] -> [B, L, 5 + Ec], both pieces
+    written into one buffer.  W is the trainable [5, 5] `word_enhance/softword_embedding`, identity at initialisation;
+    TRAIN records its gradient, read from the first 5 columns of the buffer's gradient by ner_small_table_grad."""
+    input_ids = features['token_ids']
+    B, Lq = input_ids.shape
+    char_table = device_constant(params, 'embedding')
+    n = SOFTWORD_LABELS
+    table = variables.get_variable(SOFTWORD_TABLE, (n, n), variables.constant(np.eye(n, dtype=np.float32)))
+    embedding = torch.empty((B, Lq, n + char_table.shape[1]), dtype=torch.float32, device=input_ids.device)
+    if weights is not None:
+        weights = weights.reshape(B, Lq, n)
+        ops.multihot_embed(table, weights, out=embedding)
+    else:
+        ops.embedding_lookup(table, ids, out=embedding)
+    ops.embedding_lookup(char_table, input_ids, out=embedding, col_offset=n)
+    tape = autodiff.current() if is_training else None
+    if tape is not None:
+        store = variables.default_store()
+
+        def bwd(g):
+            if g is not None:
+                ops.small_table_grad(store.grad(SOFTWORD_TABLE), g.contiguous(), ids=ids, weights=weights)
+        tape.record(embedding, bwd)
+    return embedding
 
 
 def crf_head(hidden, features, params, is_training, name='logits'):

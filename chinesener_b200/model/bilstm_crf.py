@@ -1,18 +1,14 @@
 """`bilstm_crf` (reference model/bilstm_crf.py:8-62): frozen pretrained character embedding -> dropout -> BiLSTM(128, tanh)
 -> dropout -> label projection -> CRF."""
 from .. import ops
-from ..tools.layer import dropout
 from . import _blocks as nn
 
 _const_table = nn.device_constant          # other plugins import the table cache under this name
 
 
 def build_graph(features, labels, params, is_training):
-    rate = params['embedding_dropout']
     chars = ops.embedding_lookup(nn.device_constant(params, 'embedding'), features['token_ids'])
-    hidden = nn.recurrent(dropout(chars, rate=rate, is_training=is_training, seed=1234), features, params, is_training)
-    hidden = dropout(hidden, rate=rate, is_training=is_training, seed=1234)
-    return nn.crf_head(hidden, features, params, is_training)
+    return nn.bilstm_crf_tail(chars, features, params, is_training)
 
 
 TRAIN_PARAMS = nn.hyper(

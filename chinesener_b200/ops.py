@@ -251,6 +251,45 @@ def softlexicon_pool_bwd(d_table, ids, weights, d_out, G=4, S=10):
     return d_table
 
 
+# --------------------------------------------------------------------------- small word-enhance tables
+def multihot_embed(table, weights, out=None, col_offset=0):
+    """weights [..., V] @ table [V, E] (ner_multihot_embed_fwd) into out[..., col_offset:col_offset+E]."""
+    require_cuda(table, weights, out)
+    assert table.dtype == torch.float32 and weights.dtype == torch.float32
+    V, E = table.shape
+    assert weights.shape[-1] == V
+    n_tok = weights.numel() // V
+    if out is None:
+        out = torch.empty((*weights.shape[:-1], E), dtype=torch.float32, device=table.device)
+    ld = out.shape[-1]
+    assert col_offset + E <= ld and out.numel() == n_tok * ld
+    check(lib().ner_multihot_embed_fwd(ptr(table), ptr(weights), out.data_ptr() + 4 * col_offset, n_tok, V, E, ld, stream()))
+    return out
+
+
+_small_table_scratch = {}
+
+
+def small_table_grad(d_table, d_out, ids=None, weights=None, col_offset=0):
+    """d_table [V, E] += the gradient of embedding_lookup(table, ids) (one-hot) or multihot_embed(table, weights),
+    read from d_out[..., col_offset:col_offset+E] (d_out row-major [n_tok, ld]).  Deterministic (ner_small_table_grad)."""
+    require_cuda(d_table, d_out, ids, weights)
+    assert (ids is None) != (weights is None)
+    assert d_table.dtype == torch.float32 and d_out.dtype == torch.float32
+    V, E = d_table.shape
+    n_tok = ids.numel() if ids is not None else weights.numel() // V
+    ld = d_out.shape[-1]
+    assert col_offset + E <= ld and d_out.numel() == n_tok * ld
+    need = int(lib().ner_small_table_grad_scratch_floats(V, E))
+    key = (d_table.device.index, stream())
+    scratch = _small_table_scratch.get(key)
+    if scratch is None or scratch.numel() < need:
+        scratch = _small_table_scratch[key] = torch.empty(max(need, 1), dtype=torch.float32, device=d_table.device)
+    check(lib().ner_small_table_grad(ptr(d_table), ptr(None if ids is None else _i32(ids)), ptr(weights),
+                                     d_out.data_ptr() + 4 * col_offset, n_tok, V, E, ld, ptr(scratch), stream()))
+    return d_table
+
+
 def crf_loglik_bwd(logits, tags, seq_len, trans, alpha, logz, d_ll=None, scale=1.0):
     """-> d_logits [B,L,K], d_trans [K,K] for g_b = (d_ll|1) * scale."""
     require_cuda(logits, tags, seq_len, trans, alpha, logz, d_ll)

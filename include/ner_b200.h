@@ -391,6 +391,27 @@ int ner_softlexicon_pool_bwd(float* d_table, const int32_t* ids, const float* we
                              ner_stream_t stream);
 
 /* ------------------------------------------------------------------------ *
+ * Small-table word-enhance embeddings — model/bilstm_crf_softword.py, model/bilstm_crf_ex_softword.py
+ * ------------------------------------------------------------------------ */
+
+/* ExSoftword projection: out[t, 0:E] = sum_v weights[t, v] * table[v, :], summed over v ascending, zero weights skipped.
+ * table [V,E] f32, weights [n_tok,V] f32, out row stride ld_out >= E (lets the caller write into a concat buffer).
+ * V <= 8 and E <= 128, else NER_ERR_UNSUPPORTED.  Null pointers are NER_ERR_INVALID_ARG unless n_tok == 0. */
+int ner_multihot_embed_fwd(const float* table, const float* weights, float* out, int n_tok, int V, int E,
+                           int ld_out, ner_stream_t stream);
+/* Gradient of a [V,E] table read by ner_embedding_lookup (ids) or ner_multihot_embed_fwd (weights):
+ *   d_table[v, :] += sum_t c(t, v) * d_out[t, :],  c(t, v) = [clamp(ids[t], 0, V-1) == v]  or  weights[t, v].
+ * Exactly one of ids [n_tok] i32 / weights [n_tok,V] f32 is given (both, or neither with n_tok > 0, is
+ * NER_ERR_INVALID_ARG); ids outside [0, V) are clamped into it, as the SoftLexicon pool does.  d_out row stride
+ * ld_dout >= E.  V <= 8 and E <= 128, else NER_ERR_UNSUPPORTED.  Deterministic, no float atomics: each CTA sums a fixed
+ * token range into a [V,E] partial in `scratch` (>= ner_small_table_grad_scratch_floats(V, E) floats, 0 for an
+ * unsupported V, E), and the partials are added in CTA order.  The grid depends only on n_tok and the SM count, so a
+ * device gives a bit-identical gradient on every call. */
+size_t ner_small_table_grad_scratch_floats(int V, int E);
+int ner_small_table_grad(float* d_table, const int32_t* ids, const float* weights, const float* d_out, int n_tok,
+                         int V, int E, int ld_dout, float* scratch, ner_stream_t stream);
+
+/* ------------------------------------------------------------------------ *
  * Training-side kernels — gradients of the layers above and the two optimizer steps of
  * tools/train_utils.py:246-390
  * ------------------------------------------------------------------------ */
