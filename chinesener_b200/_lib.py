@@ -75,6 +75,10 @@ SIGNATURES = {
     "ner_multihot_embed_fwd": (_i, [_vp] * 3 + [_i] * 4 + [_vp]),
     "ner_small_table_grad_scratch_floats": (_c.c_size_t, [_i, _i]),
     "ner_small_table_grad": (_i, [_vp] * 4 + [_i] * 4 + [_vp, _vp]),
+    "ner_gemm_e4m3": (_i, [_vp] * 7 + [_i] * 4 + [_vp]),
+    "ner_quantize_weight_e4m3": (_i, [_vp, _vp, _vp, _i, _i, _vp]),
+    "ner_bert_embed_ln_e4m3": (_i, [_vp] * 11 + [_i] * 6 + [_c.c_float, _vp, _i, _vp]),
+    "ner_layernorm_e4m3": (_i, [_vp, _i] + [_vp] * 7 + [_i, _i, _c.c_float, _vp]),
 }
 
 
@@ -88,6 +92,11 @@ class BertConfig(_c.Structure):
 class BertLayerWeights(_c.Structure):
     _fields_ = [(n, _vp) for n in ("wqkv", "bqkv", "wo", "bo", "ln1_gamma", "ln1_beta", "wi", "bi", "wd", "bd",
                                    "ln2_gamma", "ln2_beta")]
+
+
+class BertLayerWeightsFp8(_c.Structure):
+    _fields_ = [(n, _vp) for n in ("wqkv", "sqkv", "bqkv", "wo", "bo", "ln1_gamma", "ln1_beta", "wi", "si", "bi", "wd", "sd",
+                                   "bd", "ln2_gamma", "ln2_beta")]
 
 
 class BertLayerGrads(_c.Structure):
@@ -120,6 +129,9 @@ SIGNATURES["ner_axpy_f32"] = (_i, [_vp, _vp, _c.c_size_t, _c.c_float, _vp])
 SIGNATURES["ner_bert_encoder_workspace_bytes"] = (_c.c_size_t, [_c.POINTER(BertConfig), _i])
 SIGNATURES["ner_bert_encoder_fwd"] = (_i, [_c.POINTER(BertConfig)] + [_vp] * 5 + [_c.POINTER(BertLayerWeights)] + [_vp] * 3
                                       + [_i, _i, _vp, _vp, _i, _vp, _vp, _vp, _c.c_size_t, _vp])
+SIGNATURES["ner_bert_encoder_fp8_workspace_bytes"] = (_c.c_size_t, [_c.POINTER(BertConfig), _i])
+SIGNATURES["ner_bert_encoder_fwd_fp8"] = (_i, [_c.POINTER(BertConfig)] + [_vp] * 5 + [_c.POINTER(BertLayerWeightsFp8)] + [_vp] * 3
+                                          + [_i, _i, _vp, _vp, _i, _vp, _vp, _vp, _c.c_size_t, _vp])
 
 class PackEntry(_c.Structure):
     _fields_ = [("src", _vp), ("K", _i), ("N", _i), ("dst_nk_bf16", _vp), ("ld_nk", _i), ("dst_kn_bf16", _vp), ("ld_kn", _i)]

@@ -266,6 +266,108 @@ def bert_forward(input_ids, input_mask, segment_ids, cfg, store=None, scope="ber
     return x32, x16
 
 
+# =========================================================================== FP8 inference
+def _packed_fp8(store, cfg, scope):
+    """FP8 operands of every layer, rebuilt when the store changes: e4m3 [N,K] packs + per-channel scales of the QKV (query |
+    key | value fused), FFN1 and FFN2 kernels; the out-projection keeps its bf16 pack (shared with the bf16 path)."""
+    bf = _packed(store, cfg, scope)
+
+    def build():
+        v, out = store.vars, []
+        for l, w in enumerate(bf):
+            p = f"{scope}/encoder/layer_{l}"
+            wqkv = torch.cat([v[f"{p}/attention/self/{n}/kernel"] for n in ("query", "key", "value")], dim=1).contiguous()
+            (wq, sq), (wi, si), (wd, sd) = (ops.quantize_weight_e4m3(t) for t in
+                                            (wqkv, v[f"{p}/intermediate/dense/kernel"], v[f"{p}/output/dense/kernel"]))
+            out.append(dict(w, wqkv=wq, sqkv=sq, wi=wi, si=si, wd=wd, sd=sd))
+        return out
+    return store.cached(("bert_pack_fp8", scope), build)
+
+
+def _c_tables_fp8(store, cfg, scope, gelu):
+    """ctypes config + per-layer pointer table for ner_bert_encoder_fwd_fp8 (rebuilt with the packs)."""
+    layers = _packed_fp8(store, cfg, scope)
+
+    def build():
+        from . import _lib
+        c = _lib.BertConfig(cfg["hidden_size"], cfg["num_attention_heads"], cfg["intermediate_size"],
+                            cfg["num_hidden_layers"], cfg["vocab_size"], cfg["type_vocab_size"],
+                            cfg["max_position_embeddings"], 1e-12, 1 if gelu == "erf" else 0, 0)
+        arr = (_lib.BertLayerWeightsFp8 * len(layers))()
+        for i, w in enumerate(layers):
+            arr[i] = _lib.BertLayerWeightsFp8(*[w[k].data_ptr() for k in ("wqkv", "sqkv", "bqkv", "wo", "bo", "g1", "b1", "wi", "si",
+                                                                         "bi", "wd", "sd", "bd", "g2", "b2")])
+        return c, arr, layers
+    return store.cached(("bert_ctable_fp8", scope, gelu), build)
+
+
+def _check_fp8_shape(cfg):
+    H, I = cfg["hidden_size"], cfg["intermediate_size"]
+    if H % 128 or I % 128:
+        raise ValueError(f"bert_precision='fp8' needs hidden_size and intermediate_size to be multiples of 128 (its activation "
+                         f"scales cover 1 x 128 blocks); this BERT has hidden_size={H}, intermediate_size={I}")
+
+
+def bert_forward_fp8(input_ids, input_mask, segment_ids, cfg, store=None, scope="bert", gelu="tanh", pack=None,
+                     per_kernel=None):
+    """Inference BertModel forward with FP8 (e4m3, block-scaled) QKV / FFN1 / FFN2 GEMMs -> (f32 [rows,H], bf16 [rows,H]),
+    the outputs of bert_forward.  Default: ONE C-ABI call (ner_bert_encoder_fwd_fp8); per_kernel=True drives the same kernels
+    one ops.* call at a time."""
+    store = store or variables.default_store()
+    create_bert_variables(cfg, store, scope)
+    _check_fp8_shape(cfg)
+    if per_kernel is None:
+        per_kernel = PER_KERNEL
+    B, L = input_ids.shape
+    H, NH = cfg["hidden_size"], cfg["num_attention_heads"]
+    v = store.vars
+    rows = pack.total if pack else B * L
+    dev = input_ids.device
+    if not per_kernel:
+        import ctypes
+        from . import _lib
+        c, arr, _ = _c_tables_fp8(store, cfg, scope, gelu)
+        c.gemm_tile = ops.DEFAULT_TILE
+        of = torch.empty((rows, H), dtype=torch.float32, device=dev)
+        ob = torch.empty((rows, H), dtype=torch.bfloat16, device=dev)
+        need = _lib.lib().ner_bert_encoder_fp8_workspace_bytes(ctypes.byref(c), rows)
+        key = (dev.index, _lib.stream())
+        ws = _ws_cache.get(key)
+        if ws is None or ws.numel() < need:
+            ws = torch.empty((need,), dtype=torch.uint8, device=dev)
+            _ws_cache[key] = ws
+        ids, mask = ops._i32(input_ids), ops._i32(input_mask)
+        seg = None if segment_ids is None else ops._i32(segment_ids)
+        _lib.check(_lib.lib().ner_bert_encoder_fwd_fp8(
+            ctypes.byref(c), v[f"{scope}/embeddings/word_embeddings"].data_ptr(),
+            v[f"{scope}/embeddings/token_type_embeddings"].data_ptr(), v[f"{scope}/embeddings/position_embeddings"].data_ptr(),
+            v[f"{scope}/embeddings/LayerNorm/gamma"].data_ptr(), v[f"{scope}/embeddings/LayerNorm/beta"].data_ptr(), arr,
+            ids.data_ptr(), mask.data_ptr(), _lib.ptr(seg), B, L, _lib.ptr(pack.cu_seqlens if pack else None),
+            _lib.ptr(pack.tok_src if pack else None), pack.total if pack else 0, of.data_ptr(), ob.data_ptr(),
+            ws.data_ptr(), ws.numel(), _lib.stream()))
+        _lib.LAUNCHES += 7 * cfg["num_hidden_layers"]      # the call above enqueued 1 + 7/layer kernels
+        return of, ob
+    layers = _packed_fp8(store, cfg, scope)
+    x32, xq, xs = ops.bert_embed_ln_e4m3(v[f"{scope}/embeddings/word_embeddings"], v[f"{scope}/embeddings/token_type_embeddings"],
+                                         v[f"{scope}/embeddings/position_embeddings"], v[f"{scope}/embeddings/LayerNorm/gamma"],
+                                         v[f"{scope}/embeddings/LayerNorm/beta"], input_ids, segment_ids, eps=1e-12,
+                                         tok_src=pack.tok_src if pack else None, n_packed=pack.total if pack else 0)
+    epi_gelu = ops.EPI_GELU_ERF_E4M3 if gelu == "erf" else ops.EPI_GELU_TANH_E4M3
+    cu = pack.cu_seqlens if pack else None
+    for i, w in enumerate(layers):
+        qkv = ops.gemm_e4m3(xq, xs, w["wqkv"], w["sqkv"], w["bqkv"], epilogue=ops.EPI_BF16)
+        ctx = ops.bert_attention(qkv, input_mask, B, L, NH, H // NH, cu_seqlens=cu)
+        y = ops.gemm_bf16(ctx, w["wo"], w["bo"], epilogue=ops.EPI_BF16)
+        x1, xq, xs = ops.layernorm_e4m3(y, w["g1"], w["b1"], residual=x32, eps=1e-12)
+        iq, isc = ops.gemm_e4m3(xq, xs, w["wi"], w["si"], w["bi"], epilogue=epi_gelu)
+        y = ops.gemm_e4m3(iq, isc, w["wd"], w["sd"], w["bd"], epilogue=ops.EPI_BF16)
+        if i + 1 < len(layers):
+            x32, xq, xs = ops.layernorm_e4m3(y, w["g2"], w["b2"], residual=x1, eps=1e-12)
+        else:
+            x32, x16 = ops.layernorm(y, w["g2"], w["b2"], residual=x1, eps=1e-12)
+    return x32, x16
+
+
 # =========================================================================== training
 def _tf_casts(store, cfg, scope):
     """bf16 casts of the dense kernels in their TF layout [in, out]: the K-major B operand of the

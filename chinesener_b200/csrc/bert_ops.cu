@@ -14,9 +14,13 @@ constexpr int LN_MAXV = 8;  // float4 per lane -> H <= 1024
 
 // Row LayerNorm over registers: v holds this lane's float4s (nv4 valid), H = row length.
 // Matches tf.contrib.layers.layer_norm / tf.nn.moments: biased variance of (x - mean).
+// Q: also write the row as e4m3 (out_q) with one scale per 128 columns (out_s).  Needs H % 128 == 0: float4 k of every lane
+// is then valid and the 32 lanes' float4 k are exactly columns [128k, 128k + 128), so a block's amax is one warp_max.
+template <bool Q = false>
 __device__ __forceinline__ void ln_row(float4 (&v)[LN_MAXV], int nv4, int H, int lane, float eps,
                                        const float* __restrict__ gamma, const float* __restrict__ beta,
-                                       float* __restrict__ out_f32, __nv_bfloat16* __restrict__ out_bf16) {
+                                       float* __restrict__ out_f32, __nv_bfloat16* __restrict__ out_bf16,
+                                       uint8_t* __restrict__ out_q = nullptr, float* __restrict__ out_s = nullptr) {
   float s = 0.f;
 #pragma unroll
   for (int k = 0; k < LN_MAXV; ++k)
@@ -51,18 +55,25 @@ __device__ __forceinline__ void ln_row(float4 (&v)[LN_MAXV], int nv4, int H, int
         pk.y = *reinterpret_cast<uint32_t*>(&hi);
         *reinterpret_cast<uint2*>(out_bf16 + e) = pk;
       }
+      if constexpr (Q) {
+        const float s = e4m3_scale(warp_max(fmaxf(fmaxf(fabsf(o.x), fabsf(o.y)), fmaxf(fabsf(o.z), fabsf(o.w)))));
+        const uint32_t lo = cvt_e4m3x2(__fdiv_rn(o.x, s), __fdiv_rn(o.y, s)), hi = cvt_e4m3x2(__fdiv_rn(o.z, s), __fdiv_rn(o.w, s));
+        *reinterpret_cast<uint32_t*>(out_q + e) = lo | (hi << 16);
+        if (lane == 0) out_s[k] = s;
+      }
     }
   }
 }
 
-// one warp per token
+// one warp per token; Q: also the e4m3 + block-scale copy (out_q [n_tok, H], out_s [n_tok, H/128])
+template <bool Q>
 __global__ void __launch_bounds__(256)
 bert_embed_ln_kernel(const float* __restrict__ word_emb, const float* __restrict__ type_emb,
                      const float* __restrict__ pos_emb, const float* __restrict__ gamma,
                      const float* __restrict__ beta, const int32_t* __restrict__ ids,
                      const int32_t* __restrict__ seg, float* __restrict__ out_f32,
                      __nv_bfloat16* __restrict__ out_bf16, int n_tok, int L, int H, int V, int n_type, float eps,
-                     const int32_t* __restrict__ tok_src) {
+                     const int32_t* __restrict__ tok_src, uint8_t* __restrict__ out_q, float* __restrict__ out_s) {
   const int lane = threadIdx.x & 31;
   const int nv4 = (H / 4 + 31) / 32;
   for (int tok = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); tok < n_tok; tok += gridDim.x * (blockDim.x >> 5)) {
@@ -86,8 +97,9 @@ bert_embed_ln_kernel(const float* __restrict__ word_emb, const float* __restrict
         v[k] = make_float4(a.x + b.x + c.x, a.y + b.y + c.y, a.z + b.z + c.z, a.w + b.w + c.w);
       }
     }
-    ln_row(v, nv4, H, lane, eps, gamma, beta, out_f32 ? out_f32 + (size_t)tok * H : nullptr,
-           out_bf16 ? out_bf16 + (size_t)tok * H : nullptr);
+    ln_row<Q>(v, nv4, H, lane, eps, gamma, beta, out_f32 ? out_f32 + (size_t)tok * H : nullptr,
+              out_bf16 ? out_bf16 + (size_t)tok * H : nullptr, Q ? out_q + (size_t)tok * H : nullptr,
+              Q ? out_s + (size_t)tok * (H / 128) : nullptr);
   }
 }
 
@@ -115,11 +127,13 @@ bert_embed_sum_kernel(const float* __restrict__ word_emb, const float* __restric
 // y (+ optional residual) -> LayerNorm -> fp32 and/or bf16.  y is fp32 or (YBF16) bf16.
 // DROP: y is first passed through dropout (counter-based mask of ner_dropout: element index row*H + col) —
 // BertModel's hidden dropout in front of the residual add, fused so the dropped tensor is never written.
-template <bool YBF16, bool DROP>
+// Q: also the e4m3 + block-scale copy (out_q [M, H], out_s [M, H/128]).
+template <bool YBF16, bool DROP, bool Q>
 __global__ void __launch_bounds__(256)
 layernorm_kernel(const void* __restrict__ yv, const float* __restrict__ residual, const float* __restrict__ gamma,
                  const float* __restrict__ beta, float* __restrict__ out_f32, __nv_bfloat16* __restrict__ out_bf16,
-                 int M, int H, float eps, float keep, uint32_t seed_lo, uint32_t seed_hi) {
+                 int M, int H, float eps, float keep, uint32_t seed_lo, uint32_t seed_hi, uint8_t* __restrict__ out_q,
+                 float* __restrict__ out_s) {
   pdl_launch_dependents();
   pdl_wait();
   const int lane = threadIdx.x & 31;
@@ -158,8 +172,9 @@ layernorm_kernel(const void* __restrict__ yv, const float* __restrict__ residual
         }
       }
     }
-    ln_row(v, nv4, H, lane, eps, gamma, beta, out_f32 ? out_f32 + (size_t)row * H : nullptr,
-           out_bf16 ? out_bf16 + (size_t)row * H : nullptr);
+    ln_row<Q>(v, nv4, H, lane, eps, gamma, beta, out_f32 ? out_f32 + (size_t)row * H : nullptr,
+              out_bf16 ? out_bf16 + (size_t)row * H : nullptr, Q ? out_q + (size_t)row * H : nullptr,
+              Q ? out_s + (size_t)row * (H / 128) : nullptr);
   }
 }
 
@@ -252,6 +267,39 @@ pack_group_kernel(const ner_pack_entry* __restrict__ entries, const int32_t* __r
         }
       }
     }
+  }
+}
+
+// TF dense kernel [K,N] fp32 -> e4m3 [N,K] (K contiguous) with one scale per output channel n (= column of src).  One CTA per
+// 32 channels: the column amax over K, then the scaled, transposed pack through a 32 x 33 smem tile.
+__global__ void __launch_bounds__(256)
+quantize_weight_e4m3_kernel(const float* __restrict__ src, uint8_t* __restrict__ dst, float* __restrict__ scale, int K, int N) {
+  __shared__ float tile[32][33];
+  __shared__ float red[8][32];
+  const int n0 = blockIdx.x * 32, tx = threadIdx.x & 31, ty = threadIdx.x >> 5, n = n0 + tx;
+  float m = 0.f;
+  if (n < N)
+    for (int k = ty; k < K; k += 8) m = fmaxf(m, fabsf(src[(size_t)k * N + n]));
+  red[ty][tx] = m;
+  __syncthreads();
+  if (ty == 0) {
+    for (int i = 1; i < 8; ++i) m = fmaxf(m, red[i][tx]);
+    const float s = e4m3_scale(m);
+    red[0][tx] = s;
+    if (n < N) scale[n] = s;
+  }
+  __syncthreads();
+  for (int k0 = 0; k0 < K; k0 += 32) {
+    for (int i = ty; i < 32; i += 8) {
+      const int k = k0 + i;
+      tile[i][tx] = (k < K && n < N) ? src[(size_t)k * N + n] : 0.f;
+    }
+    __syncthreads();
+    for (int i = ty; i < 32; i += 8) {
+      const int nn = n0 + i, k = k0 + tx;
+      if (nn < N && k < K) dst[(size_t)nn * K + k] = (uint8_t)(cvt_e4m3x2(__fdiv_rn(tile[tx][i], red[0][i]), 0.f) & 0xffu);
+    }
+    __syncthreads();
   }
 }
 
@@ -389,9 +437,9 @@ extern "C" int ner_bert_embed_ln(const float* word_emb, const float* type_emb, c
   const int n_tok = tok_src ? n_packed : B * L;
   if (n_tok < 0 || n_tok > B * L) return NER_ERR_INVALID_ARG;
   if (n_tok == 0) return NER_OK;
-  bert_embed_ln_kernel<<<grid_for_rows(n_tok, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+  bert_embed_ln_kernel<false><<<grid_for_rows(n_tok, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       word_emb, type_emb, pos_emb, gamma, beta, ids, seg, out_f32, static_cast<__nv_bfloat16*>(out_bf16), n_tok, L, H,
-      vocab, n_type, eps, tok_src);
+      vocab, n_type, eps, tok_src, nullptr, nullptr);
   return ner_launch_status();
 }
 
@@ -415,11 +463,11 @@ extern "C" int ner_layernorm_dropout(const void* y, int y_is_bf16, const float* 
   if (!(keep_prob > 0.f) || keep_prob > 1.f) return NER_ERR_INVALID_ARG;
   if (H % 4 != 0 || H > 128 * LN_MAXV) return NER_ERR_UNSUPPORTED;
   const bool drop = keep_prob < 1.f;
-  auto kern = y_is_bf16 ? (drop ? layernorm_kernel<true, true> : layernorm_kernel<true, false>)
-                        : (drop ? layernorm_kernel<false, true> : layernorm_kernel<false, false>);
+  auto kern = y_is_bf16 ? (drop ? layernorm_kernel<true, true, false> : layernorm_kernel<true, false, false>)
+                        : (drop ? layernorm_kernel<false, true, false> : layernorm_kernel<false, false, false>);
   cudaError_t e = ner_launch_pdl(kern, dim3(grid_for_rows(M, 8)), dim3(256), 0, static_cast<cudaStream_t>(stream), y, residual,
                                  gamma, beta, out_f32, static_cast<__nv_bfloat16*>(out_bf16), M, H, eps, keep_prob,
-                                 (uint32_t)seed, (uint32_t)(seed >> 32));
+                                 (uint32_t)seed, (uint32_t)(seed >> 32), (uint8_t*)nullptr, (float*)nullptr);
   if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
   return ner_launch_status();
 }
@@ -527,5 +575,44 @@ extern "C" int ner_split_bf16(const float* src, void* hi_bf16, void* lo_bf16, in
   if (g > ner_num_sms() * 32) g = ner_num_sms() * 32;
   split_bf16_kernel<<<(int)g, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       src, static_cast<__nv_bfloat16*>(hi_bf16), static_cast<__nv_bfloat16*>(lo_bf16), M, D, Dp, ld_src);
+  return ner_launch_status();
+}
+
+extern "C" int ner_bert_embed_ln_e4m3(const float* word_emb, const float* type_emb, const float* pos_emb, const float* gamma,
+                                      const float* beta, const int32_t* ids, const int32_t* seg, float* out_f32, void* out_bf16,
+                                      void* out_e4m3, float* out_scale, int B, int L, int H, int vocab, int n_type, int max_pos,
+                                      float eps, const int32_t* tok_src, int n_packed, ner_stream_t stream) {
+  if (B < 0 || L < 1 || H < 4 || vocab < 1 || n_type < 1) return NER_ERR_INVALID_ARG;
+  if (B == 0) return NER_OK;
+  if (!word_emb || !type_emb || !pos_emb || !gamma || !beta || !ids || !out_e4m3 || !out_scale) return NER_ERR_INVALID_ARG;
+  if (H % 128 != 0 || H > 128 * LN_MAXV || L > max_pos) return NER_ERR_UNSUPPORTED;
+  const int n_tok = tok_src ? n_packed : B * L;
+  if (n_tok < 0 || n_tok > B * L) return NER_ERR_INVALID_ARG;
+  if (n_tok == 0) return NER_OK;
+  bert_embed_ln_kernel<true><<<grid_for_rows(n_tok, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      word_emb, type_emb, pos_emb, gamma, beta, ids, seg, out_f32, static_cast<__nv_bfloat16*>(out_bf16), n_tok, L, H,
+      vocab, n_type, eps, tok_src, static_cast<uint8_t*>(out_e4m3), out_scale);
+  return ner_launch_status();
+}
+
+extern "C" int ner_layernorm_e4m3(const void* y, int y_is_bf16, const float* residual, const float* gamma, const float* beta,
+                                  float* out_f32, void* out_bf16, void* out_e4m3, float* out_scale, int M, int H, float eps,
+                                  ner_stream_t stream) {
+  if (M < 0 || H < 4) return NER_ERR_INVALID_ARG;
+  if (M == 0) return NER_OK;
+  if (!y || !gamma || !beta || !out_e4m3 || !out_scale) return NER_ERR_INVALID_ARG;
+  if (H % 128 != 0 || H > 128 * LN_MAXV) return NER_ERR_UNSUPPORTED;
+  auto kern = y_is_bf16 ? layernorm_kernel<true, false, true> : layernorm_kernel<false, false, true>;
+  cudaError_t e = ner_launch_pdl(kern, dim3(grid_for_rows(M, 8)), dim3(256), 0, static_cast<cudaStream_t>(stream), y, residual,
+                                 gamma, beta, out_f32, static_cast<__nv_bfloat16*>(out_bf16), M, H, eps, 1.0f, 0u, 0u,
+                                 static_cast<uint8_t*>(out_e4m3), out_scale);
+  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
+  return ner_launch_status();
+}
+
+extern "C" int ner_quantize_weight_e4m3(const float* w_kn, void* wt_nk_e4m3, float* w_scale, int K, int N, ner_stream_t stream) {
+  if (K < 1 || N < 1 || !w_kn || !wt_nk_e4m3 || !w_scale) return NER_ERR_INVALID_ARG;
+  quantize_weight_e4m3_kernel<<<(N + 31) / 32, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      w_kn, static_cast<uint8_t*>(wt_nk_e4m3), w_scale, K, N);
   return ner_launch_status();
 }

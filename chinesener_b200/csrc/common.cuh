@@ -128,4 +128,15 @@ __device__ __forceinline__ uint32_t keep_threshold(float keep) {
   return (uint32_t)fminf(keep * 4294967296.f, 4294967295.f);
 }
 
+// OCP e4m3 ("fn", max 448) block scaling of the FP8 encoder: scale = amax / 448 in fp32, 1 when amax == 0;
+// q = e4m3(x / scale), round to nearest even, saturating.
+constexpr float kE4m3Max = 448.f;
+__device__ __forceinline__ float e4m3_scale(float amax) { return amax > 0.f ? __fdiv_rn(amax, kE4m3Max) : 1.f; }
+// two floats -> packed e4m3 pair: `lo` in the low byte (the lower address)
+__device__ __forceinline__ uint16_t cvt_e4m3x2(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+
 }  // namespace nerdev

@@ -569,6 +569,197 @@ gemm_wgrad_group_kernel(const __grid_constant__ WgradGroup grp) {
   }
 }
 
+// ===================================================================== FP8 (e4m3) GEMM with block scales
+//   out[M,N] = epi( s_w[n] · Σ_j s_a[m,j] · (Σ_{k in block j} qa[m,k] · qw[n,k]) + bias[n] )
+// A e4m3 [M,K] with fp32 scales s_a [M, K/128] (row m, columns [128j, 128j+128)); Wt e4m3 [N,K] with one fp32 scale per
+// output channel s_w [N].  The persistent warp-specialised shape of gemm_bf16_tc_kernel with a 128 x 128 tile: a k-block is
+// 128 e4m3 = 128 B, one SWIZZLE_128B row, so a ring stage holds as many bytes as the bf16 kernel's (Cfg<128>, Ring<128>).
+// Per k-block four wgmma.m64n128k32 e4m3 accumulate into a temporary, which is then promoted into the fp32 accumulator with
+// one FMA per element scaled by s_a[row, kb]: Hopper's FP8 wgmma accumulator keeps fewer mantissa bits than fp32, and
+// promoting every 128 products bounds that loss to one block.  A warpgroup waits for its k-block's wgmma before promoting
+// it (64 accumulator + 64 temporary registers per thread); the tensor cores stay fed by the other MMA warpgroup, whose
+// wgmma runs while this one promotes.  Keeping a second k-block in flight through a second temporary makes ptxas serialise
+// every wgmma (C7514: the promotion reads one accumulator while the other's group is pending) and spill.
+// Epilogues: acc · s_w + bias -> bf16 through epilogue_tma, or GELU(acc · s_w + bias) -> e4m3 with 1 x 128 block scales.
+constexpr int FP8_BN = 128;
+constexpr int FP8_BK = 128;     // e4m3 per k-block = 128 B
+constexpr int FP8_MMA_K = 32;
+
+template <int EPI>
+__host__ __device__ constexpr bool epi_e4m3() { return EPI == NER_EPI_GELU_TANH_E4M3 || EPI == NER_EPI_GELU_ERF_E4M3; }
+
+// Four K = 32 wgmma of one k-block into the temporary `t` (the first one overwrites it), committed as one group.
+__device__ __forceinline__ void fp8_issue(float (&t)[FP8_BN / 2], const Ring<FP8_BN>& ring, int stage, uint32_t a_off) {
+  const uint32_t a_addr = smem_u32(ring.a + stage * Cfg<FP8_BN>::A_BYTES) + a_off;
+  const uint32_t b_addr = smem_u32(ring.b + stage * Cfg<FP8_BN>::B_BYTES);
+  reg_fence(t);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < FP8_BK / FP8_MMA_K; ++k)
+    wgmma_m64n128k32_e4m3(t, make_wgmma_desc_sw128(a_addr + k * FP8_MMA_K), make_wgmma_desc_sw128(b_addr + k * FP8_MMA_K),
+                          k > 0 ? 1u : 0u);
+  wgmma_commit();
+  reg_fence(t);
+}
+
+// acc += t · s_a of the fragment's rows (s0: row r, s1: row r + 8)
+__device__ __forceinline__ void fp8_promote(float (&acc)[FP8_BN / 2], const float (&t)[FP8_BN / 2], float s0, float s1) {
+#pragma unroll
+  for (int i = 0; i < FP8_BN / 2; ++i) acc[i] = fmaf(t[i], (i & 2) ? s1 : s0, acc[i]);
+}
+
+// GELU(acc · s_w + bias) -> e4m3 with one scale per row and 128-column block.  A row's 128 tile columns sit in the four lanes
+// of one quad, so the block amax is two shuffles.  The tanh form uses the accurate tanhf (not tanh.approx as the bf16
+// epilogue does), so the quantised bytes are a function of the fp32 accumulator alone.  Values are quantised as x · (1/s)
+// rather than x / s (the LayerNorm's form): the two differ by at most one fp32 ulp before the e4m3 rounding, and the 64
+// divisions per thread were a measurable share of the FFN1 epilogue.  The warpgroup's 64 x 128 bytes are
+// one 8 KB SWIZZLE_128B staging chunk, stored by TMA; the scales go straight to out_scale [M, N/128].
+template <int EPI>
+__device__ __forceinline__ void epilogue_e4m3(float (&acc)[FP8_BN / 2], const float* bias, float* out_scale,
+                                              const CUtensorMap* tma_out, uint8_t* stage, uint32_t& buf, int row_wg, int n0,
+                                              int M, int N) {
+  const int t = threadIdx.x & 127, lane = t & 31, warp = t >> 5;
+  const int bar = 1 + (threadIdx.x >> 7);
+  const int r0 = 16 * warp + (lane >> 2);
+  if (row_wg >= M) return;
+  uint8_t* sb = stage + buf * OUT_CHUNK_BYTES;
+  if (t == 0) tma_store_wait_read<1>();
+  wg_bar_sync(bar);
+  float amax[2] = {0.f, 0.f};
+#pragma unroll
+  for (int j = 0; j < FP8_BN / 8; ++j) {
+    const int col = n0 + 8 * j + 2 * (lane & 3);
+    const float2 b = bias != nullptr ? __ldg(reinterpret_cast<const float2*>(bias + col)) : make_float2(0.f, 0.f);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const float x = acc[4 * j + 2 * h + c] + (c ? b.y : b.x);
+        float v;
+        if constexpr (EPI == NER_EPI_GELU_ERF_E4M3) v = gelu_erf(x);
+        else v = 0.5f * x * (1.f + tanhf(0.7978845608028654f * fmaf(0.044715f * x * x, x, x)));
+        acc[4 * j + 2 * h + c] = v;
+        amax[h] = fmaxf(amax[h], fabsf(v));
+      }
+    }
+  }
+  float inv[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    amax[h] = fmaxf(amax[h], __shfl_xor_sync(0xffffffffu, amax[h], 1));
+    amax[h] = fmaxf(amax[h], __shfl_xor_sync(0xffffffffu, amax[h], 2));
+    const float s = nerdev::e4m3_scale(amax[h]);
+    inv[h] = __frcp_rn(s);
+    const int row = row_wg + r0 + 8 * h;
+    if ((lane & 3) == 0 && row < M) out_scale[(size_t)row * (N / FP8_BN) + n0 / FP8_BN] = s;
+  }
+#pragma unroll
+  for (int j = 0; j < FP8_BN / 8; ++j) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = r0 + 8 * h;
+      const uint16_t q = nerdev::cvt_e4m3x2(acc[4 * j + 2 * h] * inv[h], acc[4 * j + 2 * h + 1] * inv[h]);
+      *reinterpret_cast<uint16_t*>(sb + r * 128 + (((j >> 1) ^ (r & 7)) << 4) + 8 * (j & 1) + 2 * (lane & 3)) = q;
+    }
+  }
+  fence_proxy_async();
+  wg_bar_sync(bar);
+  if (t == 0) {
+    tma_store_2d(tma_out, sb, n0, row_wg);
+    tma_store_commit();
+  }
+  buf ^= 1u;
+}
+
+template <int EPI>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_e4m3_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
+                    const __grid_constant__ CUtensorMap tma_out, const float* __restrict__ a_scale,
+                    const float* __restrict__ w_scale, const float* __restrict__ bias, float* __restrict__ out_scale, int M,
+                    int N, int K) {
+  using C = Cfg<FP8_BN>;
+  constexpr int STAGES = C::STAGES;
+  nerdev::pdl_launch_dependents();
+
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  if ((smem_u32(smem_raw) & 1023u) != 0u) __trap();
+  const Ring<FP8_BN> ring(smem_raw);
+
+  const int wg = threadIdx.x >> 7;
+  const int num_n = N / FP8_BN;
+  const int num_tiles = ((M + BM - 1) / BM) * num_n;
+  const int num_kb = K / FP8_BK;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tma_a);
+    tma_prefetch_desc(&tma_b);
+    tma_prefetch_desc(&tma_out);
+  }
+  init_ring<FP8_BN, 1>(ring);
+  __syncthreads();
+  nerdev::pdl_wait();
+
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x < 32 && elect_one()) {
+      RingPos pos;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m_blk = tile / num_n, n_blk = tile - m_blk * num_n;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&ring.empty[pos.stage], pos.phase ^ 1u);
+          mbar_arrive_expect_tx(&ring.full[pos.stage], C::A_BYTES + C::B_BYTES);
+          tma_load_2d(ring.a + pos.stage * C::A_BYTES, &tma_a, &ring.full[pos.stage], kb * FP8_BK, m_blk * BM);
+          tma_load_2d(ring.b + pos.stage * C::B_BYTES, &tma_b, &ring.full[pos.stage], kb * FP8_BK, n_blk * FP8_BN);
+          pos.advance<STAGES>();
+        }
+      }
+    }
+  } else {
+    setmaxnreg_inc<232>();
+    const int mw = wg - 1;
+    const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
+    uint8_t* stage = ring.out + mw * 2 * OUT_CHUNK_BYTES;
+    uint32_t buf = 0;
+    const uint32_t a_off = (uint32_t)(mw * 64 * FP8_BK);
+    RingPos pos;
+    float acc[FP8_BN / 2], tmp[FP8_BN / 2];
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int m_blk = tile / num_n, n_blk = tile - m_blk * num_n;
+      const int row_wg = m_blk * BM + mw * 64, n0 = n_blk * FP8_BN;
+      const int ra = row_wg + 16 * warp + (lane >> 2);
+      // s_a rows of this thread's fragment (rows past M read row M - 1: TMA zero-fills their A, the value is unused)
+      const float* sa0 = a_scale + (size_t)min(ra, M - 1) * num_kb;
+      const float* sa1 = a_scale + (size_t)min(ra + 8, M - 1) * num_kb;
+#pragma unroll
+      for (int i = 0; i < FP8_BN / 2; ++i) acc[i] = 0.f;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        const float s0 = __ldg(sa0 + kb), s1 = __ldg(sa1 + kb);
+        mbar_wait(&ring.full[pos.stage], pos.phase);
+        fp8_issue(tmp, ring, pos.stage, a_off);
+        wgmma_wait<0>();
+        reg_fence(tmp);
+        if (lane == 0) mbar_arrive(&ring.empty[pos.stage]);
+        fp8_promote(acc, tmp, s0, s1);
+        pos.advance<STAGES>();
+      }
+      // per-channel weight scale
+#pragma unroll
+      for (int j = 0; j < FP8_BN / 8; ++j) {
+        const float2 sw = __ldg(reinterpret_cast<const float2*>(w_scale + n0 + 8 * j + 2 * (lane & 3)));
+        acc[4 * j] *= sw.x;
+        acc[4 * j + 1] *= sw.y;
+        acc[4 * j + 2] *= sw.x;
+        acc[4 * j + 3] *= sw.y;
+      }
+      if constexpr (epi_e4m3<EPI>())
+        epilogue_e4m3<EPI>(acc, bias, out_scale, &tma_out, stage, buf, row_wg, n0, M, N);
+      else
+        epilogue_tma<FP8_BN, NER_EPI_BF16>(acc, EpiArgs{bias, nullptr}, &tma_out, stage, buf, row_wg, n0, M, N);
+    }
+    if ((threadIdx.x & 127) == 0) tma_store_wait_all();
+  }
+}
+
 // ---------------------------------------------------------------- host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -848,5 +1039,60 @@ extern "C" int ner_gemm_bf16(const void* A, const void* Wt, const float* bias, c
     case NER_TILE_2CTA_256: return launch_gemm<256, 2>(A, Wt, ep, out, M, N, K, epilogue, st);
     case NER_TILE_2CTA_128: return launch_gemm<128, 2>(A, Wt, ep, out, M, N, K, epilogue, st);
     default: return NER_ERR_INVALID_ARG;
+  }
+}
+
+namespace {
+// e4m3 row-major [rows, cols] (one byte per element) with a {128 columns, box_rows} box, 128-byte swizzle.
+int make_map_e4m3(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (fn == nullptr) return NER_ERR_NO_DRIVER;
+  cuuint64_t dims[2] = {cols, rows};
+  cuuint64_t strides[1] = {cols};
+  cuuint32_t box[2] = {128, box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? NER_OK : NER_ERR_INVALID_ARG;
+}
+
+template <int EPI>
+int launch_gemm_e4m3(const void* A, const float* a_scale, const void* Wt, const float* w_scale, const float* bias, void* out,
+                     float* out_scale, int M, int N, int K, cudaStream_t st) {
+  CUtensorMap ma, mb, mo;
+  int rc = make_map_e4m3(&ma, A, (uint64_t)M, (uint64_t)K, BM);
+  if (rc != NER_OK) return rc;
+  rc = make_map_e4m3(&mb, Wt, (uint64_t)N, (uint64_t)K, FP8_BN);
+  if (rc != NER_OK) return rc;
+  rc = epi_e4m3<EPI>() ? make_map_e4m3(&mo, out, (uint64_t)M, (uint64_t)N, 64) : make_map_2d(&mo, out, (uint64_t)M, (uint64_t)N, 64);
+  if (rc != NER_OK) return rc;
+  const int tiles = ((M + BM - 1) / BM) * (N / FP8_BN);
+  const cudaError_t e = launch_ex(gemm_e4m3_tc_kernel<EPI>, tiles < sm_count() ? tiles : sm_count(), Cfg<FP8_BN>::SMEM, st, 1,
+                                  ma, mb, mo, a_scale, w_scale, bias, out_scale, M, N, K);
+  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
+  return ner_launch_status();
+}
+}  // namespace
+
+extern "C" int ner_gemm_e4m3(const void* A, const float* a_scale, const void* Wt, const float* w_scale, const float* bias,
+                             void* out, float* out_scale, int M, int N, int K, int epilogue, ner_stream_t stream) {
+  if (M < 0 || N < 1 || K < 1) return NER_ERR_INVALID_ARG;
+  if (epilogue != NER_EPI_BF16 && epilogue != NER_EPI_GELU_TANH_E4M3 && epilogue != NER_EPI_GELU_ERF_E4M3)
+    return NER_ERR_INVALID_ARG;
+  if (K % FP8_BK != 0 || N % FP8_BN != 0) return NER_ERR_UNSUPPORTED;   // whole 128-wide scale blocks and tiles
+  if (M == 0) return NER_OK;
+  const bool q_out = epilogue != NER_EPI_BF16;
+  if (!A || !a_scale || !Wt || !w_scale || !out || (q_out && !out_scale)) return NER_ERR_INVALID_ARG;
+  if ((reinterpret_cast<uintptr_t>(A) & 15) || (reinterpret_cast<uintptr_t>(Wt) & 15) || (reinterpret_cast<uintptr_t>(out) & 15))
+    return NER_ERR_INVALID_ARG;
+  // w_scale and bias are read as float2 column pairs
+  if ((reinterpret_cast<uintptr_t>(w_scale) & 7) || (reinterpret_cast<uintptr_t>(bias) & 7)) return NER_ERR_INVALID_ARG;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  switch (epilogue) {
+    case NER_EPI_BF16: return launch_gemm_e4m3<NER_EPI_BF16>(A, a_scale, Wt, w_scale, bias, out, out_scale, M, N, K, st);
+    case NER_EPI_GELU_TANH_E4M3:
+      return launch_gemm_e4m3<NER_EPI_GELU_TANH_E4M3>(A, a_scale, Wt, w_scale, bias, out, out_scale, M, N, K, st);
+    default: return launch_gemm_e4m3<NER_EPI_GELU_ERF_E4M3>(A, a_scale, Wt, w_scale, bias, out, out_scale, M, N, K, st);
   }
 }

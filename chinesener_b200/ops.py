@@ -10,6 +10,8 @@ from ._lib import NerB200Error, check, lib, ptr, require_cuda, stream
 
 EPI_F32, EPI_BF16, EPI_GELU_TANH_BF16, EPI_GELU_ERF_BF16, EPI_RELU_BF16, EPI_RES_F32, EPI_RES_RELU_F32 = range(7)
 EPI_DIAG_DISCARD = 99
+EPI_GELU_TANH_E4M3, EPI_GELU_ERF_E4M3 = 7, 8   # ner_gemm_e4m3 only: GELU -> e4m3 with 1 x 128 block scales
+E4M3 = torch.float8_e4m3fn
 TILE_2CTA_128, TILE_2CTA_256 = 1128, 1256   # CTA-pair (cta_group::2) tiles of ner_gemm_bf16
 TILE_SK_128, TILE_SK_256 = 2128, 2256       # stream-K scheduling of 128 x {128,256} tiles
 TILE_AUTO_THROUGHPUT = 3000                 # auto, preferring the tile with the best FLOP rate (multi-stream serving)
@@ -85,6 +87,42 @@ def pack_weight_bf16(w_kn):
     return out
 
 
+def gemm_e4m3(a, a_scale, wt, w_scale, bias=None, epilogue=EPI_BF16, out=None, out_scale=None):
+    """FP8 dense layer with block scales (ner_gemm_e4m3): a e4m3 [M,K] + a_scale f32 [M, K/128], wt e4m3 [N,K] + w_scale
+    f32 [N].  EPI_BF16 -> bf16 [M,N]; EPI_GELU_*_E4M3 -> (e4m3 [M,N], f32 block scales [M, N/128])."""
+    require_cuda(a, a_scale, wt, w_scale, bias, out, out_scale)
+    assert a.dtype == E4M3 and wt.dtype == E4M3 and a_scale.dtype == torch.float32 and w_scale.dtype == torch.float32
+    M, K = a.shape
+    N, K2 = wt.shape
+    assert K == K2 and w_scale.numel() == N and a_scale.shape == (M, K // 128)
+    if bias is not None:
+        assert bias.dtype == torch.float32 and bias.numel() == N
+    q_out = epilogue in (EPI_GELU_TANH_E4M3, EPI_GELU_ERF_E4M3)
+    if out is None:
+        out = torch.empty((M, N), dtype=E4M3 if q_out else torch.bfloat16, device=a.device)
+    if q_out and out_scale is None:
+        out_scale = torch.empty((M, N // 128), dtype=torch.float32, device=a.device)
+    hook = _lib._HOOK
+    args = (ptr(a), ptr(a_scale), ptr(wt), ptr(w_scale), ptr(bias), ptr(out), ptr(out_scale), M, N, K, epilogue, stream())
+    if hook is not None:
+        with hook("gemm_e4m3", 2.0 * M * N * K):
+            check(lib().ner_gemm_e4m3(*args))
+    else:
+        check(lib().ner_gemm_e4m3(*args))
+    return (out, out_scale) if q_out else out
+
+
+def quantize_weight_e4m3(w_kn):
+    """TF dense kernel [K,N] f32 -> (e4m3 [N,K], f32 per-channel scales [N]): the B operand of gemm_e4m3."""
+    require_cuda(w_kn)
+    assert w_kn.dtype == torch.float32 and w_kn.dim() == 2
+    K, N = w_kn.shape
+    q = torch.empty((N, K), dtype=E4M3, device=w_kn.device)
+    sc = torch.empty((N,), dtype=torch.float32, device=w_kn.device)
+    check(lib().ner_quantize_weight_e4m3(ptr(w_kn), ptr(q), ptr(sc), K, N, stream()))
+    return q, sc
+
+
 def cast_bf16(x):
     require_cuda(x)
     assert x.dtype == torch.float32
@@ -148,6 +186,36 @@ def layernorm(y, gamma, beta, residual=None, eps=1e-12, want_f32=True, want_bf16
     check(lib().ner_layernorm_dropout(ptr(y), 1 if y.dtype == torch.bfloat16 else 0, ptr(residual), ptr(gamma), ptr(beta),
                                       ptr(of), ptr(ob), M, H, eps, float(keep_prob), int(seed) & 0xFFFFFFFFFFFFFFFF, stream()))
     return of, ob
+
+
+def bert_embed_ln_e4m3(word_emb, type_emb, pos_emb, gamma, beta, ids, seg, eps=1e-12, tok_src=None, n_packed=0):
+    """bert_embed_ln writing f32 + the e4m3 copy with 1 x 128 block scales -> (f32 [rows,H], e4m3 [rows,H], f32 [rows,H/128])."""
+    require_cuda(word_emb, type_emb, pos_emb, gamma, beta, ids, seg, tok_src)
+    B, L = ids.shape
+    V, H = word_emb.shape
+    ids = _i32(ids)
+    seg = None if seg is None else _i32(seg)
+    rows = n_packed if tok_src is not None else B * L
+    of = torch.empty((rows, H), dtype=torch.float32, device=ids.device)
+    oq = torch.empty((rows, H), dtype=E4M3, device=ids.device)
+    osc = torch.empty((rows, H // 128), dtype=torch.float32, device=ids.device)
+    check(lib().ner_bert_embed_ln_e4m3(ptr(word_emb), ptr(type_emb), ptr(pos_emb), ptr(gamma), ptr(beta), ptr(ids), ptr(seg),
+                                       ptr(of), None, ptr(oq), ptr(osc), B, L, H, V, type_emb.shape[0], pos_emb.shape[0], eps,
+                                       ptr(tok_src), n_packed, stream()))
+    return of, oq, osc
+
+
+def layernorm_e4m3(y, gamma, beta, residual=None, eps=1e-12):
+    """LN(y + residual) -> (f32 [M,H], e4m3 [M,H], f32 block scales [M, H/128])."""
+    require_cuda(y, gamma, beta, residual)
+    assert y.dtype in (torch.float32, torch.bfloat16)
+    M, H = y.shape
+    of = torch.empty((M, H), dtype=torch.float32, device=y.device)
+    oq = torch.empty((M, H), dtype=E4M3, device=y.device)
+    osc = torch.empty((M, H // 128), dtype=torch.float32, device=y.device)
+    check(lib().ner_layernorm_e4m3(ptr(y), 1 if y.dtype == torch.bfloat16 else 0, ptr(residual), ptr(gamma), ptr(beta),
+                                   ptr(of), None, ptr(oq), ptr(osc), M, H, eps, stream()))
+    return of, oq, osc
 
 
 def bert_attention(qkv, mask, B, L, num_heads, head_dim=64, scale=None, mask_add=-10000.0, cu_seqlens=None, keep_prob=1.0,

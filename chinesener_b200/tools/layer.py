@@ -16,8 +16,9 @@ PACK_SEQUENCES = os.environ.get("NER_B200_PACK", "1") != "0"
 # TRAIN mode of BertModel on the packed layout too (ner_bert_encoder_train_fwd_packed / _bwd_packed)
 TRAIN_PACK = os.environ.get("NER_B200_TRAIN_PACK", "1") != "0"
 # 'bf16': bf16 wgmma operands (BASELINE config 3, the benchmark path); 'fp32': fp32-accurate encoder (config 2's
-# "fp32": split-bf16 dense + fp32 attention, emission logits within 1e-3 of the reference).  Estimator sets it from
-# params['bert_precision'] around build_graph.
+# "fp32": split-bf16 dense + fp32 attention, emission logits within 1e-3 of the reference); 'fp8': PREDICT / EVAL only,
+# the QKV and FFN GEMMs on block-scaled e4m3 wgmma (bert.bert_forward_fp8; TRAIN ignores it, as it does 'fp32').
+# Estimator sets it from params['bert_precision'] around build_graph.
 BERT_PRECISION = os.environ.get("NER_B200_BERT_PRECISION", "bf16")
 
 
@@ -44,13 +45,14 @@ def pretrain_bert_embedding(input_ids, input_mask, segment_ids, pretrain_dir, dr
         return dropout(emb, rate=drop_out, is_training=True, seed=1234)
     if BERT_PRECISION == 'fp32':
         return _bert.bert_forward_f32(input_ids, input_mask, segment_ids, cfg).view(B, L, -1)
+    forward = _bert.bert_forward_fp8 if BERT_PRECISION == 'fp8' else _bert.bert_forward
     if PACK_SEQUENCES:
         pack = _bert.make_pack(input_mask)
-        x32, x16 = _bert.bert_forward(input_ids, input_mask, segment_ids, cfg, pack=pack)
+        x32, x16 = forward(input_ids, input_mask, segment_ids, cfg, pack=pack)
         emb = x32                      # [total_tokens, H]: packed rows, see PackInfo
         emb.bf16, emb.pack = x16, pack
         return emb
-    x32, x16 = _bert.bert_forward(input_ids, input_mask, segment_ids, cfg)
+    x32, x16 = forward(input_ids, input_mask, segment_ids, cfg)
     emb = x32.view(B, L, -1)
     emb.bf16 = x16.view(B, L, -1)
     return emb

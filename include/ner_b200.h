@@ -112,6 +112,23 @@ int ner_gemm_bf16(const void* A, const void* Wt, const float* bias, const float*
                   void* out, int M, int N, int K, int epilogue, int tile_n,
                   ner_stream_t stream);
 
+/* FP8 (OCP e4m3 "fn", max 448) dense layer with block scales, the inference-only FP8 encoder's QKV / FFN GEMMs:
+ *   out[M,N] = epi( w_scale[n] · Σ_j a_scale[m,j] · (Σ_{k in [128j, 128j+128)} A[m,k] · Wt[n,k]) + bias[n] )
+ * A e4m3 [M,K] row-major with f32 a_scale [M, K/128]; Wt e4m3 [N,K] (K contiguous, from ner_quantize_weight_e4m3) with
+ * f32 w_scale [N].  Each 128-wide k-block is accumulated by wgmma and promoted into an fp32 accumulator.
+ * epilogue: NER_EPI_BF16 (out bf16 [M,N] = acc + bias), or NER_EPI_GELU_TANH_E4M3 / NER_EPI_GELU_ERF_E4M3: out e4m3 [M,N]
+ * = GELU(acc + bias) quantised per 1 x 128 block, with the block scales in out_scale [M, N/128] (scale = amax / 448, or 1
+ * for an all-zero block; round to nearest even, saturating).  bias may be NULL.  K % 128 == 0 and N % 128 == 0, else
+ * NER_ERR_UNSUPPORTED.  A, Wt, out 16-byte aligned; w_scale, bias 8-byte aligned. */
+#define NER_EPI_GELU_TANH_E4M3 7 /* out e4m3 + block scales = gelu_tanh(acc + bias) (ner_gemm_e4m3 only) */
+#define NER_EPI_GELU_ERF_E4M3 8  /* out e4m3 + block scales = gelu_erf(acc + bias)  (ner_gemm_e4m3 only) */
+int ner_gemm_e4m3(const void* A, const float* a_scale, const void* Wt, const float* w_scale, const float* bias,
+                  void* out, float* out_scale, int M, int N, int K, int epilogue, ner_stream_t stream);
+
+/* TF dense kernel w_kn [K,N] f32 -> e4m3 [N,K] (K contiguous) with one scale per output channel:
+ * w_scale[n] = max_k |W[k,n]| / 448 (1 for an all-zero column), wt[n,k] = e4m3(W[k,n] / w_scale[n]). */
+int ner_quantize_weight_e4m3(const float* w_kn, void* wt_nk_e4m3, float* w_scale, int K, int N, ner_stream_t stream);
+
 /* TF dense kernel [K,N] f32 -> bf16 [N,K] (K contiguous), the B-operand layout of
  * ner_gemm_bf16.  Done once per weight (or per optimizer step). */
 int ner_pack_weight_bf16(const float* w_kn, void* wt_nk_bf16, int K, int N, ner_stream_t stream);
@@ -198,6 +215,18 @@ int ner_layernorm(const void* y, int y_is_bf16, const float* residual, const flo
                   const float* beta, float* out_f32, void* out_bf16, int M, int H, float eps,
                   ner_stream_t stream);
 
+/* ner_bert_embed_ln / ner_layernorm that also write the normalised row as e4m3 [M,H] with 1 x 128 block scales
+ * out_scale [M, H/128] (the A operand of ner_gemm_e4m3), quantised from the same fp32 values out_f32 receives.
+ * out_e4m3 and out_scale are required; out_f32 / out_bf16 may be NULL.  H % 128 == 0, else NER_ERR_UNSUPPORTED. */
+int ner_bert_embed_ln_e4m3(const float* word_emb, const float* type_emb, const float* pos_emb,
+                           const float* gamma, const float* beta, const int32_t* ids,
+                           const int32_t* seg, float* out_f32, void* out_bf16, void* out_e4m3, float* out_scale,
+                           int B, int L, int H, int vocab, int n_type, int max_pos, float eps,
+                           const int32_t* tok_src, int n_packed, ner_stream_t stream);
+int ner_layernorm_e4m3(const void* y, int y_is_bf16, const float* residual, const float* gamma,
+                       const float* beta, float* out_f32, void* out_bf16, void* out_e4m3, float* out_scale, int M,
+                       int H, float eps, ner_stream_t stream);
+
 /* ner_layernorm with BertModel's hidden dropout fused in front of the residual add:
  * out = LN(dropout(y) + residual), mask = the counter-based decisions of ner_dropout (element = row*H + col).
  * keep_prob = 1: identical to ner_layernorm. */
@@ -262,6 +291,29 @@ int ner_bert_encoder_fwd(const ner_bert_config* cfg, const float* word_emb, cons
                          const int32_t* cu_seqlens, const int32_t* tok_src, int n_packed,
                          float* out_f32, void* out_bf16, void* workspace, size_t workspace_bytes,
                          ner_stream_t stream);
+
+/* The same forward with FP8 dense layers (inference only): QKV, FFN1 and FFN2 run on ner_gemm_e4m3, their A operands
+ * written by the LayerNorms (ner_bert_embed_ln_e4m3 / ner_layernorm_e4m3) and by FFN1's GELU -> e4m3 epilogue.  The
+ * out-projection, attention, the f32 residual stream and LayerNorm arithmetic are those of ner_bert_encoder_fwd.
+ * Same modes and outputs (the last LayerNorm writes f32 + bf16).  hidden_size and intermediate_size must be multiples of
+ * 128, else NER_ERR_UNSUPPORTED. */
+typedef struct {
+  const void* wqkv;  const float* sqkv;  const float* bqkv;   /* [3H,H] e4m3, [3H] scales, [3H] bias */
+  const void* wo;    const float* bo;                         /* attention/output/dense, [H,H] bf16 */
+  const float* ln1_gamma; const float* ln1_beta;
+  const void* wi;    const float* si;    const float* bi;     /* intermediate/dense [I,H] e4m3, [I], [I] */
+  const void* wd;    const float* sd;    const float* bd;     /* output/dense [H,I] e4m3, [H], [H] */
+  const float* ln2_gamma; const float* ln2_beta;
+} ner_bert_layer_weights_fp8;
+
+size_t ner_bert_encoder_fp8_workspace_bytes(const ner_bert_config* cfg, int rows);
+int ner_bert_encoder_fwd_fp8(const ner_bert_config* cfg, const float* word_emb, const float* type_emb,
+                             const float* pos_emb, const float* emb_ln_gamma, const float* emb_ln_beta,
+                             const ner_bert_layer_weights_fp8* layers, const int32_t* ids,
+                             const int32_t* mask, const int32_t* seg, int B, int L,
+                             const int32_t* cu_seqlens, const int32_t* tok_src, int n_packed,
+                             float* out_f32, void* out_bf16, void* workspace, size_t workspace_bytes,
+                             ner_stream_t stream);
 
 /* TRAIN-mode BertModel (is_training=True) as two calls: forward keeping every activation the backward
  * pass needs, and backward accumulating into the caller's gradient tensors (tf.gradients of
