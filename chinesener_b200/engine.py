@@ -45,8 +45,10 @@ class Estimator:
                 out[k] = v
         m = features.get('mask')
         if torch.is_tensor(m) and not m.is_cuda and 'mask' in out:
-            # host-side token count rides along so sequence packing needs no device sync
+            # host-side token count rides along so sequence packing needs no device sync; the count of non-empty rows
+            # sizes the query/context pairs of bert_mrc the same way
             out['mask'].total_tokens = int(m.sum())
+            out['mask'].nonempty_rows = int(m.any(1).sum())
         return out
 
     def predict_device(self, dev_features):
@@ -95,14 +97,17 @@ class Estimator:
                     dst[r:r + n].copy_(f[k], non_blocking=True)
                     r += n
                 out[k] = dst
+        nonempty = 0
         for f in feature_list:
             m = f.get('mask')
             if not (torch.is_tensor(m) and not m.is_cuda):
                 total = None
                 break
             total += int(m.sum())
+            nonempty += int(m.any(1).sum())
         if total is not None and 'mask' in out:
             out['mask'].total_tokens = total
+            out['mask'].nonempty_rows = nonempty
         return out
 
     def predict_iter(self, batches, depth=2, streams=1, group=1):

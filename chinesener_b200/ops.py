@@ -536,6 +536,43 @@ def token_dice(logits, labels, seq_len, alpha=1.0, gamma=1.0, want_pred=True, wa
     return pred, loss, dz
 
 
+# --------------------------------------------------------------------------- MRC pairs and tag merge (bert_mrc)
+def mrc_pairs(token_ids, seq_len, query_ids, query_len, type_tag, L2, sep_id, label_ids=None):
+    """[B, L] BERT batch -> its B*T query/context pairs (ner_mrc_pairs): dict of ids / segment_ids / mask [B*T, L2] i32,
+    seq_len [B*T] i32, align [B*T*L] i32 (pair row of each sentence position) and labels [B*T, L] i32 (per-type BIO; None
+    without label_ids).  query_ids [T, Qmax] i32, query_len [T] i32, type_tag [T, 2] i32."""
+    require_cuda(token_ids, seq_len, query_ids, query_len, type_tag, label_ids)
+    B, L = token_ids.shape
+    T, Qmax = query_ids.shape
+    token_ids, seq_len = _i32(token_ids), _i32(seq_len)
+    label_ids = None if label_ids is None else _i32(label_ids)
+    assert query_len.dtype == torch.int32 and type_tag.dtype == torch.int32 and tuple(type_tag.shape) == (T, 2)
+    dev = token_ids.device
+    pair = lambda *shape: torch.empty(shape, dtype=torch.int32, device=dev)
+    out = dict(ids=pair(B * T, L2), segment_ids=pair(B * T, L2), mask=pair(B * T, L2), seq_len=pair(B * T),
+               align=pair(B * T * L), labels=None if label_ids is None else pair(B * T, L))
+    check(lib().ner_mrc_pairs(ptr(token_ids), ptr(seq_len), ptr(label_ids), ptr(query_ids) if Qmax else None, ptr(query_len),
+                              ptr(type_tag), B, L, T, Qmax, L2, int(sep_id), ptr(out['ids']), ptr(out['segment_ids']),
+                              ptr(out['mask']), ptr(out['seq_len']), ptr(out['labels']), ptr(out['align']), stream()))
+    return out
+
+
+def mrc_merge(logits, seq_len, type_tag, o_id, cls_id, sep_id):
+    """Per-type logits [B*T, L, 3] f32 -> pred_ids [B, L] i32 in the dataset's tag space (ner_mrc_merge)."""
+    require_cuda(logits, seq_len, type_tag)
+    assert logits.dtype == torch.float32 and logits.dim() == 3 and logits.shape[2] == 3
+    T = type_tag.shape[0]
+    BT, L, _ = logits.shape
+    assert BT % T == 0 and type_tag.dtype == torch.int32
+    seq_len = _i32(seq_len)
+    B = BT // T
+    assert tuple(seq_len.shape) == (B,)
+    pred = torch.empty((B, L), dtype=torch.int32, device=logits.device)
+    check(lib().ner_mrc_merge(ptr(logits), ptr(seq_len), ptr(type_tag), B, L, T, int(o_id), int(cls_id), int(sep_id), ptr(pred),
+                              stream()))
+    return pred
+
+
 # --------------------------------------------------------------------------- training-side kernels
 def _require_rows(x2d):
     """CUDA f32 2-D tensor whose rows are contiguous (a column slice of a wider buffer is fine)."""

@@ -526,6 +526,29 @@ int ner_token_xent(const float* logits, const int32_t* labels, const int32_t* se
 int ner_token_dice(const float* logits, const int32_t* labels, const int32_t* seq_len, int32_t* pred_ids, float* loss,
                    float* d_logits, float d_loss, float alpha, float gamma, float* scratch, int B, int L, int K,
                    ner_stream_t stream);
+/* model/bert_mrc.py (MRC-style NER, one BERT query per entity type; a restatement, not pinned to the reference's mrc/):
+ * expands the [B,L] BERT batch (token_ids, seq_len [B] counting [CLS] and [SEP]) into the B*T pairs p = b*T + t,
+ *   pair row p = token_ids[b,0] ([CLS]), query_ids[t, 0:q_t], sep_id, token_ids[b, 1:len_b]
+ * of n_p = q_t + 1 + len_b tokens (0 when len_b = 0), len_b = clamp(seq_len[b], 0, L), q_t = clamp(query_len[t], 0, Qmax).
+ * query_ids [T,Qmax] i32 (may be NULL when Qmax = 0), query_len [T] i32, type_tag [T,2] i32 = tag ids of (B-X_t, I-X_t).
+ * Writes pair_ids / pair_segment_ids / pair_mask [B*T, L2] i32 (segment 0 up to and including the query's [SEP], 1 after;
+ * mask 1 for j < n_p; all three 0 from n_p on), pair_seq_len [B*T] = len_b, align_rows [B*T*L] = the pair row of
+ * sentence position s: p*L2 + (s == 0 ? 0 : q_t + 1 + s) (a [PAD] row of the pair when s >= len_b), and, when
+ * pair_labels [B*T, L] is not NULL, the per-type BIO labels of label_ids [B,L] (required then): for s < len_b 1 if the
+ * tag is B-X_t, 2 if I-X_t, else 0; 0 for s >= len_b.  T in [1, 32] (T > 32: NER_ERR_UNSUPPORTED), L2 >= Qmax + 1 + L and
+ * B*T*L2 < 2^31, else an error before any CUDA call.  One launch, no host synchronisation. */
+int ner_mrc_pairs(const int32_t* token_ids, const int32_t* seq_len, const int32_t* label_ids, const int32_t* query_ids,
+                  const int32_t* query_len, const int32_t* type_tag, int B, int L, int T, int Qmax, int L2, int sep_id,
+                  int32_t* pair_ids, int32_t* pair_segment_ids, int32_t* pair_mask, int32_t* pair_seq_len,
+                  int32_t* pair_labels, int32_t* align_rows, ner_stream_t stream);
+/* The bert_mrc tag merge: logits [B*T, L, 3] f32 (O, B, I of pair p = b*T + t at sentence position s), seq_len [B],
+ * type_tag [T,2] as ner_mrc_pairs -> pred_ids [B,L] i32 in the dataset's tag space.  With len_b = clamp(seq_len[b], 0, L):
+ *   s >= len_b: 0;  s == 0: cls_id;  s == len_b - 1: sep_id;
+ *   otherwise a_t = first argmax of type t's logits; among the types with a_t != O the one with the highest
+ *   z[a_t] - logsumexp(z) (fp32) wins, the lowest t on a tie; its B-X / I-X tag id, o_id when no type claims s.
+ * T in [1, 32] (T > 32: NER_ERR_UNSUPPORTED), B*T*L < 2^31.  One launch. */
+int ner_mrc_merge(const float* logits, const int32_t* seq_len, const int32_t* type_tag, int B, int L, int T, int o_id,
+                  int cls_id, int sep_id, int32_t* pred_ids, ner_stream_t stream);
 /* dst[i] += a * src[i]. */
 int ner_axpy_f32(float* dst, const float* src, size_t n, float a, ner_stream_t stream);
 /* out[0] += sum(g^2)  (tf.clip_by_global_norm, tools/train_utils.py:315).  Deterministic (no float atomics): per-CTA partial
