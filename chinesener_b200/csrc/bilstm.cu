@@ -17,42 +17,11 @@
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "dsmem.cuh"
 
 namespace cg = cooperative_groups;
 
 namespace {
-
-// --- DSMEM signalling without a cluster barrier: a remote 4-byte store that completes transaction
-// bytes on the DESTINATION CTA's mbarrier (st.async), so publishing h needs no fence over this
-// thread's earlier global stores and no L1 invalidate (barrier.cluster costs both every step).
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t local_smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void st_async_f32(uint32_t remote_addr, float v, uint32_t remote_bar) {
-  asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(remote_addr),
-               "r"(__float_as_uint(v)), "r"(remote_bar)
-               : "memory");
-}
-__device__ __forceinline__ void mbar_init_(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(nerdev::smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx_(uint64_t* bar, uint32_t tx_bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(nerdev::smem_u32(bar)), "r"(tx_bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_(uint64_t* bar, uint32_t parity) {
-  uint32_t ok = 0;
-  while (!ok) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(nerdev::smem_u32(bar)), "r"(parity)
-        : "memory");
-  }
-}
 
 // ex2.approx-based forms (abs. error ~1e-7, far inside the 1e-4 parity bar of tests/test_bilstm_gpu.py):
 // the activations sit on the per-step critical path of the recurrence.

@@ -44,7 +44,7 @@ def bert_bilstm_crf_predict(est, dev):
     H = cfg["hidden_size"]
     c, arr, _ = _bert._c_tables(store, cfg, "bert", "tanh")
     c.gemm_tile = ops.DEFAULT_TILE
-    pk = _layer._lstm_pack(store, H, Hl, lscope)
+    pk = _layer._rnn_pack(store, {d: _layer._rnn_names(lscope, d, "lstm", 0) for d in ("fw", "bw")}, H, False)
     if pk["Dp"] != H:
         return None
     ids, seg, m32, sl = ops._i32(dev['token_ids']), ops._i32(dev['segment_ids']), ops._i32(mask), ops._i32(dev['seq_len'])

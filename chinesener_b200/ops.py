@@ -269,6 +269,43 @@ def bilstm_recurrence_bwd(d_out, gates, cstate, wh_fw, wh_bw, seq_len, B, L, H, 
     return d_xproj
 
 
+# --------------------------------------------------------------------------- BiGRU
+def bigru_recurrence(xproj, wh_fw, wh_bw, seq_len, B, L, H, activation="tanh", cu_seqlens=None, save_for_backward=False,
+                     keep_prob=1.0, seed=0):
+    """GRUCell recurrence of both directions: xproj [rows, >= 6H] (extra columns are GEMM padding), wh_* [H, 3H] (columns r, u, c) -> out [B,L,2H]; with
+    save_for_backward also (gates [B*L,6H] = r, u, c; hstate [B,L,2H] carried h; rh [B,L,2H] = r ⊙ h_prev) for
+    bigru_recurrence_bwd.  keep_prob < 1: DropoutWrapper output/state dropout (training)."""
+    require_cuda(xproj, wh_fw, wh_bw, seq_len, cu_seqlens)
+    assert xproj.dtype == torch.float32 and xproj.shape[1] >= 6 * H
+    assert cu_seqlens is not None or xproj.shape[0] == B * L
+    assert wh_fw.shape == (H, 3 * H) and wh_bw.shape == (H, 3 * H)
+    act = {"tanh": 0, "relu": 1}[activation]
+    out = torch.empty((B, L, 2 * H), dtype=torch.float32, device=xproj.device)
+    gates = hst = rh = None
+    if save_for_backward:
+        assert cu_seqlens is None, "training runs on the padded layout"
+        gates = torch.zeros((B * L, 6 * H), dtype=torch.float32, device=xproj.device)
+        hst = torch.zeros((B, L, 2 * H), dtype=torch.float32, device=xproj.device)
+        rh = torch.zeros((B, L, 2 * H), dtype=torch.float32, device=xproj.device)
+    check(lib().ner_bigru_recurrence(ptr(xproj), ptr(wh_fw), ptr(wh_bw), ptr(_i32(seq_len)), ptr(out), B, L, H, xproj.shape[1],
+                                     act, ptr(cu_seqlens), ptr(gates), ptr(hst), ptr(rh), float(keep_prob),
+                                     int(seed) & 0xFFFFFFFFFFFFFFFF, stream()))
+    return (out, gates, hst, rh) if save_for_backward else out
+
+
+def bigru_recurrence_bwd(d_out, gates, hstate, wh_fw, wh_bw, seq_len, B, L, H, activation="tanh", keep_prob=1.0, seed=0):
+    """-> d_xproj [B*L, 6H] f32 (columns da_r, da_u, da_c per direction: the gradient of the hoisted input projection)."""
+    require_cuda(d_out, gates, hstate, wh_fw, wh_bw, seq_len)
+    assert d_out.shape == (B, L, 2 * H) and d_out.dtype == torch.float32
+    assert gates.shape == (B * L, 6 * H) and hstate.shape == (B, L, 2 * H)
+    act = {"tanh": 0, "relu": 1}[activation]
+    d_xproj = torch.empty((B * L, 6 * H), dtype=torch.float32, device=d_out.device)
+    check(lib().ner_bigru_recurrence_bwd(ptr(d_out), ptr(gates), ptr(hstate), ptr(wh_fw), ptr(wh_bw), ptr(_i32(seq_len)),
+                                         ptr(d_xproj), B, L, H, act, float(keep_prob), int(seed) & 0xFFFFFFFFFFFFFFFF,
+                                         stream()))
+    return d_xproj
+
+
 # --------------------------------------------------------------------------- SoftLexicon
 def softlexicon_pool(table, ids, weights, G=4, S=10, out=None):
     """ids/weights [..., G*S] -> [..., G*E]; `out` may be a wider [n_tok, >=G*E] buffer (concat target)."""

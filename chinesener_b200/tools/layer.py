@@ -82,75 +82,156 @@ def dropout(inputs, rate, is_training, seed=1234):
     return y
 
 
-def _lstm_pack(store, D, H, scope):
-    """bf16 [8H, Dp] input-projection pack (fw | bw), fused bias [8H], fp32 recurrent matrices."""
+RNN_COLUMNS = {'lstm': 4, 'gru': 3}   # recurrent columns per hidden unit: LSTMCell (i, j, f, o), GRUCell (r, u, c)
+
+
+def _rnn_config(cell_type, hidden_units_list, keep_prob_list, cell_size):
+    """-> (cell, n_layers) after checking bilstm()'s RNN arguments.  The reference indexes hidden_units_list[i] and
+    keep_prob_list[i] per layer (an IndexError there); here a list shorter than cell_size is a ValueError naming it."""
+    cell = str(cell_type).lower()
+    if cell not in RNN_COLUMNS:
+        raise Exception(f"cell_type={cell_type!r}: only 'lstm' and 'gru' are built on the sm_90a path")
+    n = int(cell_size)
+    if n < 1:
+        raise ValueError(f"cell_size must be >= 1, got {cell_size}")
+    for name, lst in (("hidden_units_list", hidden_units_list), ("keep_prob_list", keep_prob_list)):
+        if len(lst) < n:
+            raise ValueError(f"{name} has {len(lst)} entries but cell_size={n} needs one per layer")
+    return cell, n
+
+
+def _rnn_names(scope, d, cell, i):
+    """[(kernel, bias), ...] of layer i of direction d: one pair for LSTMCell, gates then candidate for GRUCell."""
+    base = f"{scope}/{d}/multi_rnn_cell/cell_{i}"
+    if cell == 'lstm':
+        return [(f"{base}/lstm_cell/kernel", f"{base}/lstm_cell/bias")]
+    return [(f"{base}/gru_cell/gates/kernel", f"{base}/gru_cell/gates/bias"),
+            (f"{base}/gru_cell/candidate/kernel", f"{base}/gru_cell/candidate/bias")]
+
+
+def _rnn_variables(store, scope, cell, i, Din, H):
+    """Create layer i of both directions under the reference's names -> {d: _rnn_names(...)}.  Initialisers as TF:
+    glorot_uniform kernels, zero LSTM bias, GRU gates bias 1.0 and candidate bias 0."""
+    names = {d: _rnn_names(scope, d, cell, i) for d in ("fw", "bw")}
+    for d in ("fw", "bw"):
+        if cell == 'lstm':
+            store.get_variable(names[d][0][0], (Din + H, 4 * H), variables.glorot_uniform)
+            store.get_variable(names[d][0][1], (4 * H,), variables.zeros)
+        else:
+            store.get_variable(names[d][0][0], (Din + H, 2 * H), variables.glorot_uniform)
+            store.get_variable(names[d][0][1], (2 * H,), variables.ones)
+            store.get_variable(names[d][1][0], (Din + H, H), variables.glorot_uniform)
+            store.get_variable(names[d][1][1], (H,), variables.zeros)
+    return names
+
+
+def _rnn_kernels(store, names):
+    """[Din + H, G*H] per direction: the cell's kernels side by side (GRU: [gates | candidate], columns r, u, c)."""
+    return [torch.cat([store.vars[k] for k, _ in names[d]], dim=1) if len(names[d]) > 1 else store.vars[names[d][0][0]]
+            for d in ("fw", "bw")]
+
+
+def _rnn_input_kernel(ks, Din, split):
+    """Input half of both directions -> f32 [D, 2GH] (fw columns | bw columns).  split: the layer reads [fw | bw] of the
+    layer below and each direction only its own half, so the kernel is block-diagonal (D = 2 Din)."""
+    if not split:
+        return torch.cat([k[:Din] for k in ks], dim=1)
+    G = ks[0].shape[1]
+    wx = torch.zeros((2 * Din, 2 * G), dtype=torch.float32, device=ks[0].device)
+    wx[:Din, :G] = ks[0][:Din]
+    wx[Din:, G:] = ks[1][:Din]
+    return wx
+
+
+def _rnn_pack(store, names, Din, split):
+    """bf16 [Np, Dp] input-projection pack (fw | bw), fused bias [Np], fp32 recurrent matrices [H, GH].  Np = 2GH, padded
+    with zero columns to the GEMM's 32-column granule (GRU with H % 16 != 0; the recurrence reads the row stride)."""
+    D = 2 * Din if split else Din
     Dp = (D + 7) // 8 * 8
 
     def build():
-        ks = [store.vars[f"{scope}/{d}/multi_rnn_cell/cell_0/lstm_cell/kernel"] for d in ("fw", "bw")]
-        bs = [store.vars[f"{scope}/{d}/multi_rnn_cell/cell_0/lstm_cell/bias"] for d in ("fw", "bw")]
-        wx = torch.cat([k[:D] for k in ks], dim=1)                      # [D, 8H]
-        if Dp != D:
-            wx = torch.nn.functional.pad(wx, (0, 0, 0, Dp - D))         # zero rows for the K padding
-        return dict(wx=ops.pack_weight_bf16(wx.contiguous()), bias=torch.cat(bs).contiguous(),
-                    wh_fw=ks[0][D:].contiguous(), wh_bw=ks[1][D:].contiguous(), Dp=Dp)
-    return store.cached(("lstm_pack", scope, D, H), build)
+        ks = _rnn_kernels(store, names)
+        bs = [store.vars[b] for d in ("fw", "bw") for _, b in names[d]]
+        wx = _rnn_input_kernel(ks, Din, split)
+        N = wx.shape[1]
+        Np = (N + 31) // 32 * 32
+        if Dp != D or Np != N:
+            wx = torch.nn.functional.pad(wx, (0, Np - N, 0, Dp - D))    # zero rows for the K padding, columns for N
+        bias = torch.cat(bs)
+        if Np != N:
+            bias = torch.nn.functional.pad(bias, (0, Np - N))
+        return dict(wx=ops.pack_weight_bf16(wx.contiguous()), bias=bias.contiguous(),
+                    wh_fw=ks[0][Din:].contiguous(), wh_bw=ks[1][Din:].contiguous(), Dp=Dp)
+    return store.cached(("rnn_pack", names["fw"][0][0], Din, split), build)
 
 
 def bilstm(embedding, cell_type, activation, hidden_units_list, keep_prob_list, cell_size, seq_len, dtype, is_training):
-    """reference tools/layer.py:27-41 — bidirectional_dynamic_rnn over LSTMCell; -> [B,L,2H] f32."""
-    if is_training:
-        return _bilstm_train(embedding, activation, hidden_units_list, keep_prob_list, cell_size, seq_len)
-    if cell_type.lower() != 'lstm':
-        raise Exception('Only lstm is built on the sm_90a path (reference models all use cell_type=lstm)')
-    if cell_size != 1:
-        raise Exception('cell_size must be 1 (every reference model uses a single LSTM layer)')
+    """reference tools/layer.py:27-41 — bidirectional_dynamic_rnn over a MultiRNNCell of `cell_size` DropoutWrapper-ed
+    LSTMCell / GRUCell layers; -> [B,L,2H] f32 of the top layer.
+
+    The fw and bw stacks are independent: layer i+1 of a direction reads layer i of the same direction (not the
+    [fw | bw] concat torch.nn.LSTM(bidirectional=True) feeds forward), through one GEMM with a block-diagonal weight.
+    Layer i has hidden_units_list[i] units and keep_prob_list[i] (TRAIN) on its output and carried state, each layer
+    with its own dropout seed.  PREDICT keeps a packed BERT layout for layer 0; upper layers read the padded output."""
+    cell, n = _rnn_config(cell_type, hidden_units_list, keep_prob_list, cell_size)
+    scope = variables.scoped("bilstm_layer/bidirectional_rnn")
+    x = embedding
+    for i in range(n):
+        H = int(hidden_units_list[i])
+        if is_training:
+            x = _rnn_layer_train(x, cell, i, scope, activation, H, float(keep_prob_list[i]), seq_len)
+        else:
+            x = _rnn_layer_predict(x, cell, i, scope, activation, H, seq_len)
+    return x
+
+
+def _rnn_layer_predict(embedding, cell, i, scope, activation, H, seq_len):
     pack = getattr(embedding, "pack", None)
     if pack is not None:
         B, L, D = pack.B, pack.L, embedding.shape[-1]
     else:
         B, L, D = embedding.shape
-    H = hidden_units_list[0]
+    Din = D if i == 0 else D // 2
     store = variables.default_store()
-    scope = variables.scoped("bilstm_layer/bidirectional_rnn")
-    for d in ("fw", "bw"):
-        store.get_variable(f"{scope}/{d}/multi_rnn_cell/cell_0/lstm_cell/kernel", (D + H, 4 * H), variables.glorot_uniform)
-        store.get_variable(f"{scope}/{d}/multi_rnn_cell/cell_0/lstm_cell/bias", (4 * H,), variables.zeros)
-    pk = _lstm_pack(store, D, H, scope)
+    names = _rnn_variables(store, scope, cell, i, Din, H)
+    pk = _rnn_pack(store, names, Din, i > 0)
     x16 = getattr(embedding, "bf16", None)
     if x16 is not None and pk["Dp"] == D:
         x16 = x16.reshape(-1, D)
     else:
         x16 = ops.cast_pad_bf16(embedding.reshape(-1, D), pk["Dp"])
     xproj = ops.gemm_bf16(x16, pk["wx"], pk["bias"], epilogue=ops.EPI_F32)
-    return ops.bilstm_recurrence(xproj, pk["wh_fw"], pk["wh_bw"], seq_len, B, L, H, activation=activation, forget_bias=1.0,
-                                 cu_seqlens=pack.cu_seqlens if pack is not None else None)
+    cu = pack.cu_seqlens if pack is not None else None
+    if cell == 'lstm':
+        return ops.bilstm_recurrence(xproj, pk["wh_fw"], pk["wh_bw"], seq_len, B, L, H, activation=activation,
+                                     forget_bias=1.0, cu_seqlens=cu)
+    return ops.bigru_recurrence(xproj, pk["wh_fw"], pk["wh_bw"], seq_len, B, L, H, activation=activation, cu_seqlens=cu)
 
 
-def _bilstm_train(embedding, activation, hidden_units_list, keep_prob_list, cell_size, seq_len):
-    """Training-mode bilstm(): same kernels on the padded layout, saves gates / cell states / carried
-    h and records the BPTT closure.  keep_prob < 1 = DropoutWrapper(output_keep_prob, state_keep_prob)
-    (reference tools/layer.py:20-23): counter-based masks inside the recurrence kernels."""
-    if cell_size != 1:
-        raise Exception('cell_size must be 1')
-    keep = float(keep_prob_list[0])
+def _rnn_layer_train(embedding, cell, i, scope, activation, H, keep, seq_len):
+    """Training-mode layer i: same kernels on the padded layout, saves what BPTT reads and records the backward closure.
+    keep < 1 = DropoutWrapper(output_keep_prob, state_keep_prob) (reference tools/layer.py:20-23): counter-based masks
+    inside the recurrence kernels."""
     B, L, D = embedding.shape
-    H = hidden_units_list[0]
+    split = i > 0
+    Din = D // 2 if split else D
+    G = RNN_COLUMNS[cell] * H
     store = variables.default_store()
-    scope = variables.scoped("bilstm_layer/bidirectional_rnn")
-    names = {}
-    for d in ("fw", "bw"):
-        names[d] = (f"{scope}/{d}/multi_rnn_cell/cell_0/lstm_cell/kernel", f"{scope}/{d}/multi_rnn_cell/cell_0/lstm_cell/bias")
-        store.get_variable(names[d][0], (D + H, 4 * H), variables.glorot_uniform)
-        store.get_variable(names[d][1], (4 * H,), variables.zeros)
-    pk = _lstm_pack(store, D, H, scope)
+    names = _rnn_variables(store, scope, cell, i, Din, H)
+    pk = _rnn_pack(store, names, Din, split)
     x2d = embedding.reshape(B * L, D).contiguous()
     x16 = ops.cast_pad_bf16(x2d, pk["Dp"])
     xproj = ops.gemm_bf16(x16, pk["wx"], pk["bias"], epilogue=ops.EPI_F32)
     store.dropout_calls += 1
     seed = (1234 * 1000003 + store.global_step) * 1009 + store.dropout_calls
-    out, gates, cst, hst = ops.bilstm_recurrence(xproj, pk["wh_fw"], pk["wh_bw"], seq_len, B, L, H, activation=activation,
-                                                 forget_bias=1.0, save_for_backward=True, keep_prob=keep, seed=seed)
+    if cell == 'lstm':
+        out, gates, cst, hst = ops.bilstm_recurrence(xproj, pk["wh_fw"], pk["wh_bw"], seq_len, B, L, H,
+                                                     activation=activation, forget_bias=1.0, save_for_backward=True,
+                                                     keep_prob=keep, seed=seed)
+    else:
+        out, gates, hst, rh = ops.bigru_recurrence(xproj, pk["wh_fw"], pk["wh_bw"], seq_len, B, L, H,
+                                                   activation=activation, save_for_backward=True, keep_prob=keep,
+                                                   seed=seed)
     tape = autodiff.current()
     if tape is not None:
         need_dx = tape.needs_grad(embedding)
@@ -158,13 +239,22 @@ def _bilstm_train(embedding, activation, hidden_units_list, keep_prob_list, cell
         def bwd(g):
             if g is None:
                 return
-            dxp = ops.bilstm_recurrence_bwd(g.contiguous(), gates, cst, pk["wh_fw"], pk["wh_bw"], seq_len, B, L, H,
-                                            activation=activation, keep_prob=keep, seed=seed)
+            if cell == 'lstm':
+                dxp = ops.bilstm_recurrence_bwd(g.contiguous(), gates, cst, pk["wh_fw"], pk["wh_bw"], seq_len, B, L, H,
+                                                activation=activation, keep_prob=keep, seed=seed)
+            else:
+                dxp = ops.bigru_recurrence_bwd(g.contiguous(), gates, hst, pk["wh_fw"], pk["wh_bw"], seq_len, B, L, H,
+                                               activation=activation, keep_prob=keep, seed=seed)
             dxp16 = ops.cast_bf16(dxp)
-            gks = [store.grad(names[d][0]) for d in ("fw", "bw")]
             for di, d in enumerate(("fw", "bw")):
-                ops.colsum_add(dxp[:, di * 4 * H:(di + 1) * 4 * H], store.grad(names[d][1]), 1.0)
-            grouped = pk["Dp"] == D and D % 128 == 0 and H % 128 == 0 and (4 * H) % 256 == 0 and all(k.is_contiguous() for k in gks)
+                col = di * G
+                for k, b in names[d]:
+                    n_col = store.vars[b].shape[0]
+                    ops.colsum_add(dxp[:, col:col + n_col], store.grad(b), 1.0)
+                    col += n_col
+            gks = [store.grad(names[d][0][0]) for d in ("fw", "bw")]
+            grouped = cell == 'lstm' and not split and pk["Dp"] == D and D % 128 == 0 and H % 128 == 0 \
+                and (4 * H) % 256 == 0 and all(k.is_contiguous() for k in gks)
             if grouped:
                 # dW_x (both directions) and dW_h (both directions) as ONE grouped launch: token-major operands read in place
                 # (ner_wgrad_group_bf16) instead of fp32 transposes + three stream-K GEMMs
@@ -177,19 +267,27 @@ def _bilstm_train(embedding, activation, hidden_units_list, keep_prob_list, cell
                     probs.append((hprev16[di].view(B * L, H), dxp16, di * 4 * H, gks[di][D:]))
                 ops.wgrad_group(probs, B * L)
             else:
-                dwx = ops.wgrad_gemm(x2d, dxp)                                   # [D, 8H] = x^T d_xproj
+                dwx = ops.wgrad_gemm(x2d, dxp)                                   # [D, 2GH] = x^T d_xproj
                 for di, d in enumerate(("fw", "bw")):
-                    gk = gks[di]
-                    dz = dxp[:, di * 4 * H:(di + 1) * 4 * H]
-                    gk[:D] += dwx[:, di * 4 * H:(di + 1) * 4 * H]
+                    dz = dxp[:, di * G:(di + 1) * G]
+                    rows = slice(di * Din, (di + 1) * Din) if split else slice(0, Din)
                     hprev = torch.zeros((B, L, H), dtype=torch.float32, device=out.device)
                     if di == 0:                       # carried (state-dropped) h of the previous forward step
                         hprev[:, 1:] = hst[:, :-1, :H]
                     else:
                         hprev[:, :-1] = hst[:, 1:, H:]
-                    gk[D:] += ops.wgrad_gemm(hprev.view(B * L, H), dz)            # dW_h = h_prev^T dz
+                    if cell == 'lstm':
+                        gks[di][:Din] += dwx[rows, di * G:(di + 1) * G]
+                        gks[di][Din:] += ops.wgrad_gemm(hprev.view(B * L, H), dz)   # dW_h = h_prev^T dz
+                    else:
+                        gc = store.grad(names[d][1][0])
+                        gks[di][:Din] += dwx[rows, di * G:di * G + 2 * H]
+                        gc[:Din] += dwx[rows, di * G + 2 * H:(di + 1) * G]
+                        gks[di][Din:] += ops.wgrad_gemm(hprev.view(B * L, H), dz[:, :2 * H])   # dW_g^h = h_prev^T da_g
+                        rh_d = rh.view(B * L, 2 * H)[:, di * H:(di + 1) * H]
+                        gc[Din:] += ops.wgrad_gemm(rh_d, dz[:, 2 * H:])                     # dW_c^h = (r h_prev)^T da_c
             if need_dx:
-                wx = torch.cat([store.vars[names[d][0]][:D] for d in ("fw", "bw")], dim=1)   # [D, 8H]: K-major for dx
+                wx = _rnn_input_kernel(_rnn_kernels(store, names), Din, split)       # [D, 2GH]: K-major for dx
                 Dn = (D + 31) // 32 * 32
                 wxp = torch.nn.functional.pad(wx, (0, 0, 0, Dn - D)).to(torch.bfloat16).contiguous()
                 dx = ops.gemm_bf16(dxp16, wxp, None, epilogue=ops.EPI_F32)[:, :D]

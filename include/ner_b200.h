@@ -428,6 +428,34 @@ int ner_bilstm_recurrence_bwd(const float* d_out, const float* gates, const floa
                               uint64_t seed, ner_stream_t stream);
 
 /* ------------------------------------------------------------------------ *
+ * BiGRU — tools/layer.py:10-41 bilstm(cell_type='gru') -> bidirectional_dynamic_rnn(GRUCell)
+ * ------------------------------------------------------------------------ */
+
+/* Sequential half of both directions of TF 1.14 GRUCell (r, u = sigmoid(split([x,h]·Wg + bg)); c = act([x, r⊙h]·Wc + bc);
+ * h' = u⊙h + (1-u)⊙c).  xproj [rows, 6H] f32 = x · [Wg_fw[:D] | Wc_fw[:D] | Wg_bw[:D] | Wc_bw[:D]] + biases (one
+ * ner_gemm_bf16 call) with row stride ld_xproj >= 6H (the GEMM needs N % 32 == 0: its weight pack is padded with zero
+ * columns when H % 16 != 0); wh_fw / wh_bw [H,3H] f32 = [gates/kernel[D:] | candidate/kernel[D:]] (columns r, u, c).
+ * out [B,L,2H] f32 = concat(fw, bw), zero for t >= seq_len.  activation: 0 tanh, 1 relu.  H % 4 == 0 and H small
+ * enough for the recurrent slice to fit an 8-CTA cluster (every H <= 256), else NER_ERR_UNSUPPORTED.  cu_seqlens as
+ * ner_bilstm_recurrence.  gates_out [B*L, 6H], hstate_out [B,L,2H], rh_out [B,L,2H]: all NULL (inference) or all given
+ * (training): post-activation r, u, c, the carried (state-dropped) h and r ⊙ h_prev (the operand of dW_c^h).
+ * keep_prob < 1: DropoutWrapper(output_keep_prob, state_keep_prob) with independent counter-based masks (seed) on the
+ * output and on the carried state, the masks of ner_bilstm_recurrence. */
+int ner_bigru_recurrence(const float* xproj, const float* wh_fw, const float* wh_bw, const int32_t* seq_len,
+                         float* out, int B, int L, int H, int ld_xproj, int activation,
+                         const int32_t* cu_seqlens, float* gates_out, float* hstate_out, float* rh_out, float keep_prob, uint64_t seed,
+                         ner_stream_t stream);
+
+/* Back-propagation through time of ner_bigru_recurrence (padded layout; TF GRUCell over tools/layer.py:10-41).
+ * d_out [B,L,2H]; gates [B*L, 6H] and hstate [B,L,2H] saved by the forward call.  Writes d_xproj [B*L, 6H] f32
+ * (columns da_r, da_u, da_c per direction; zeros for t >= seq_len).  The caller finishes with GEMMs / column sums over
+ * it: dW_x = x^T d_xproj, d_bias = colsum(d_xproj), dx = d_xproj W_x^T, dW_g^h = h_prev^T da_g, dW_c^h = (r⊙h_prev)^T
+ * da_c. */
+int ner_bigru_recurrence_bwd(const float* d_out, const float* gates, const float* hstate, const float* wh_fw,
+                             const float* wh_bw, const int32_t* seq_len, float* d_xproj, int B, int L, int H,
+                             int activation, float keep_prob, uint64_t seed, ner_stream_t stream);
+
+/* ------------------------------------------------------------------------ *
  * SoftLexicon gather-and-pool — model/bilstm_crf_softlexicon.py:37-44
  * ------------------------------------------------------------------------ */
 
