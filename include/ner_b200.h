@@ -639,12 +639,14 @@ int ner_bert_embed_bwd(const float* dx, const int32_t* ids, const int32_t* seg, 
                        ner_stream_t stream);
 /* Backward of ner_bert_attention (padded layout, head_dim 64): qkv / ctx from the forward pass,
  * dctx = dL/dctx; writes d_qkv (bf16, layout of qkv).  Scores are recomputed, nothing L x L is stored;
- * (keep_prob, seed) must be the forward call's so the dropout mask is regenerated. */
+ * (keep_prob, seed) must be the forward call's so the dropout mask is regenerated.  Any L: above 384 the kernels tile
+ * the keys and keep per-row statistics in d_qkv between launches, so d_qkv must not alias qkv, ctx or dctx. */
 int ner_bert_attention_bwd(const void* qkv_bf16, const int32_t* mask, const void* ctx_bf16,
                            const void* dctx_bf16, void* dqkv_bf16, int B, int L, int num_heads,
                            int head_dim, float scale, float mask_add, float keep_prob, uint64_t seed,
                            ner_stream_t stream);
-/* Packed layout: sequence b occupies rows [cu_seqlens[b], cu_seqlens[b+1]) of qkv / ctx / dctx / dqkv, every key valid. */
+/* Packed layout: sequence b occupies rows [cu_seqlens[b], cu_seqlens[b+1]) of qkv / ctx / dctx / dqkv, every key valid;
+ * L is the longest sequence.  Rows of dqkv past cu_seqlens[B] are not touched; dqkv must not alias qkv, ctx or dctx. */
 int ner_bert_attention_bwd_packed(const void* qkv_bf16, const int32_t* cu_seqlens, const void* ctx_bf16,
                                   const void* dctx_bf16, void* dqkv_bf16, int B, int L, int num_heads,
                                   int head_dim, float scale, float keep_prob, uint64_t seed,
