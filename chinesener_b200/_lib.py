@@ -55,6 +55,7 @@ SIGNATURES = {
     "ner_token_dice": (_i, [_vp] * 6 + [_c.c_float] * 3 + [_vp, _i, _i, _i, _vp]),
     "ner_mrc_pairs": (_i, [_vp] * 6 + [_i] * 6 + [_vp] * 7),
     "ner_mrc_merge": (_i, [_vp] * 3 + [_i] * 6 + [_vp, _vp]),
+    "ner_window_plan": (_i, [_vp] * 3 + [_i] * 5 + [_vp] * 6),
     "ner_layernorm_bwd": (_i, [_vp, _i] + [_vp] * 7 + [_i, _i, _c.c_float, _vp]),
     "ner_layernorm_dropout_bwd": (_i, [_vp, _i] + [_vp] * 7 + [_i, _i, _c.c_float, _c.c_float, _c.c_uint64, _vp]),
     "ner_layernorm_dropout_bwd_bias": (_i, [_vp, _i] + [_vp] * 8 + [_i, _i, _c.c_float, _c.c_float, _c.c_uint64, _vp]),

@@ -837,8 +837,13 @@ extern "C" int ner_crf_viterbi(const float* logits, const int32_t* seq_len, cons
     const int rc = ner_crf_viterbi_small(logits, seq_len, trans, tags_out, best_score, B, L, K, st);
     if (rc != NER_ERR_UNSUPPORTED) return rc;
   }
-#define CALL(KK) return launch_viterbi<KK>(logits, seq_len, trans, tags_out, best_score, B, L, st)
+  int rc = NER_ERR_UNSUPPORTED;
+#define CALL(KK) rc = launch_viterbi<KK>(logits, seq_len, trans, tags_out, best_score, B, L, st)
   NER_CRF_DISPATCH_K(K, CALL)
 #undef CALL
-  return NER_ERR_UNSUPPORTED;
+  // L past the throughput kernels' on-chip backpointers (document-length batches stacked past NER_CRF_SMALL_B rows): the
+  // lane-per-tag kernel keeps 32 + 4*SPW bytes per step on chip and serves any B
+  if (rc == NER_ERR_UNSUPPORTED && B > NER_CRF_SMALL_B)
+    rc = ner_crf_viterbi_small(logits, seq_len, trans, tags_out, best_score, B, L, K, st);
+  return rc;
 }

@@ -46,9 +46,11 @@ class Estimator:
         m = features.get('mask')
         if torch.is_tensor(m) and not m.is_cuda and 'mask' in out:
             # host-side token count rides along so sequence packing needs no device sync; the count of non-empty rows
-            # sizes the query/context pairs of bert_mrc the same way
-            out['mask'].total_tokens = int(m.sum())
-            out['mask'].nonempty_rows = int(m.any(1).sum())
+            # sizes the query/context pairs of bert_mrc the same way, and the per-row lengths the windows of document mode
+            lens = m.sum(1)
+            out['mask'].row_lengths = lens.numpy()
+            out['mask'].total_tokens = int(lens.sum())
+            out['mask'].nonempty_rows = int((lens > 0).sum())
         return out
 
     def predict_device(self, dev_features):
@@ -64,15 +66,40 @@ class Estimator:
                     return pred
         return self.forward_device(dev_features, False)[1]      # multi-task plugins return (loss, pred_ids, task_ids)
 
-    def forward_device(self, dev_features, is_training=False):
+    def document_window(self):
+        """-> (W, S) of the BERT plugins' document mode from params['bert_window'] / ['bert_window_stride'] (ValueError when
+        out of range), None for a plugin without BERT."""
+        if 'bert' not in self.model_name:
+            return None
+        from . import bert, windows
+        max_pos = bert.load_bert_config(self.params.get('pretrain_dir', ''))["max_position_embeddings"]
+        return windows.settings(self.params.get('bert_window'), self.params.get('bert_window_stride'), max_pos)
+
+    @contextlib.contextmanager
+    def _layer_settings(self, dev_features):
+        """The module settings of tools/layer.py this Estimator's params select, checked before anything is launched."""
+        from . import windows
         from .tools import layer
-        prec0 = layer.BERT_PRECISION
-        layer.BERT_PRECISION = self.params.get('bert_precision', prec0)
+        ws = self.document_window()
+        if ws is not None and torch.is_tensor(dev_features.get('token_ids')):
+            windows.check_batch(self.model_name, dev_features['token_ids'].shape[1], ws[0])
+        keys = ('BERT_PRECISION', 'BERT_WINDOW', 'BERT_WINDOW_STRIDE', 'DOCUMENT_REFUSAL')
+        saved = {k: getattr(layer, k) for k in keys}
+        layer.BERT_PRECISION = self.params.get('bert_precision', saved['BERT_PRECISION'])
+        if ws is not None:
+            layer.BERT_WINDOW, layer.BERT_WINDOW_STRIDE = ws
+            if self.model_name in windows.REFUSED:
+                layer.DOCUMENT_REFUSAL = (f"{self.model_name} cannot run BERT over sequences longer than bert_window = {ws[0]}: "
+                                          f"{windows.REFUSED[self.model_name]}")
         try:
-            with variables.use_store(self.store):
-                return self.build_graph(dev_features, None, self.params, is_training)
+            yield
         finally:
-            layer.BERT_PRECISION = prec0
+            for k, v in saved.items():
+                setattr(layer, k, v)
+
+    def forward_device(self, dev_features, is_training=False):
+        with self._layer_settings(dev_features), variables.use_store(self.store):
+            return self.build_graph(dev_features, None, self.params, is_training)
 
     def predict(self, features):
         """PREDICT mode on one host batch -> dict(pred_ids int32 [B,L] on host, label_ids, tokens)."""
@@ -85,7 +112,7 @@ class Estimator:
         at the summed batch size and each host part is copied straight into its row slice (pinned -> non-blocking)."""
         if len(feature_list) == 1:
             return self.to_device(feature_list[0])
-        out, total = {}, 0
+        out = {}
         first = feature_list[0]
         for k, v in first.items():
             if k in _DEVICE_KEYS and torch.is_tensor(v):
@@ -97,17 +124,18 @@ class Estimator:
                     dst[r:r + n].copy_(f[k], non_blocking=True)
                     r += n
                 out[k] = dst
-        nonempty = 0
+        lens = []
         for f in feature_list:
             m = f.get('mask')
             if not (torch.is_tensor(m) and not m.is_cuda):
-                total = None
+                lens = None
                 break
-            total += int(m.sum())
-            nonempty += int(m.any(1).sum())
-        if total is not None and 'mask' in out:
-            out['mask'].total_tokens = total
-            out['mask'].nonempty_rows = nonempty
+            lens.append(m.sum(1))
+        if lens is not None and 'mask' in out:
+            lens = torch.cat(lens)
+            out['mask'].row_lengths = lens.numpy()
+            out['mask'].total_tokens = int(lens.sum())
+            out['mask'].nonempty_rows = int((lens > 0).sum())
         return out
 
     def predict_iter(self, batches, depth=2, streams=1, group=1):
@@ -211,7 +239,7 @@ class Estimator:
         from .tools import train_utils
         dev = features if all(not torch.is_tensor(v) or v.is_cuda for v in features.values()) else self.to_device(features)
         self.store.dropout_calls = 0
-        with variables.use_store(self.store), autodiff.recording(self.store) as tape:
+        with self._layer_settings(dev), variables.use_store(self.store), autodiff.recording(self.store) as tape:
             loss = self.build_graph(dev, None, self.params, True)[0]
             tape.backward()
             p = self.params

@@ -125,6 +125,7 @@ def singletask_train(args):
         TRAIN_PARAMS['pretrain_dir'] = args.pretrain_dir
     if args.batch_size:
         TRAIN_PARAMS['batch_size'] = args.batch_size
+    _window_params(TRAIN_PARAMS, args)
     input_pipe = NerDataset(data_dir, TRAIN_PARAMS['batch_size'], TRAIN_PARAMS['epoch_size'], model_name, seed=args.seed)
     TRAIN_PARAMS.update(input_pipe.params)       # label_size, max_seq_len, num_train_steps ... (main.py:25)
     print('=' * 10 + 'TRAIN PARAMS' + '=' * 10)
@@ -185,6 +186,7 @@ def multitask_train(args):
         TRAIN_PARAMS['pretrain_dir'] = args.pretrain_dir
     if args.batch_size:
         TRAIN_PARAMS['batch_size'] = args.batch_size
+    _window_params(TRAIN_PARAMS, args)
     input_pipe = MultiDataset(data_root, data_list, TRAIN_PARAMS['batch_size'], TRAIN_PARAMS['epoch_size'], model_name, seed=args.seed)
     TRAIN_PARAMS.update(input_pipe.params)       # per-dataset params, task_list, step_per_epoch, num_train_steps, max_seq_len
     print('=' * 10 + 'TRAIN PARAMS' + '=' * 10)
@@ -244,7 +246,18 @@ def build_parser():
     parser.add_argument('--max_steps', type=int, default=None)
     parser.add_argument('--seed', type=int, default=1234)
     parser.add_argument('--report', type=str, default='', help='write a JSON summary (eval history + test F1) here')
+    parser.add_argument('--bert_window', type=int, default=0, help='override params["bert_window"]: BERT plugins encode '
+                        'longer batches as overlapping windows of this many tokens (default max_position_embeddings)')
+    parser.add_argument('--bert_window_stride', type=int, default=0, help='override params["bert_window_stride"]: content '
+                        'tokens between window starts (default (bert_window - 2) // 2)')
     return parser
+
+
+def _window_params(params, args):
+    """--bert_window / --bert_window_stride over the params (read with params.get by the BERT plugins' document mode)."""
+    for k in ('bert_window', 'bert_window_stride'):
+        if getattr(args, k, 0):
+            params[k] = getattr(args, k)
 
 
 def main(argv=None):

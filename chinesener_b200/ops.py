@@ -610,6 +610,26 @@ def mrc_merge(logits, seq_len, type_tag, o_id, cls_id, sep_id):
     return pred
 
 
+# --------------------------------------------------------------------------- document windows (BERT document mode)
+def window_plan(token_ids, segment_ids, seq_len, W, S, NW, n_doc, packed=False, padded=False):
+    """[B, L] documents -> their W-token windows (ner_window_plan): dict of ids / segment_ids / mask [NW, W] i32 and the
+    owner row of every document token (n_doc of them, documents back to back) in the window-packed layout
+    (doc_src_packed, when packed) and the window-padded one (doc_src_padded, when padded).  NW and n_doc are host counts
+    (windows.window_counts and the mask's token count)."""
+    require_cuda(token_ids, segment_ids, seq_len)
+    B, L = token_ids.shape
+    token_ids, seq_len = _i32(token_ids), _i32(seq_len)
+    segment_ids = None if segment_ids is None else _i32(segment_ids)
+    dev = token_ids.device
+    i32 = lambda *shape: torch.empty(shape, dtype=torch.int32, device=dev)
+    out = dict(ids=i32(NW, W), segment_ids=i32(NW, W), mask=i32(NW, W), doc_src_packed=i32(n_doc) if packed else None,
+               doc_src_padded=i32(n_doc) if padded else None)
+    check(lib().ner_window_plan(ptr(token_ids), ptr(segment_ids), ptr(seq_len), B, L, int(W), int(S), int(NW), ptr(out['ids']),
+                                ptr(out['segment_ids']), ptr(out['mask']), ptr(out['doc_src_packed']),
+                                ptr(out['doc_src_padded']), stream()))
+    return out
+
+
 # --------------------------------------------------------------------------- training-side kernels
 def _require_rows(x2d):
     """CUDA f32 2-D tensor whose rows are contiguous (a column slice of a wider buffer is fine)."""

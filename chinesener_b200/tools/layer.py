@@ -9,6 +9,7 @@ import torch
 from .. import autodiff
 from .. import bert as _bert
 from .. import ops, variables
+from .. import windows as _windows
 
 # Remove padding rows from the token-major activations of the BERT plugins (exact for loss and
 # pred_ids: the CRF never reads t >= seq_len).  NER_B200_PACK=0 keeps the padded layout.
@@ -20,6 +21,13 @@ TRAIN_PACK = os.environ.get("NER_B200_TRAIN_PACK", "1") != "0"
 # the QKV and FFN GEMMs on block-scaled e4m3 wgmma (bert.bert_forward_fp8; TRAIN ignores it, as it does 'fp32').
 # Estimator sets it from params['bert_precision'] around build_graph.
 BERT_PRECISION = os.environ.get("NER_B200_BERT_PRECISION", "bf16")
+# Document mode (chinesener_b200/windows.py): a batch longer than the window W is encoded as overlapping windows and stitched
+# back.  None = the defaults (W = max_position_embeddings, S = (W - 2) // 2).  Estimator sets both from
+# params['bert_window'] / params['bert_window_stride'], and DOCUMENT_REFUSAL to the reason a plugin cannot take document
+# mode (windows.REFUSED), around build_graph.
+BERT_WINDOW = None
+BERT_WINDOW_STRIDE = None
+DOCUMENT_REFUSAL = None
 
 
 class TrainingPathNotBuilt(NotImplementedError):
@@ -30,10 +38,17 @@ def pretrain_bert_embedding(input_ids, input_mask, segment_ids, pretrain_dir, dr
     """reference tools/layer.py:63-81 — BertModel(...).get_sequence_output() (+ dropout when training).
 
     Returns sequence_output [B,L,H] f32; its bf16 copy (what the next GEMM consumes) rides along
-    as attribute `.bf16`.
+    as attribute `.bf16`.  A batch longer than the window takes document mode (_document_embedding), with the same
+    output layouts.
     """
     cfg = _bert.load_bert_config(pretrain_dir)
     B, L = input_ids.shape
+    W, S = _windows.settings(BERT_WINDOW, BERT_WINDOW_STRIDE, cfg["max_position_embeddings"])
+    if L > W:
+        if DOCUMENT_REFUSAL:
+            raise ValueError(DOCUMENT_REFUSAL)
+        _windows.check_batch(None, L, W)
+        return _document_embedding(input_ids, input_mask, segment_ids, cfg, W, S, drop_out, is_training)
     if is_training:
         tape = autodiff.current()
         if tape is None:
@@ -55,6 +70,62 @@ def pretrain_bert_embedding(input_ids, input_mask, segment_ids, pretrain_dir, dr
     x32, x16 = forward(input_ids, input_mask, segment_ids, cfg)
     emb = x32.view(B, L, -1)
     emb.bf16 = x16.view(B, L, -1)
+    return emb
+
+
+def _document_embedding(input_ids, input_mask, segment_ids, cfg, W, S, drop_out, is_training):
+    """Document mode of pretrain_bert_embedding: ner_window_plan cuts the documents into W-token windows, the encoder of
+    the current mode runs on the window batch, and row gathers take each document token's row from its owner window.
+    The result has the layouts of the plain path: packed [total_tokens, H] with .bf16 and .pack of the document mask, or
+    [B, L, H] with zero rows at [PAD] (padded, fp32 and TRAIN).  TRAIN's stitch backward scatters each document row's
+    gradient to its owner window row; window rows that own no token get zero."""
+    B, L = input_ids.shape
+    lengths = getattr(input_mask, "row_lengths", None)
+    if lengths is None:
+        lengths = input_mask.sum(1).cpu()                 # device sync; engine.Estimator attaches the host lengths
+    NW, n_win = _windows.window_counts(lengths, W, S)
+    n_doc = int(getattr(input_mask, "total_tokens", None) or sum(int(n) for n in lengths))
+    doc_pack = _bert.make_pack(input_mask, n_doc)
+    seq_len = input_mask.sum(1, dtype=torch.int32)
+    train_pack = is_training and PACK_SEQUENCES and TRAIN_PACK and not _bert.PER_KERNEL
+    packed = not is_training and PACK_SEQUENCES and BERT_PRECISION != 'fp32'
+    plan = ops.window_plan(input_ids, segment_ids, seq_len, W, S, NW, n_doc, packed=packed, padded=not packed)
+    ids, mask, seg = plan['ids'], plan['mask'], plan['segment_ids']
+    mask.total_tokens = n_win
+
+    def to_doc(rows, src):
+        """window rows -> [B, L, H], zero at [PAD]"""
+        H = rows.shape[-1]
+        return ops.scatter_rows(ops.gather_rows(rows.reshape(-1, H), src, n_doc), doc_pack.tok_src, B * L).view(B, L, H)
+
+    if is_training:
+        tape = autodiff.current()
+        if tape is None:
+            raise TrainingPathNotBuilt("pretrain_bert_embedding(is_training=True) needs an autodiff tape (engine.train_step)")
+        win_pack = _bert.make_pack(mask, n_win) if train_pack else None
+        win = _bert.bert_forward_train(ids, mask, seg, cfg, variables.default_store(), tape, pack=win_pack)
+        src = plan['doc_src_padded']
+        emb = to_doc(win, src)
+        n_rows, H = NW * W, win.shape[-1]
+
+        def bwd(g):
+            if g is not None:
+                g_doc = ops.gather_rows(g.reshape(-1, H).contiguous(), doc_pack.tok_src, n_doc)
+                tape.add_grad(win, ops.scatter_rows(g_doc, src, n_rows).view(win.shape))
+        tape.record(emb, bwd)
+        return dropout(emb, rate=drop_out, is_training=True, seed=1234)
+    if BERT_PRECISION == 'fp32':
+        return to_doc(_bert.bert_forward_f32(ids, mask, seg, cfg), plan['doc_src_padded'])
+    forward = _bert.bert_forward_fp8 if BERT_PRECISION == 'fp8' else _bert.bert_forward
+    if packed:
+        x32, x16 = forward(ids, mask, seg, cfg, pack=_bert.make_pack(mask, n_win))
+        src = plan['doc_src_packed']
+        emb = ops.gather_rows(x32, src, n_doc)
+        emb.bf16, emb.pack = ops.gather_rows(x16, src, n_doc), doc_pack
+        return emb
+    x32, x16 = forward(ids, mask, seg, cfg)
+    emb = to_doc(x32, plan['doc_src_padded'])
+    emb.bf16 = to_doc(x16, plan['doc_src_padded'])
     return emb
 
 

@@ -577,6 +577,24 @@ int ner_mrc_pairs(const int32_t* token_ids, const int32_t* seq_len, const int32_
  * T in [1, 32] (T > 32: NER_ERR_UNSUPPORTED), B*T*L < 2^31.  One launch. */
 int ner_mrc_merge(const float* logits, const int32_t* seq_len, const int32_t* type_tag, int B, int L, int T, int o_id,
                   int cls_id, int sep_id, int32_t* pred_ids, ner_stream_t stream);
+/* Window plan of the BERT plugins' document mode (documents longer than the position table).  Document b of the [B,L]
+ * batch has n_b = clamp(seq_len[b], 0, L) tokens ([CLS] ... [SEP]), m = n_b - 2 content tokens; C = W - 2.
+ *   n_b = 0: no window;  n_b <= W: one window, the document itself (its rows past n_b are [PAD]);
+ *   n_b > W: nw_b = 1 + ceil((m - C) / S) windows; window k starts at content offset a_k = min(k*S, m - C) and holds doc
+ *   positions 0, 1 + a_k ... a_k + C, n_b - 1 (W tokens).
+ * Windows are numbered document by document.  win_ids / win_segment_ids / win_mask [NW, W] i32 get the gathered
+ * token_ids / segment_ids (segment_ids may be NULL: zeros) and a prefix mask; rows past the plan's windows are zero.
+ * Owner of doc position t: row 0 of window 0 for t = 0, row W - 1 of the last window for t = n_b - 1; content index
+ * c = t - 1 goes to the window with a_k <= c < a_k + C maximising min(c - a_k, a_k + C - 1 - c), the lowest k on a tie.
+ * doc_src_padded [sum n_b] (nullable) = w*W + p of the owner (window w, row p), doc_src_packed [sum n_b] (nullable) = the
+ * owner's row in the window-packed layout (windows back to back, n_b rows for a one-window document, W otherwise); both
+ * indexed by the document's packed order (documents back to back, n_b rows each).
+ * NW must be sum_b nw_b (windows past NW are not written).  No output may alias another output or an input.
+ * W >= 3, 1 <= S <= W - 2, B, NW >= 0, L >= 1 and null token_ids / seq_len / window outputs are NER_ERR_INVALID_ARG;
+ * NW*W or B*L >= 2^31 is NER_ERR_UNSUPPORTED; all before any CUDA call.  One launch, no atomics, bit-identical repeats. */
+int ner_window_plan(const int32_t* token_ids, const int32_t* segment_ids, const int32_t* seq_len, int B, int L, int W, int S,
+                    int NW, int32_t* win_ids, int32_t* win_segment_ids, int32_t* win_mask, int32_t* doc_src_packed,
+                    int32_t* doc_src_padded, ner_stream_t stream);
 /* dst[i] += a * src[i]. */
 int ner_axpy_f32(float* dst, const float* src, size_t n, float a, ner_stream_t stream);
 /* out[0] += sum(g^2)  (tf.clip_by_global_norm, tools/train_utils.py:315).  Deterministic (no float atomics): per-CTA partial
