@@ -55,6 +55,15 @@ SIGNATURES = {
     "ner_token_dice": (_i, [_vp] * 6 + [_c.c_float] * 3 + [_vp, _i, _i, _i, _vp]),
     "ner_mrc_pairs": (_i, [_vp] * 6 + [_i] * 6 + [_vp] * 7),
     "ner_mrc_merge": (_i, [_vp] * 3 + [_i] * 6 + [_vp, _vp]),
+    "ner_mrc_span_targets": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
+    "ner_mrc_span_match_fwd_workspace_bytes": (_c.c_size_t, [_i, _i]),
+    "ner_mrc_span_match_fwd": (_i, [_vp, _i] + [_vp] * 5 + [_i] * 3 + [_c.c_float, _c.c_uint64] + [_vp] * 3
+                               + [_c.c_size_t, _vp]),
+    "ner_mrc_span_match_bwd_workspace_bytes": (_c.c_size_t, [_i, _i]),
+    "ner_mrc_span_match_bwd": (_i, [_vp, _i] + [_vp] * 5 + [_i] * 3 + [_c.c_float, _c.c_float, _c.c_uint64] + [_vp] * 5
+                               + [_c.c_size_t, _vp]),
+    "ner_mrc_span_decode_workspace_bytes": (_c.c_size_t, [_i, _i]),
+    "ner_mrc_span_decode": (_i, [_vp] * 3 + [_i] + [_vp] * 5 + [_i] * 8 + [_vp] * 5 + [_c.c_size_t, _vp]),
     "ner_window_plan": (_i, [_vp] * 3 + [_i] * 5 + [_vp] * 6),
     "ner_layernorm_bwd": (_i, [_vp, _i] + [_vp] * 7 + [_i, _i, _c.c_float, _vp]),
     "ner_layernorm_dropout_bwd": (_i, [_vp, _i] + [_vp] * 7 + [_i, _i, _c.c_float, _c.c_float, _c.c_uint64, _vp]),

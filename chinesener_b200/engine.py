@@ -102,10 +102,16 @@ class Estimator:
             return self.build_graph(dev_features, None, self.params, is_training)
 
     def predict(self, features):
-        """PREDICT mode on one host batch -> dict(pred_ids int32 [B,L] on host, label_ids, tokens)."""
+        """PREDICT mode on one host batch -> dict(pred_ids int32 [B,L] on host, label_ids, tokens), and 'pred_spans' (per
+        sentence a list of (type name, start, end_exclusive, probability)) when the plugin's pred_ids carries spans."""
         dev = self.to_device(features)
         pred_ids = self.predict_device(dev)
-        return {'pred_ids': pred_ids.cpu(), 'label_ids': features.get('label_ids'), 'tokens': features.get('tokens')}
+        out = {'pred_ids': pred_ids.cpu(), 'label_ids': features.get('label_ids'), 'tokens': features.get('tokens')}
+        from .tools.infer_utils import span_lists
+        spans = span_lists(pred_ids)
+        if spans is not None:
+            out['pred_spans'] = spans
+        return out
 
     def stack_to_device(self, feature_list):
         """Several host batches -> ONE device batch (rows concatenated in order): every device feature is allocated once

@@ -46,13 +46,20 @@ class InferHelper(object):
     def infer(self, text):
         feature = self.make_feature(text)
         out = self.estimator.predict(features_to_batch([feature]))
+        if 'pred_spans' in out:                  # span-pointer plugin: every (possibly nested) span, not the tag scan
+            from .tools.infer_utils import span_entities
+            return span_entities([feature['tokens']], out['pred_spans'])[0]
         return self.decode_prediction(out['pred_ids'].numpy())
 
     def infer_batch(self, texts):
         """Many sentences per call: one PREDICT batch, the tag scan of extract_entity on the GPU (ner_extract_spans) —
-        the tag tensor stays on the device, only the spans come back.  -> one entity dict per text, as infer() gives."""
-        from .tools.infer_utils import extract_entity_device
+        the tag tensor stays on the device, only the spans come back.  -> one entity dict per text, as infer() gives.
+        A span-pointer plugin (bert_mrc_span) returns its own spans instead, nested and overlapping ones included."""
+        from .tools.infer_utils import extract_entity_device, span_entities, span_lists
         feats = [dict(self.make_feature(t)) for t in texts]
         dev = self.estimator.to_device(features_to_batch(feats, pin_memory=True))
         pred = self.estimator.predict_device(dev)
+        spans = span_lists(pred)
+        if spans is not None:
+            return span_entities([f['tokens'] for f in feats], spans)
         return extract_entity_device([f['tokens'] for f in feats], pred, self.idx2tag)

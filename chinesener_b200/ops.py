@@ -610,6 +610,108 @@ def mrc_merge(logits, seq_len, type_tag, o_id, cls_id, sep_id):
     return pred
 
 
+# --------------------------------------------------------------------------- MRC span pointer (bert_mrc_span)
+_span_workspace = {}
+
+
+def _span_scratch(kind, nbytes, dev):
+    """Workspace of one ner_mrc_span_* entry point: one growing buffer per (kind, device, stream)."""
+    key = (kind, dev.index, stream())
+    buf = _span_workspace.get(key)
+    if buf is None or buf.numel() < nbytes:
+        buf = _span_workspace[key] = torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=dev)
+    return buf
+
+
+def _span_uv(uv):
+    """[P*L, >= 2I] f32 U | V rows with contiguous rows -> (row stride, I is implied by the caller)."""
+    if not uv.is_cuda:
+        raise NerB200Error("ner_b200 kernels take CUDA tensors (got a CPU tensor); there is no CPU path")
+    assert uv.dtype == torch.float32 and uv.dim() == 2 and uv.stride(1) == 1
+    return uv.stride(0)
+
+
+def mrc_span_targets(pair_labels, pair_seq_len):
+    """Per-type BIO labels [P, L] -> (start_y, end_y, span_end) [P, L] i32 (ner_mrc_span_targets)."""
+    require_cuda(pair_labels, pair_seq_len)
+    P, L = pair_labels.shape
+    pair_labels, pair_seq_len = _i32(pair_labels), _i32(pair_seq_len)
+    out = [torch.empty((P, L), dtype=torch.int32, device=pair_labels.device) for _ in range(3)]
+    check(lib().ner_mrc_span_targets(ptr(pair_labels), ptr(pair_seq_len), P, L, *(ptr(t) for t in out), stream()))
+    return tuple(out)
+
+
+def mrc_span_match_fwd(uv, b1, w2, b2, pair_seq_len, L, span_end=None, keep_prob=1.0, seed=0):
+    """Match logits z [P, L, L] f32 (0 off the candidates) and, with span_end, the mean BCE loss [] f32 over the batch's
+    candidates (ner_mrc_span_match_fwd).  uv [P*L, >= 2I] f32 (U | V), b1 / w2 [I], b2 [1]."""
+    require_cuda(b1, w2, b2, pair_seq_len, span_end)
+    ld = _span_uv(uv)
+    I = b1.numel()
+    P = pair_seq_len.numel()
+    dev = uv.device
+    z = torch.empty((P, L, L), dtype=torch.float32, device=dev)
+    loss = torch.empty((), dtype=torch.float32, device=dev) if span_end is not None else None
+    ws, nbytes = None, 0
+    if loss is not None:
+        nbytes = int(lib().ner_mrc_span_match_fwd_workspace_bytes(P, L))
+        ws = _span_scratch('fwd', nbytes, dev)
+    check(lib().ner_mrc_span_match_fwd(ptr(uv), ld, ptr(b1), ptr(w2), ptr(b2), ptr(_i32(pair_seq_len)),
+                                       ptr(None if span_end is None else _i32(span_end)), P, L, I, float(keep_prob),
+                                       int(seed) & 0xFFFFFFFFFFFFFFFF, ptr(z), ptr(loss), ptr(ws), nbytes, stream()))
+    if P == 0 and loss is not None:
+        loss.zero_()
+    return z, loss
+
+
+def mrc_span_match_bwd(uv, z, b1, w2, pair_seq_len, span_end, d_loss=1.0, keep_prob=1.0, seed=0):
+    """-> (d_uv [P*L, 2I], d_b1 [I], d_w2 [I], d_b2 [1]) f32 of d_loss * the forward's loss (ner_mrc_span_match_bwd)."""
+    require_cuda(z, b1, w2, pair_seq_len, span_end)
+    ld = _span_uv(uv)
+    I = b1.numel()
+    P, L, _ = z.shape
+    dev = uv.device
+    d_uv = torch.empty((P * L, 2 * I), dtype=torch.float32, device=dev)
+    d_b1 = torch.empty((I,), dtype=torch.float32, device=dev)
+    d_w2 = torch.empty((I,), dtype=torch.float32, device=dev)
+    d_b2 = torch.empty((1,), dtype=torch.float32, device=dev)
+    nbytes = int(lib().ner_mrc_span_match_bwd_workspace_bytes(P, I))
+    ws = _span_scratch('bwd', nbytes, dev)
+    check(lib().ner_mrc_span_match_bwd(ptr(uv), ld, ptr(z), ptr(b1), ptr(w2), ptr(_i32(pair_seq_len)), ptr(_i32(span_end)), P, L,
+                                       I, float(d_loss), float(keep_prob), int(seed) & 0xFFFFFFFFFFFFFFFF, ptr(d_uv), ptr(d_b1),
+                                       ptr(d_w2), ptr(d_b2), ptr(ws), nbytes, stream()))
+    if P == 0:
+        for t in (d_uv, d_b1, d_w2, d_b2):
+            t.zero_()
+    return d_uv, d_b1, d_w2, d_b2
+
+
+def mrc_span_decode(start_logits, end_logits, uv, b1, w2, b2, seq_len, type_tag, o_id, cls_id, sep_id, cap=None):
+    """Start / end logits [B*T, L, 2] f32 and U | V rows -> pred_ids [B, L] i32 carrying .spans [B, cap] i32,
+    .span_probs [B, cap] f32 and .span_counts [B] i32 (ner_mrc_span_decode).  cap None = L."""
+    require_cuda(start_logits, end_logits, b1, w2, b2, seq_len, type_tag)
+    assert start_logits.dtype == torch.float32 and end_logits.dtype == torch.float32
+    ld = _span_uv(uv)
+    T = type_tag.shape[0]
+    P, L, _ = start_logits.shape
+    B = P // T
+    I = b1.numel()
+    cap = L if cap is None else int(cap)
+    dev = start_logits.device
+    pred = torch.empty((B, L), dtype=torch.int32, device=dev)
+    spans = torch.empty((B, cap), dtype=torch.int32, device=dev)
+    probs = torch.empty((B, cap), dtype=torch.float32, device=dev)
+    counts = torch.empty((B,), dtype=torch.int32, device=dev)
+    nbytes = int(lib().ner_mrc_span_decode_workspace_bytes(P, L))
+    ws = _span_scratch('decode', nbytes, dev)
+    check(lib().ner_mrc_span_decode(ptr(start_logits.contiguous()), ptr(end_logits.contiguous()), ptr(uv), ld, ptr(b1), ptr(w2),
+                                    ptr(b2), ptr(_i32(seq_len)), ptr(type_tag), B, T, L, I, int(o_id), int(cls_id), int(sep_id),
+                                    cap, ptr(pred), ptr(spans), ptr(probs), ptr(counts), ptr(ws), nbytes, stream()))
+    if B == 0:
+        counts.zero_()
+    pred.spans, pred.span_probs, pred.span_counts = spans, probs, counts
+    return pred
+
+
 # --------------------------------------------------------------------------- document windows (BERT document mode)
 def window_plan(token_ids, segment_ids, seq_len, W, S, NW, n_doc, packed=False, padded=False):
     """[B, L] documents -> their W-token windows (ner_window_plan): dict of ids / segment_ids / mask [NW, W] i32 and the

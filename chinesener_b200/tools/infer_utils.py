@@ -51,6 +51,37 @@ def fix_tokens(sentence, tokens):
     return tokens
 
 
+def span_lists(pred_ids):
+    """The spans a span-pointer plugin (bert_mrc_span) attaches to its device pred_ids -> per sentence a list of
+    (type name, start, end_exclusive, probability), ordered by (start, end, type); None when pred_ids carries no spans."""
+    spans = getattr(pred_ids, 'spans', None)
+    if spans is None:
+        return None
+    names = pred_ids.span_types
+    counts = pred_ids.span_counts.cpu().numpy()
+    words, probs = spans.cpu().numpy(), pred_ids.span_probs.cpu().numpy()
+    out = []
+    for b in range(len(counts)):
+        n = min(int(counts[b]), words.shape[1])
+        out.append([(names[int(w) >> 24], int(w) & 0xFFF, (int(w) >> 12) & 0xFFF, float(p))
+                    for w, p in zip(words[b, :n], probs[b, :n])])
+    return out
+
+
+def span_entities(tokens_batch, spans_batch):
+    """Per sentence {type: set of surface strings} from span_lists' output, by the host join of extract_entity_device:
+    overlapping and nested entities are all returned."""
+    out = []
+    for toks, spans in zip(tokens_batch, spans_batch):
+        found = defaultdict(set)
+        for name, s, e, _ in spans:
+            text = ''.join(toks[s:e])
+            if text != '':
+                found[name].add(text)
+        out.append(found)
+    return out
+
+
 def extract_entity_device(tokens_batch, pred_ids, idx2tag, _cache={}):
     """Batched extract_entity with the tag scan on the GPU (ner_extract_spans): pred_ids [B, L] int32 on the device,
     tokens_batch B lists of L token strings -> list of {type: set of surface strings}, equal to

@@ -15,6 +15,7 @@ REFUSED = {
     'bert_ce': "its PREDICT argmax covers [PAD] positions",
     'bert_dice': "its PREDICT argmax covers [PAD] positions",
     'bert_mrc': "its query/context pairs would need the query repeated in every window",
+    'bert_mrc_span': "its query/context pairs would need the query repeated in every window",
 }
 
 

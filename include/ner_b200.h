@@ -577,6 +577,54 @@ int ner_mrc_pairs(const int32_t* token_ids, const int32_t* seq_len, const int32_
  * T in [1, 32] (T > 32: NER_ERR_UNSUPPORTED), B*T*L < 2^31.  One launch. */
 int ner_mrc_merge(const float* logits, const int32_t* seq_len, const int32_t* type_tag, int B, int L, int T, int o_id,
                   int cls_id, int sep_id, int32_t* pred_ids, ner_stream_t stream);
+/* model/bert_mrc_span.py: the span-pointer MRC model (Li et al., ACL 2020) over the bert_mrc pairs p = b*T + t, each with
+ * the sentence-aligned rows [L, H] of ner_mrc_pairs / ner_gather_rows, len_p = clamp(pair_seq_len[p], 0, L), m_p = len_p-2.
+ * Candidates are the (i, j) with 1 <= i <= j <= m_p (sentence content, no [CLS] / [SEP]).  Common rules: L <= 511, I % 32 == 0
+ * and I <= 4096, T <= 32, else NER_ERR_UNSUPPORTED; P*L*L < 2^31; P = 0 / B = 0 is a no-op; every check runs before any CUDA
+ * call; no allocation, no float atomics, bit-identical repeats.
+ *
+ * Targets from the per-type BIO labels y [P, L] of ner_mrc_pairs (0 O, 1 B, 2 I): start_y[p,s] = [s < len_p and y = 1];
+ * span_end[p,s] = r(s), the last j >= s, j < len_p, with y[s+1..j] all 2, for a start s, else -1; end_y[p,j] = [j = r(s) for
+ * some start s].  An I-run without a B in front gives no span.  All three [P, L] i32, fully written.  One launch. */
+int ner_mrc_span_targets(const int32_t* pair_labels, const int32_t* pair_seq_len, int P, int L, int32_t* start_y,
+                         int32_t* end_y, int32_t* span_end, ner_stream_t stream);
+/* Match head forward.  uv [P*L, ld_uv] f32 is the projection GEMM's output as it lies: row p*L + s holds U[p,s,0:I] in
+ * columns [0, I) and V[p,s,0:I] in [I, 2I) (ld_uv >= 2I, ld_uv % 4 == 0; uv, b1, w2 16-byte aligned).  b1 [I], w2 [I], b2 [1].
+ *   z[p,i,j] = b2 + sum_k w2[k] * m_k / keep * GELU_tanh(U[p,i,k] + V[p,j,k] + b1[k])   (k ascending, fp32; tanh.approx)
+ * with m_k = [hash3(lo(seed), hi(seed) ^ (p*L + i), j*I + k) < keep * 2^32] (common.cuh) when keep_prob < 1, else 1.
+ * z [P, L, L] f32 is written everywhere: the logit at the candidates, 0 elsewhere.  loss [1] (nullable) = mean over every
+ * candidate of the batch of BCE-with-logits(z, [j = span_end[p,i]]) (span_end required then), 0 without candidates; the
+ * candidate count is taken on the device; per-tile partials in workspace (>= ner_mrc_span_match_fwd_workspace_bytes)
+ * summed in index order.  keep_prob in (0, 1]. */
+size_t ner_mrc_span_match_fwd_workspace_bytes(int P, int L);
+int ner_mrc_span_match_fwd(const float* uv, int ld_uv, const float* b1, const float* w2, const float* b2,
+                           const int32_t* pair_seq_len, const int32_t* span_end, int P, int L, int I, float keep_prob,
+                           uint64_t seed, float* z, float* loss, void* workspace, size_t workspace_bytes, ner_stream_t stream);
+/* Its backward for loss * d_loss: dz = d_loss / N * (sigmoid(z) - y) at the candidates (N the candidate count), the GELU' and
+ * the dropout mask recomputed from uv, b1, w2 and the forward's (keep_prob, seed).  Writes d_uv [P*L, 2I] f32 (dU | dV, 0
+ * off the candidate rows), d_b1 [I], d_w2 [I], d_b2 [1] (overwritten, not accumulated).  The sums over j, over i and over
+ * the pairs have one owner each or are per-CTA partials in workspace (>= ner_mrc_span_match_bwd_workspace_bytes) added in
+ * pair order.  Three launches. */
+size_t ner_mrc_span_match_bwd_workspace_bytes(int P, int I);
+int ner_mrc_span_match_bwd(const float* uv, int ld_uv, const float* z, const float* b1, const float* w2,
+                           const int32_t* pair_seq_len, const int32_t* span_end, int P, int L, int I, float d_loss,
+                           float keep_prob, uint64_t seed, float* d_uv, float* d_b1, float* d_w2, float* d_b2, void* workspace,
+                           size_t workspace_bytes, ner_stream_t stream);
+/* PREDICT / EVAL decode of B sentences (seq_len [B]; P = B*T pairs, pair p = b*T + t).  start_logits / end_logits [P, L, 2]
+ * f32: s is a start (end) of type t when 1 <= s <= m and its two logits' first argmax is 1.  z is computed (bit-identical to
+ * ner_mrc_span_match_fwd at keep 1) only for start i <= end j; a span (i, j, t) is kept when z > 0, with probability
+ * sigmoid(z).  spans [B, cap] i32 = i | (j + 1) << 12 | t << 24 (ner_extract_spans' word), span_probs [B, cap] f32, ordered
+ * by (start, end, type); span_counts [B] = the true count (spans past cap are dropped; slots past the count are 0).  pred_ids [B, L]:
+ * the greedy non-overlapping projection of all spans of the sentence (descending z, then lower type, start, end; a span
+ * overlapping a kept one is skipped), B-X_t at i and I-X_t on i+1..j by type_tag [T, 2], o_id elsewhere in 1..len-2;
+ * cls_id at 0, sep_id at len - 1, 0 from len on (ner_mrc_merge's rules).  workspace >=
+ * ner_mrc_span_decode_workspace_bytes(B*T, L).  cap >= 0 (spans / span_probs may be NULL when cap = 0).  Three launches. */
+size_t ner_mrc_span_decode_workspace_bytes(int P, int L);
+int ner_mrc_span_decode(const float* start_logits, const float* end_logits, const float* uv, int ld_uv, const float* b1,
+                        const float* w2, const float* b2, const int32_t* seq_len, const int32_t* type_tag, int B, int T, int L,
+                        int I, int o_id, int cls_id, int sep_id, int cap, int32_t* pred_ids, int32_t* spans,
+                        float* span_probs, int32_t* span_counts, void* workspace, size_t workspace_bytes,
+                        ner_stream_t stream);
 /* Window plan of the BERT plugins' document mode (documents longer than the position table).  Document b of the [B,L]
  * batch has n_b = clamp(seq_len[b], 0, L) tokens ([CLS] ... [SEP]), m = n_b - 2 content tokens; C = W - 2.
  *   n_b = 0: no window;  n_b <= W: one window, the document itself (its rows past n_b are [PAD]);
