@@ -21,6 +21,7 @@ SIGNATURES = {
     "ner_abi_version": (_i, []),
     "ner_build_info": (_c.c_char_p, []),
     "ner_crf_viterbi": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "ner_crf_viterbi_plan": (_i, [_i, _i, _i, _i, _i]),
     "ner_crf_loglik_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "ner_crf_loglik_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c.c_float, _vp, _vp, _i, _i, _i, _vp]),
     "ner_gemm_bf16": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
@@ -166,6 +167,9 @@ SIGNATURES["ner_lexicon_create"] = (_vp, [_vp, _vp, _vp, _i])
 SIGNATURES["ner_lexicon_destroy"] = (None, [_vp])
 SIGNATURES["ner_lexicon_num_nodes"] = (_c.c_int64, [_vp])
 SIGNATURES["ner_lexicon_build"] = (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _i])
+
+# return values of ner_crf_viterbi_plan, by enum value (include/ner_b200.h: NER_VIT_*)
+VIT_PLANS = ("small", "tma", "parked", "onchip_128", "onchip_32", "small_any_b", "none")
 
 _lib = None
 

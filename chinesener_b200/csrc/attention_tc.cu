@@ -206,25 +206,6 @@ bert_attention_tc_kernel(const __grid_constant__ CUtensorMap tma_qkv, const int3
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-    (void)cudaGetLastError();
-  }
-  return fn;
-}
-
 template <int NKMAX>
 int launch(const CUtensorMap& map, const int32_t* mask, void* ctx, int B, int L, int NH, float scale, float mask_add,
            const int32_t* cu_seqlens, cudaStream_t st) {
@@ -250,7 +231,7 @@ int ner_bert_attention_tc(const void* qkv_bf16, const int32_t* mask, void* ctx_b
   if ((reinterpret_cast<uintptr_t>(qkv_bf16) & 15) != 0 || (cols * 2) % 16 != 0 ||
       (reinterpret_cast<uintptr_t>(ctx_bf16) & 15) != 0)
     return NER_ERR_UNSUPPORTED;
-  EncodeTiledFn fn = encode_fn();
+  tc::EncodeTiledFn fn = tc::tensor_map_encode_fn();
   if (fn == nullptr) return NER_ERR_UNSUPPORTED;
   CUtensorMap map;
   cuuint64_t dims[2] = {cols, (cuuint64_t)n_rows};

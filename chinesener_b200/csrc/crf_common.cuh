@@ -105,6 +105,61 @@ __device__ __forceinline__ void load_group(float* xs, const float* rowp, int g) 
   }
 }
 
+// Effective length of a row: never past L, and len <= 0 decodes like 1 (tf.contrib.crf quirk).
+__device__ __forceinline__ int clamp_len(const int32_t* __restrict__ seq_len, int row, int L) {
+  return min(max(seq_len[row], 1), L);
+}
+
+// Index of the FIRST maximum of s[0..K) (strict '>': the lowest index wins a tie); its value goes to `best`.
+template <int K, bool UNROLL = Geom<K>::UNROLL>
+__device__ __forceinline__ int argmax_first(const float* s, float& best) {
+  constexpr int UNR = UNROLL ? K : 1;
+  best = s[0];
+  int y = 0;
+#pragma unroll UNR
+  for (int j = 1; j < K; ++j)
+    if (s[j] > best) {
+      best = s[j];
+      y = j;
+    }
+  return y;
+}
+
+// Coalesced [nv, L] int32 store of a CTA's decoded tags, zero beyond each row's length.  reader(r, p) returns the tag
+// of row r at position p; (r, p) of the flat index is kept incrementally: no division.
+template <int NT, typename Reader>
+__device__ __forceinline__ void store_tags_coalesced(int32_t* obase, int nv, int L, const int* s_len, Reader reader) {
+  int r = 0, p = threadIdx.x;
+  while (p >= L) {
+    p -= L;
+    ++r;
+  }
+  const int total = nv * L;
+  for (int idx = threadIdx.x; idx < total; idx += NT) {
+    obase[idx] = (p < s_len[r]) ? reader(r, p) : 0;
+    p += NT;
+    while (p >= L) {
+      p -= L;
+      ++r;
+    }
+  }
+}
+
+// Lane-per-tag kernels (crf_small.cu): a group of GS lanes holds the K-wide state of one sequence.
+template <int K>
+struct Lanes {
+  static constexpr int GS = K <= 8 ? 8 : (K <= 16 ? 16 : 32);
+  static constexpr int SPW = 32 / GS;  // sequences per warp
+};
+
+// Shared memory of the lane-per-tag Viterbi kernel: backpointers [L][32] bytes + decoded tags [SPW][L] ints.
+template <int K>
+constexpr size_t viterbi_lanes_smem_bytes(int L) {
+  return (((size_t)L * 32 + 15) & ~(size_t)15) + (size_t)Lanes<K>::SPW * L * 4;
+}
+
+constexpr size_t kMaxSmem = 227 * 1024;  // dynamic shared memory one CTA can opt in to on sm_90
+
 }  // namespace crf
 
 // Small-batch (lane-per-tag) variants, crf_small.cu.  Chosen by the C-ABI entry points when

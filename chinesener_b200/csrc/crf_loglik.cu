@@ -12,8 +12,6 @@
 // unrolled body; only the first and the ragged last chunk take the checked path.  The exact path (flags bit0, or
 // chosen automatically for wide/inf transition matrices) evaluates every logsumexp with its
 // own max, exactly as the reference's reduce_logsumexp does.
-#include <stdlib.h>
-
 #include "crf_common.cuh"
 
 namespace {
@@ -338,23 +336,13 @@ int launch_fwd_nt(const float* logits, const int32_t* tags, const int32_t* seq_l
   return ner_launch_status();
 }
 
-// NER_CRF_FWD_VARIANT=1 selects the previous configuration (8-step chunks, no register cap: 8 warps/SM)
-// so both can be timed by scripts/bench_kernels.py.
-int fwd_variant() {
-  const char* e = getenv("NER_CRF_FWD_VARIANT");   // tuning / test hook, read per call
-  return e ? atoi(e) : 0;
-}
-
 template <int K>
 int launch_fwd(const float* logits, const int32_t* tags, const int32_t* seq_len, const float* trans,
                float* ll, float* logz, float* alpha_ws, int B, int L, int flags, cudaStream_t st) {
   constexpr bool ER = (K <= 10);
-  if (B > ner_num_sms() * 64 * 2) {
-    if (fwd_variant() == 1)
-      return launch_fwd_nt<K, 64, T_CHUNK, ER>(logits, tags, seq_len, trans, ll, logz, alpha_ws, B, L, flags, st);
-    // 4-step chunks (30 KB smem / CTA) and <= 170 registers: 6 CTAs = 12 warps per SM
+  // big batches: 4-step chunks (30 KB smem / CTA) and <= 170 registers: 6 CTAs = 12 warps per SM
+  if (B > ner_num_sms() * 64 * 2)
     return launch_fwd_nt<K, 64, 4, ER, 6>(logits, tags, seq_len, trans, ll, logz, alpha_ws, B, L, flags, st);
-  }
   return launch_fwd_nt<K, 32, T_CHUNK, ER>(logits, tags, seq_len, trans, ll, logz, alpha_ws, B, L, flags, st);
 }
 

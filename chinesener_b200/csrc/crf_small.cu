@@ -14,12 +14,7 @@
 namespace {
 
 using namespace nerdev;
-
-template <int K>
-struct Lanes {
-  static constexpr int GS = K <= 8 ? 8 : (K <= 16 ? 16 : 32);
-  static constexpr int SPW = 32 / GS;  // sequences per warp
-};
+using crf::Lanes;
 
 constexpr int PF = 4;  // emission prefetch depth (time steps)
 
@@ -324,8 +319,8 @@ template <int K>
 int launch_viterbi_lanes(const float* logits, const int32_t* seq_len, const float* trans, int32_t* tags_out,
                          float* best_score, int B, int L, cudaStream_t st) {
   constexpr int SPW = Lanes<K>::SPW;
-  const size_t smem = (((size_t)L * 32 + 15) & ~(size_t)15) + (size_t)SPW * L * 4;
-  if (smem > 227 * 1024) return NER_ERR_UNSUPPORTED;
+  const size_t smem = crf::viterbi_lanes_smem_bytes<K>(L);
+  if (smem > crf::kMaxSmem) return NER_ERR_UNSUPPORTED;
   auto kern = crf_viterbi_lanes_kernel<K>;
   if (smem > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

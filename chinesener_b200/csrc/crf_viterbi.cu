@@ -1,16 +1,29 @@
 // CRF Viterbi decode for sm_90a — replaces tf.contrib.crf.crf_decode as called at
 // reference tools/layer.py:140-142 (semantics restated in SURVEY.md Appendix A.1).
 //
-// One thread per sequence, K-wide max-plus state in registers, transition matrix in
-// registers (K <= 10) or broadcast smem reads.  Backpointers never leave the SM: they are
-// packed 4 bits (K <= 16) or 8 bits per tag into smem words laid out [t][w][thread], and
-// the decoded tags are written back over word 0 of the same slots during the backtrace, so
-// the final [NT, L] int32 store to HBM is fully coalesced.
+// viterbi_plan() below picks the kernel from (B, L, K, alignment of logits, number of SMs) alone; the first row whose
+// condition holds wins.  big = B > 64 * num_sms; every kernel also needs its shared memory to fit in 227 KB.
+//
+//   plan         kernel                       picked when                       backpointers live in           shared memory per CTA
+//   SMALL        crf_viterbi_lanes_kernel     B <= 4096                         smem, 1 byte per lane          (32 + 4 SPW) L
+//                (crf_small.cu, lane per tag)
+//   TMA          crf_viterbi_tma_kernel       big, K <= 16, L*K % 4 == 0,       smem, 4 bits per tag           (160 + 32 HB) L + 0.3 KB
+//                <K, 32, 2, 2, 8>             logits 16-byte aligned                                           (L <= 1208 at K = 10)
+//   PARKED       crf_viterbi_gs_kernel        big, K <= 16, TMA ruled out       tags 0..7: the CTA's slab of   64 (1 + HB) L + 1 KB
+//                <K, 64, 4, 6>                (L*K % 4, alignment, L)           tags_out; tags 8..15: smem     (L <= 1808 at K = 10)
+//   ONCHIP_128   crf_viterbi_kernel<K, 128>   big (K > 16, or PARKED too long)  smem, 4 or 8 bits per tag      516 W L + ring (4 KB * (2K|1))
+//   ONCHIP_32    crf_viterbi_kernel<K, 32>    any B                             the same                       132 W L + ring / 4
+//   SMALL_ANY_B  crf_viterbi_lanes_kernel     B > 4096, L past all the above    as SMALL                       as SMALL
+//
+// (SPW = Lanes<K>::SPW sequences per warp, HB = BpSplit<K>::HB bytes of high nibbles per step, W = BpPack<K>::W words
+// per step.)  Every kernel but the lane-per-tag one walks one sequence per thread with the K-wide max-plus state in
+// registers.  PARKED exists because the all-on-chip kernel, which would otherwise serve its calls, is slower on them:
+// on an H100 SXM (80 GB HBM3, 700 W limit), ragged lengths, (B, L, K) = (19000, 150, 7): 0.228 ms against 0.158 ms
+// (1.45x); (262144, 127, 10): 2.22 ms against 1.25 ms (1.78x); (9490, 9, 3): 1.17x; only at (9600, 37, 7) is it 4.5 %
+// faster (scripts/bench_crf_dispatch.py).
 //
 // Bit-exactness contract (tests/test_crf_gpu.py): fp32 adds in the reference order
 // (s[i] + trans[i][j], max over i, then + logits[t][j]); ties -> lowest index (strict >).
-#include <stdlib.h>
-
 #include <type_traits>
 
 #include "crf_common.cuh"
@@ -20,8 +33,11 @@ namespace {
 
 using namespace crf;
 
-constexpr size_t kMaxSmem = 227 * 1024;
-
+// ---------------------------------------------------------------------------------------------
+// All-on-chip kernel: transition matrix in registers (K <= 10) or broadcast smem reads.  Backpointers never leave the
+// SM: they are packed 4 bits (K <= 16) or 8 bits per tag into smem words laid out [t][w][thread], and the decoded tags
+// are written back over word 0 of the same slots during the backtrace, so the final [NT, L] int32 store to HBM is fully
+// coalesced.
 template <int K>
 struct BpPack {
   static constexpr int NIB = (K <= 16) ? 4 : 8;
@@ -64,7 +80,7 @@ crf_viterbi_kernel(const float* __restrict__ logits, const int32_t* __restrict__
     s_trT[j * K + i] = trans[e];
   }
   int mylen = 1;
-  if (tid < nv) mylen = min(max(seq_len[row0 + tid], 1), L);  // len<=0 behaves like 1 (TF quirk)
+  if (tid < nv) mylen = clamp_len(seq_len, row0 + tid, L);
   s_len[tid] = mylen;
   const int bmax = block_max_int<NT>(tid < nv ? mylen : 1, reinterpret_cast<int*>(s_bp));
   // (block_max_int ends with __syncthreads: s_len / s_trT are visible)
@@ -151,14 +167,8 @@ crf_viterbi_kernel(const float* __restrict__ logits, const int32_t* __restrict__
   }
 
   if (tid < nv) {
-    float best = s[0];
-    int y = 0;
-#pragma unroll UNR
-    for (int j = 1; j < K; ++j)
-      if (s[j] > best) {
-        best = s[j];
-        y = j;
-      }
+    float best;
+    int y = argmax_first<K>(s, best);
     if (best_score != nullptr) best_score[row0 + tid] = best;
     for (int t = mylen - 1; t >= 1; --t) {
       const uint32_t w = s_bp[(t * W + y / Bp::PER) * NTP + tid];
@@ -170,23 +180,8 @@ crf_viterbi_kernel(const float* __restrict__ logits, const int32_t* __restrict__
   }
   __syncthreads();
 
-  // Coalesced [nv, L] int32 store; zero beyond each row's length.
-  int32_t* obase = tags_out + (size_t)row0 * L;
-  int r = 0, p = tid;
-  while (p >= L) {
-    p -= L;
-    ++r;
-  }
-  const int total = nv * L;
-  for (int idx = tid; idx < total; idx += NT) {
-    const int v = (p < s_len[r]) ? (int)s_bp[(p * W) * NTP + r] : 0;
-    obase[idx] = v;
-    p += NT;
-    while (p >= L) {
-      p -= L;
-      ++r;
-    }
-  }
+  store_tags_coalesced<NT>(tags_out + (size_t)row0 * L, nv, L, s_len,
+                           [&](int r, int p) { return (int)s_bp[(p * W) * NTP + r]; });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -241,7 +236,7 @@ crf_viterbi_gs_kernel(const float* __restrict__ logits, const int32_t* __restric
     s_tr[e] = (j < K) ? trans[i * K + j] : 0.f;
   }
   int mylen = 1;
-  if (tid < nv) mylen = min(max(seq_len[row0 + tid], 1), L);  // len<=0 behaves like 1 (TF quirk)
+  if (tid < nv) mylen = clamp_len(seq_len, row0 + tid, L);
   s_len[tid] = mylen;
   const int bmax = block_max_int<NT>(tid < nv ? mylen : 1, reinterpret_cast<int*>(s_stage));
 
@@ -341,14 +336,8 @@ crf_viterbi_gs_kernel(const float* __restrict__ logits, const int32_t* __restric
   }
 
   if (tid < nv) {
-    float best = s[0];
-    int y = 0;
-#pragma unroll UNR
-    for (int j = 1; j < K; ++j)
-      if (s[j] > best) {
-        best = s[j];
-        y = j;
-      }
+    float best;
+    int y = argmax_first<K>(s, best);
     if (best_score != nullptr) best_score[row0 + tid] = best;
     uint8_t* drow = s_dec + tid * Lp;
     // Backtrace: the parked words are at addresses independent of the path, so fetch 8 steps per
@@ -376,24 +365,8 @@ crf_viterbi_gs_kernel(const float* __restrict__ logits, const int32_t* __restric
   }
   __syncthreads();   // every parked word has been consumed: the slab can now take the decoded tags
 
-  // Coalesced [nv, L] int32 store; zero beyond each row's length.
-  int32_t* obase = tags_out + (size_t)row0 * L;
-  int r = 0, p = tid;
-  while (p >= L) {
-    p -= L;
-    ++r;
-  }
-  const int total = nv * L;
-  for (int idx = tid; idx < total; idx += NT) {
-    obase[idx] = (p < s_len[r]) ? (int)s_dec[r * Lp + p] : 0;
-    p += NT;
-    while (p >= L) {
-      p -= L;
-      ++r;
-    }
-  }
+  store_tags_coalesced<NT>(tags_out + (size_t)row0 * L, nv, L, s_len, [&](int r, int p) { return (int)s_dec[r * Lp + p]; });
 }
-
 
 template <int K, int J = 0, typename F>
 __device__ __forceinline__ void sel_all(F& f) {
@@ -424,8 +397,8 @@ __device__ __forceinline__ void sel_all(F& f) {
 //      without per-row length checks; chunk 0 (t = 0 has no predecessor) is peeled.  The backtrace prefetches the words
 //      of 8 steps (their addresses do not depend on the path) and resolves the chain in registers.  The transition
 //      matrix goes from global memory straight into registers (every thread reads the same K*K words).
-// NER_CRF_VIT_VARIANT=2 selects the parked-nibble kernel above instead (it is also the fallback when L*K % 4 != 0 or the
-// backpointers of L steps do not fit in shared memory).
+// The parked-nibble kernel above serves the calls this one cannot: L*K % 4 != 0, logits not 16-byte aligned, or the
+// backpointers of L steps do not fit in shared memory.
 template <int K, int TT>
 struct TmaGeom {
   static constexpr int T = (K % 2) ? 4 : TT;                // steps per chunk: T*K % 4 == 0
@@ -527,13 +500,13 @@ crf_viterbi_tma_kernel(const __grid_constant__ CUtensorMap tm_logits, const int3
     tc::fence_barrier_init();
   }
   int mylen = 1;
-  if (live) mylen = min(max(seq_len[row0 + tid], 1), L);  // len<=0 behaves like 1 (TF quirk)
+  if (live) mylen = clamp_len(seq_len, row0 + tid, L);
   s_len[tid] = mylen;
   int wmax = live ? mylen : 0;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
   const int nchunk = (wmax + T - 1) / T;                // 0 for a warp past the end of the batch
-  __syncthreads();                                      // s_tr, s_len and the barrier inits are visible
+  __syncthreads();                                      // s_len and every warp's barrier inits are visible
 
   if (tc::elect_one()) {
 #pragma unroll
@@ -650,14 +623,8 @@ crf_viterbi_tma_kernel(const __grid_constant__ CUtensorMap tm_logits, const int3
     float sv[2 * KP];
 #pragma unroll
     for (int p = 0; p < KP; ++p) upk2(s2[p], sv[2 * p], sv[2 * p + 1]);
-    float best = sv[0];
-    int y = 0;
-#pragma unroll
-    for (int j = 1; j < K; ++j)
-      if (sv[j] > best) {
-        best = sv[j];
-        y = j;
-      }
+    float best;
+    int y = argmax_first<K, true>(sv, best);
     if (best_score != nullptr) best_score[row0 + tid] = best;
     uint8_t* drow = w_dec + lane * Lp;
     // Backtrace: the words are at addresses independent of the path, so fetch 8 steps per round trip and resolve the
@@ -673,7 +640,6 @@ crf_viterbi_tma_kernel(const __grid_constant__ CUtensorMap tm_logits, const int3
         if (HB == 2) wb[u] = in ? reinterpret_cast<const uint16_t*>(hi_p)[(size_t)(t - u) * NT] : 0u;
         if (HB == 4) wb[u] = in ? reinterpret_cast<const uint32_t*>(hi_p)[(size_t)(t - u) * NT] : 0u;
       }
-      uint32_t d8[2] = {0u, 0u};             // the 8 decoded tags of this batch, one byte each (tt = t-u -> byte 7-u... stored below)
 #pragma unroll
       for (int u = 0; u < 8; ++u) {
         const int tt = t - u;
@@ -683,7 +649,6 @@ crf_viterbi_tma_kernel(const __grid_constant__ CUtensorMap tm_logits, const int3
           y = (int)((w >> (4 * (y & 7))) & 15u);
         }
       }
-      (void)d8;
     }
     drow[0] = (uint8_t)y;
   }
@@ -719,68 +684,57 @@ crf_viterbi_tma_kernel(const __grid_constant__ CUtensorMap tm_logits, const int3
   }
 }
 
-template <int K, int NT, int TT, int MINB>
-int launch_viterbi_gs(const float* logits, const int32_t* seq_len, const float* trans,
-                      int32_t* tags_out, float* best_score, int B, int L, cudaStream_t st) {
-  const size_t smem = viterbi_gs_smem_bytes<K, NT, TT>(L);
-  if (smem > 227 * 1024) return NER_ERR_UNSUPPORTED;
-  auto kern = crf_viterbi_gs_kernel<K, NT, TT, MINB>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
-  const int vec16 = ((L * K) % 4 == 0) && ((reinterpret_cast<uintptr_t>(logits) & 15) == 0);
-  const int grid = (B + NT - 1) / NT;
-  kern<<<grid, NT, smem, st>>>(logits, seq_len, trans, tags_out, best_score, B, L, vec16);
-  return ner_launch_status();
-}
-
-int vit_variant() {
-  const char* e = getenv("NER_CRF_VIT_VARIANT");   // tuning / test hook, read per call
-  return e ? atoi(e) : 0;
-}
-
-template <int K, int NT>
-int launch_viterbi_nt(const float* logits, const int32_t* seq_len, const float* trans,
-                      int32_t* tags_out, float* best_score, int B, int L, cudaStream_t st) {
-  const size_t smem = viterbi_smem_bytes<K, NT>(L);
-  auto kern = crf_viterbi_kernel<K, NT>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
-  const int vec16 = ((L * K) % 4 == 0) && ((reinterpret_cast<uintptr_t>(logits) & 15) == 0);
-  const int grid = (B + NT - 1) / NT;
-  kern<<<grid, NT, smem, st>>>(logits, seq_len, trans, tags_out, best_score, B, L, vec16);
-  return ner_launch_status();
-}
-
-
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-    (void)cudaGetLastError();
+// Which kernel serves a call: exactly the conditions of the table at the top of this file, in its order.  Pure host
+// arithmetic.  `tma_ok` = the logits pointer is 16-byte aligned (and, on the retry in ner_crf_viterbi, the driver
+// produced a tensor map).
+template <int K>
+int viterbi_plan_k(int B, int L, bool tma_ok, int num_sms) {
+  const bool lanes_fit = viterbi_lanes_smem_bytes<K>(L) <= kMaxSmem;
+  if (B <= NER_CRF_SMALL_B && lanes_fit) return NER_VIT_SMALL;
+  // Large batches: 128 sequences per CTA when the backpointer slab fits; small batches
+  // spread over more SMs with 32-sequence CTAs.
+  const bool big = B > num_sms * 32 * 2;
+  if constexpr (K <= 16) {
+    if (big && tma_ok && ((size_t)L * K) % 4 == 0 && viterbi_tma_smem_bytes<K, 32, 2, 2>(L) <= kMaxSmem) return NER_VIT_TMA;
+    if (big && viterbi_gs_smem_bytes<K, 64, 4>(L) <= kMaxSmem) return NER_VIT_PARKED;
   }
-  return fn;
+  if (big && viterbi_smem_bytes<K, 128>(L) <= kMaxSmem) return NER_VIT_ONCHIP_128;
+  if (viterbi_smem_bytes<K, 32>(L) <= kMaxSmem) return NER_VIT_ONCHIP_32;
+  // L past the throughput kernels' on-chip backpointers (document-length batches stacked past NER_CRF_SMALL_B rows): the
+  // lane-per-tag kernel keeps 32 + 4*SPW bytes per step on chip and serves any B
+  if (B > NER_CRF_SMALL_B && lanes_fit) return NER_VIT_SMALL_ANY_B;
+  return NER_VIT_NONE;
 }
 
+int viterbi_plan(int B, int L, int K, bool tma_ok, int num_sms) {
+#define CALL(KK) return viterbi_plan_k<KK>(B, L, tma_ok, num_sms)
+  NER_CRF_DISPATCH_K(K, CALL)
+#undef CALL
+  return NER_VIT_NONE;
+}
+
+// The all-on-chip and parked-nibble kernels take the same arguments and differ in CTA size and shared memory only.
+using ThreadPerSeqKernel = void (*)(const float*, const int32_t*, const float*, int32_t*, float*, int, int, int);
+
+int launch_thread_per_seq(ThreadPerSeqKernel kern, int nt, size_t smem, const float* logits, const int32_t* seq_len,
+                          const float* trans, int32_t* tags_out, float* best_score, int B, int L, int K, cudaStream_t st) {
+  if (smem > kMaxSmem) return NER_ERR_UNSUPPORTED;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
+  const int vec16 = ((L * K) % 4 == 0) && ((reinterpret_cast<uintptr_t>(logits) & 15) == 0);
+  const int grid = (B + nt - 1) / nt;
+  kern<<<grid, nt, smem, st>>>(logits, seq_len, trans, tags_out, best_score, B, L, vec16);
+  return ner_launch_status();
+}
+
+// NER_ERR_UNSUPPORTED = the driver has no cuTensorMapEncodeTiled or refused this map: the caller plans again without TMA.
 template <int K, int NT, int S, int TT, int MINB>
 int launch_viterbi_tma(const float* logits, const int32_t* seq_len, const float* trans, int32_t* tags_out,
                        float* best_score, int B, int L, cudaStream_t st) {
   using Gm = TmaGeom<K, TT>;
   const size_t LK = (size_t)L * K;
-  if ((LK & 3) != 0 || (reinterpret_cast<uintptr_t>(logits) & 15) != 0) return NER_ERR_UNSUPPORTED;
   const size_t smem = viterbi_tma_smem_bytes<K, NT, S, TT>(L);
-  if (smem > kMaxSmem) return NER_ERR_UNSUPPORTED;
-  EncodeTiledFn fn = encode_fn();
+  tc::EncodeTiledFn fn = tc::tensor_map_encode_fn();
   if (fn == nullptr) return NER_ERR_UNSUPPORTED;
   CUtensorMap map;
   cuuint64_t dims[2] = {(cuuint64_t)LK, (cuuint64_t)B};
@@ -800,30 +754,42 @@ int launch_viterbi_tma(const float* logits, const int32_t* seq_len, const float*
   return ner_launch_status();
 }
 
+// Launch the thread-per-sequence kernel `plan` names (template parameters as in viterbi_plan_k).
 template <int K>
-int launch_viterbi(const float* logits, const int32_t* seq_len, const float* trans,
-                   int32_t* tags_out, float* best_score, int B, int L, cudaStream_t st) {
-  // Large batches: 128 sequences per CTA when the backpointer slab fits; small batches
-  // spread over more SMs with 32-sequence CTAs.
-  const bool big = B > ner_num_sms() * 32 * 2;
+int launch_planned(int plan, const float* logits, const int32_t* seq_len, const float* trans, int32_t* tags_out,
+                   float* best_score, int B, int L, cudaStream_t st) {
   if constexpr (K <= 16) {
-    if (big && vit_variant() == 0) {   // default: the pipe-balanced TMA kernel (falls through when L*K % 4 != 0 or L is too long)
-      const int rc = launch_viterbi_tma<K, 32, 2, 2, 8>(logits, seq_len, trans, tags_out, best_score, B, L, st);
-      if (rc != NER_ERR_UNSUPPORTED) return rc;
-    }
-    if (big && vit_variant() != 1) {   // NER_CRF_VIT_VARIANT=2: the parked-nibble kernel; =1: the all-on-chip kernel
-      const int rc = launch_viterbi_gs<K, 64, 4, 6>(logits, seq_len, trans, tags_out, best_score, B, L, st);
-      if (rc != NER_ERR_UNSUPPORTED) return rc;
-    }
+    if (plan == NER_VIT_TMA)
+      return launch_viterbi_tma<K, 32, 2, 2, 8>(logits, seq_len, trans, tags_out, best_score, B, L, st);
+    if (plan == NER_VIT_PARKED)
+      return launch_thread_per_seq(crf_viterbi_gs_kernel<K, 64, 4, 6>, 64, viterbi_gs_smem_bytes<K, 64, 4>(L), logits, seq_len,
+                                   trans, tags_out, best_score, B, L, K, st);
   }
-  if (big && viterbi_smem_bytes<K, 128>(L) <= kMaxSmem)
-    return launch_viterbi_nt<K, 128>(logits, seq_len, trans, tags_out, best_score, B, L, st);
-  if (viterbi_smem_bytes<K, 32>(L) <= kMaxSmem)
-    return launch_viterbi_nt<K, 32>(logits, seq_len, trans, tags_out, best_score, B, L, st);
-  return NER_ERR_UNSUPPORTED;  // L too long for on-chip backpointers
+  if (plan == NER_VIT_ONCHIP_128)
+    return launch_thread_per_seq(crf_viterbi_kernel<K, 128>, 128, viterbi_smem_bytes<K, 128>(L), logits, seq_len, trans,
+                                 tags_out, best_score, B, L, K, st);
+  if (plan == NER_VIT_ONCHIP_32)
+    return launch_thread_per_seq(crf_viterbi_kernel<K, 32>, 32, viterbi_smem_bytes<K, 32>(L), logits, seq_len, trans,
+                                 tags_out, best_score, B, L, K, st);
+  return NER_ERR_UNSUPPORTED;
+}
+
+int run_plan(int plan, const float* logits, const int32_t* seq_len, const float* trans, int32_t* tags_out,
+             float* best_score, int B, int L, int K, cudaStream_t st) {
+  if (plan == NER_VIT_SMALL || plan == NER_VIT_SMALL_ANY_B)
+    return ner_crf_viterbi_small(logits, seq_len, trans, tags_out, best_score, B, L, K, st);
+#define CALL(KK) return launch_planned<KK>(plan, logits, seq_len, trans, tags_out, best_score, B, L, st)
+  NER_CRF_DISPATCH_K(K, CALL)
+#undef CALL
+  return NER_ERR_UNSUPPORTED;
 }
 
 }  // namespace
+
+extern "C" int ner_crf_viterbi_plan(int B, int L, int K, int logits_aligned, int num_sms) {
+  if (B < 1 || L < 1 || K < 1 || K > NER_MAX_TAGS) return NER_VIT_NONE;
+  return viterbi_plan(B, L, K, logits_aligned != 0, num_sms);
+}
 
 extern "C" int ner_crf_viterbi(const float* logits, const int32_t* seq_len, const float* trans,
                                int32_t* tags_out, float* best_score, int B, int L, int K,
@@ -833,17 +799,11 @@ extern "C" int ner_crf_viterbi(const float* logits, const int32_t* seq_len, cons
   if (!logits || !seq_len || !trans || !tags_out) return NER_ERR_INVALID_ARG;
   if (K > NER_MAX_TAGS) return NER_ERR_UNSUPPORTED;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (B <= NER_CRF_SMALL_B) {
-    const int rc = ner_crf_viterbi_small(logits, seq_len, trans, tags_out, best_score, B, L, K, st);
-    if (rc != NER_ERR_UNSUPPORTED) return rc;
-  }
-  int rc = NER_ERR_UNSUPPORTED;
-#define CALL(KK) rc = launch_viterbi<KK>(logits, seq_len, trans, tags_out, best_score, B, L, st)
-  NER_CRF_DISPATCH_K(K, CALL)
-#undef CALL
-  // L past the throughput kernels' on-chip backpointers (document-length batches stacked past NER_CRF_SMALL_B rows): the
-  // lane-per-tag kernel keeps 32 + 4*SPW bytes per step on chip and serves any B
-  if (rc == NER_ERR_UNSUPPORTED && B > NER_CRF_SMALL_B)
-    rc = ner_crf_viterbi_small(logits, seq_len, trans, tags_out, best_score, B, L, K, st);
+  const int plan = viterbi_plan(B, L, K, (reinterpret_cast<uintptr_t>(logits) & 15) == 0, ner_num_sms());
+  int rc = run_plan(plan, logits, seq_len, trans, tags_out, best_score, B, L, K, st);
+  // Everything the plan depends on is known before launch, except whether the driver hands out a tensor map: that is
+  // the one demotion left at launch time, to the plan computed with TMA excluded.
+  if (plan == NER_VIT_TMA && rc == NER_ERR_UNSUPPORTED)
+    rc = run_plan(viterbi_plan(B, L, K, false, ner_num_sms()), logits, seq_len, trans, tags_out, best_score, B, L, K, st);
   return rc;
 }

@@ -761,28 +761,9 @@ gemm_e4m3_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_cons
 }
 
 // ---------------------------------------------------------------- host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-    (void)cudaGetLastError();
-  }
-  return fn;
-}
-
 // Row-major [rows, cols] of bf16 (f32 = false) or fp32 with a {box_cols, box_rows} box of 128-B rows, 128-byte swizzle.
 int make_map_2d(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows, bool f32 = false) {
-  EncodeTiledFn fn = get_encode_fn();
+  EncodeTiledFn fn = tensor_map_encode_fn();
   if (fn == nullptr) return NER_ERR_NO_DRIVER;
   const uint32_t esz = f32 ? 4 : 2;
   cuuint64_t dims[2] = {cols, rows};
@@ -1045,7 +1026,7 @@ extern "C" int ner_gemm_bf16(const void* A, const void* Wt, const float* bias, c
 namespace {
 // e4m3 row-major [rows, cols] (one byte per element) with a {128 columns, box_rows} box, 128-byte swizzle.
 int make_map_e4m3(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows) {
-  EncodeTiledFn fn = get_encode_fn();
+  EncodeTiledFn fn = tensor_map_encode_fn();
   if (fn == nullptr) return NER_ERR_NO_DRIVER;
   cuuint64_t dims[2] = {cols, rows};
   cuuint64_t strides[1] = {cols};

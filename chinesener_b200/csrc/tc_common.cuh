@@ -304,4 +304,23 @@ __device__ __forceinline__ float tanh_approx(float x) {
   return y;
 }
 
+// ---------------------------------------------------------------- host side
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+// cuTensorMapEncodeTiled, resolved through the runtime (the library does not link libcuda); nullptr when the driver
+// does not provide it.
+inline EncodeTiledFn tensor_map_encode_fn() {
+  static const EncodeTiledFn fn = [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    const bool ok = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
+                    qres == cudaDriverEntryPointSuccess;
+    (void)cudaGetLastError();
+    return ok ? reinterpret_cast<EncodeTiledFn>(p) : nullptr;
+  }();
+  return fn;
+}
+
 }  // namespace tc

@@ -53,6 +53,22 @@ int ner_crf_viterbi(const float* logits, const int32_t* seq_len, const float* tr
                     int32_t* tags_out, float* best_score, int B, int L, int K,
                     ner_stream_t stream);
 
+/* Which kernel ner_crf_viterbi runs for a call of this shape.  The choice is a pure function of the arguments below
+ * (csrc/crf_viterbi.cu lists the kernels and their limits); nothing else, in particular no environment variable,
+ * changes it.  logits_aligned = the logits pointer is 16-byte aligned; num_sms = multiprocessors of the device.  No
+ * CUDA call is made, so it can be asked on a machine without a GPU.  NER_VIT_NONE: ner_crf_viterbi returns
+ * NER_ERR_UNSUPPORTED (L too long for every kernel, or K outside 1..32). */
+enum {
+  NER_VIT_SMALL = 0,       /* lane-per-tag kernel, B <= 4096 */
+  NER_VIT_TMA = 1,         /* thread-per-sequence, logits by TMA, backpointers in shared memory */
+  NER_VIT_PARKED = 2,      /* thread-per-sequence, low backpointer nibbles parked in tags_out */
+  NER_VIT_ONCHIP_128 = 3,  /* thread-per-sequence, backpointers in shared memory, 128 sequences per CTA */
+  NER_VIT_ONCHIP_32 = 4,   /* the same kernel with 32 sequences per CTA */
+  NER_VIT_SMALL_ANY_B = 5, /* lane-per-tag kernel for an L no thread-per-sequence kernel holds, B > 4096 */
+  NER_VIT_NONE = 6
+};
+int ner_crf_viterbi_plan(int B, int L, int K, int logits_aligned, int num_sms);
+
 /* tools/layer.py:122-127  crf_layer -> tf.contrib.crf.crf_log_likelihood
  * ll[b] = gold-path score - log-partition (forward-alpha recursion).
  * tags [B,L] i32.  alpha_ws: NULL, or [B,L,K] f32 that receives alpha_t for

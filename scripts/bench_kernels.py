@@ -39,9 +39,9 @@ def bench_crf(B=262144, L=128, K=10):
     med, best = timeit(lambda: ops.crf_viterbi(x, lens, tr))
     byts = B * L * (4 * K) + 4 * B + 4 * K * K + B * L * 4 + 4 * B
     out["viterbi"] = dict(ms=med, best_ms=best, GBps=byts / med / 1e6, bytes=byts)
-    import os
-    out["fwd_variant"] = os.environ.get("NER_CRF_FWD_VARIANT", "0")
-    out["vit_variant"] = os.environ.get("NER_CRF_VIT_VARIANT", "0")
+    from chinesener_b200 import _lib
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    out["viterbi_plan"] = _lib.VIT_PLANS[_lib.lib().ner_crf_viterbi_plan(B, L, K, x.data_ptr() % 16 == 0, sms)]
     for exact in (False, True):
         med, best = timeit(lambda: ops.crf_loglik_fwd(x, tags, lens, tr, exact=exact))
         byts = B * L * (4 * K + 4) + 8 * B + 4 * K * K

@@ -1,6 +1,6 @@
 // Stand-alone timing harness for ner_crf_viterbi at the roofline shape (no Python start-up: the whole run is seconds).
 //   nvcc -O3 -o vit_harness vit_harness.cu -I../../include -L../../chinesener_b200 -lner_b200 -Xlinker -rpath -Xlinker '$ORIGIN/../../chinesener_b200'
-// Prints ms, algorithmic GB/s and a checksum of the tags (equal across NER_CRF_VIT_VARIANT / tuning variants).
+// Prints the kernel plan (NER_VIT_* of ner_b200.h), ms, algorithmic GB/s and a checksum of the tags (equal across builds).
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>
@@ -55,8 +55,10 @@ int main(int argc, char** argv) {
   checksum<<<1184, 256>>>(tags, (size_t)B * L, cs);
   unsigned long long h; cudaMemcpy(&h, cs, 8, cudaMemcpyDeviceToHost);
   const double bytes = (double)B * L * 4 * K + 4.0 * B + 4.0 * K * K + (double)B * L * 4 + 4.0 * B;
-  printf("variant=%s tune=%s B=%d L=%d K=%d ragged=%d  mean %.4f ms  best %.4f ms  %.0f GB/s  checksum %llu  %s\n",
-         getenv("NER_CRF_VIT_VARIANT") ? getenv("NER_CRF_VIT_VARIANT") : "0", getenv("NER_CRF_VIT_TUNE") ? getenv("NER_CRF_VIT_TUNE") : "-",
+  cudaDeviceProp prop;
+  cudaGetDeviceProperties(&prop, 0);
+  printf("plan=%d B=%d L=%d K=%d ragged=%d  mean %.4f ms  best %.4f ms  %.0f GB/s  checksum %llu  %s\n",
+         ner_crf_viterbi_plan(B, L, K, ((uintptr_t)x & 15) == 0, prop.multiProcessorCount),
          B, L, K, ragged, sum / R, best_ms, bytes / (sum / R) / 1e6, h, cudaGetErrorString(cudaGetLastError()));
   return 0;
 }

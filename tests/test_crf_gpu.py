@@ -8,6 +8,7 @@ import pytest
 import torch
 
 from chinesener_b200 import ops
+from chinesener_b200._lib import VIT_PLANS, lib
 from oracle import crf
 
 pytestmark = pytest.mark.gpu
@@ -20,6 +21,12 @@ def _case(B, L, K, seed, ragged=True, scale=2.0):
     lens = rng.integers(1, L + 1, size=B).astype(np.int32) if ragged else np.full(B, L, np.int32)
     tags = rng.integers(0, K, size=(B, L)).astype(np.int32)
     return x, tr, lens, tags
+
+
+def _plan(B, L, K, aligned=True):
+    """Name of the kernel ner_crf_viterbi runs for this shape on this device."""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    return VIT_PLANS[lib().ner_crf_viterbi_plan(B, L, K, int(aligned), sms)]
 
 
 @pytest.mark.parametrize("B,L,K", [(64, 128, 10), (8, 64, 10), (37, 150, 7), (5, 1, 4), (3, 17, 1), (130, 33, 13),
@@ -49,16 +56,18 @@ def test_viterbi_ties_resolve_to_lowest_index():
     np.testing.assert_array_equal(tags.cpu().numpy(), ref_tags)
 
 
-def test_viterbi_mid_batch_uses_thread_per_sequence_kernel():
-    B, L, K = 5000, 40, 10                              # above the lane-per-tag threshold, NT=32 CTAs
+def test_viterbi_mid_batch_uses_all_on_chip_kernel_with_32_thread_ctas():
+    B, L, K = 5000, 40, 10                              # above the lane-per-tag threshold, below the big-batch one
+    assert _plan(B, L, K) == "onchip_32"
     x, tr, lens, _ = _case(B, L, K, seed=17)
     ref_tags, _ = crf.crf_decode(x, tr, lens, dtype=np.float32)
     tags = ops.crf_viterbi(torch.from_numpy(x).cuda(), torch.from_numpy(lens).cuda(), torch.from_numpy(tr).cuda())
     np.testing.assert_array_equal(tags.cpu().numpy(), ref_tags)
 
 
-def test_viterbi_large_batch_uses_128_thread_ctas():
+def test_viterbi_large_batch_uses_tma_kernel():
     B, L, K = 148 * 64 + 77, 128, 10                    # > big-batch threshold, ragged tail CTA
+    assert _plan(B, L, K) == "tma"
     x, tr, lens, _ = _case(B, L, K, seed=11)
     ref_tags, _ = crf.crf_decode(x, tr, lens, dtype=np.float32)
     tags = ops.crf_viterbi(torch.from_numpy(x).cuda(), torch.from_numpy(lens).cuda(), torch.from_numpy(tr).cuda())
@@ -105,31 +114,56 @@ def test_loglik_alpha_workspace():
         np.testing.assert_allclose(a[b, :n], alphas[b, :n], rtol=1e-4, atol=1e-4)
 
 
-@pytest.mark.parametrize("variant", [0, 1, 2])
-@pytest.mark.parametrize("B,L,K", [(148 * 64 + 77, 128, 10), (9600, 37, 7), (9500, 50, 16), (9601, 21, 12), (9490, 9, 3),
-                                   (9500, 12, 5), (9533, 16, 9), (9480, 20, 8), (9479, 8, 11), (9600, 256, 10), (9500, 6, 2)])
-def test_viterbi_large_batch_kernels_bit_exact(monkeypatch, variant, B, L, K):
-    """variant 0 = the pipe-balanced TMA kernel (max tree + first-equal index, all backpointers in shared memory; taken
-    when L*K % 4 == 0, otherwise the call falls through to variant 2), variant 2 = the occupancy-first kernel (low
-    backpointer nibbles parked in the tags_out slab), variant 1 = the all-on-chip kernel (the fallback for K > 16): all
-    must reproduce the oracle's tags and scores, ragged lengths and a partial tail CTA included."""
-    monkeypatch.setenv("NER_CRF_VIT_VARIANT", str(variant))
-    x, tr, lens, _ = _case(B, L, K, seed=variant * 100 + K)
+# (B, L, K, logits 16-byte aligned, kernel the plan must name).  A big batch has more than 64 sequences per SM: 8448 on
+# the 132 SMs of an H100 SXM.
+_PLANNED = [
+    # logits by TMA: K <= 16, L*K % 4 == 0, aligned
+    (148 * 64 + 77, 128, 10, True, "tma"), (9500, 50, 16, True, "tma"), (9601, 21, 12, True, "tma"),
+    (9500, 12, 5, True, "tma"), (9533, 16, 9, True, "tma"), (9480, 20, 8, True, "tma"), (9479, 8, 11, True, "tma"),
+    (9600, 256, 10, True, "tma"), (9500, 6, 2, True, "tma"), (9490, 1200, 10, True, "tma"),
+    # parked nibbles: L*K % 4 != 0, logits off a 16-byte boundary, or L past the TMA kernel's shared memory
+    (9600, 37, 7, True, "parked"), (9490, 9, 3, True, "parked"), (19000, 150, 7, True, "parked"),
+    (9500, 127, 10, True, "parked"), (9500, 33, 13, True, "parked"), (9511, 21, 15, True, "parked"),
+    (148 * 64 + 77, 128, 10, False, "parked"), (9500, 50, 16, False, "parked"), (9480, 20, 8, False, "parked"),
+    (9601, 21, 12, False, "parked"), (9479, 8, 11, False, "parked"), (9490, 1500, 10, True, "parked"),
+    # all on chip, 128-thread CTAs: big batches of more than 16 tags
+    (9500, 20, 20, True, "onchip_128"), (9600, 30, 17, True, "onchip_128"), (9490, 24, 18, True, "onchip_128"),
+    (9479, 8, 24, True, "onchip_128"), (9500, 20, 20, False, "onchip_128"),
+    # all on chip, 32-thread CTAs: mid batches, and big ones past the 128-thread slab (every L at K >= 28)
+    (9490, 24, 32, True, "onchip_32"),
+    (5000, 40, 10, True, "onchip_32"), (6000, 33, 13, True, "onchip_32"), (4500, 30, 20, True, "onchip_32"),
+    (7000, 37, 7, False, "onchip_32"), (9500, 120, 20, True, "onchip_32"), (9490, 100, 32, True, "onchip_32"),
+    # lane per tag: up to 4096 sequences, and any B when L is past every thread-per-sequence limit
+    (4096, 16, 10, True, "small"), (4200, 1500, 20, True, "small_any_b"), (4200, 800, 10, True, "small_any_b"),
+]
+
+
+@pytest.mark.parametrize("B,L,K,aligned,plan", _PLANNED)
+def test_viterbi_large_batch_kernels_bit_exact(B, L, K, aligned, plan):
+    """Every kernel the plan can name must reproduce the oracle's tags and scores, ragged lengths and a partial tail CTA
+    included, on shapes that reach it by themselves."""
+    assert _plan(B, L, K, aligned) == plan
+    x, tr, lens, _ = _case(B, L, K, seed=100 * len(plan) + K)
     lens[0], lens[1], lens[2] = L, 1, 0
     x[5] = np.round(x[5])                                # a row with many exact ties
     ref_tags, ref_best = crf.crf_decode(x, tr, lens, dtype=np.float32)
-    tags, best = ops.crf_viterbi(torch.from_numpy(x).cuda(), torch.from_numpy(lens).cuda(),
-                                 torch.from_numpy(tr).cuda(), return_score=True)
+    if aligned:
+        xd = torch.from_numpy(x).cuda()
+    else:                                                # the same logits 4 bytes past a 16-byte boundary
+        flat = torch.empty(x.size + 1, dtype=torch.float32, device="cuda")
+        xd = flat[1:].view(B, L, K)
+        xd.copy_(torch.from_numpy(x))
+    assert (xd.data_ptr() % 16 == 0) == aligned
+    tags, best = ops.crf_viterbi(xd, torch.from_numpy(lens).cuda(), torch.from_numpy(tr).cuda(), return_score=True)
     np.testing.assert_array_equal(tags.cpu().numpy(), ref_tags)
     np.testing.assert_array_equal(best.cpu().numpy(), ref_best.astype(np.float32))
 
 
-@pytest.mark.parametrize("variant", [0, 1])
+@pytest.mark.parametrize("B", [19000, 5000])             # 64-thread CTAs with 4-step chunks / 32-thread CTAs
 @pytest.mark.parametrize("K", [10, 7, 13])
-def test_loglik_large_batch_configurations(monkeypatch, variant, K):
-    monkeypatch.setenv("NER_CRF_FWD_VARIANT", str(variant))
-    B, L = 19000, 40
-    x, tr, lens, tags = _case(B, L, K, seed=variant + K)
+def test_loglik_large_batch_configurations(B, K):
+    L = 40
+    x, tr, lens, tags = _case(B, L, K, seed=B % 7 + K)
     ref = crf.crf_log_likelihood(x, tags, lens, tr, dtype=np.float64)
     ll, _, _ = ops.crf_loglik_fwd(torch.from_numpy(x).cuda(), torch.from_numpy(tags).cuda(),
                                   torch.from_numpy(lens).cuda(), torch.from_numpy(tr).cuda())
