@@ -65,6 +65,14 @@ SIGNATURES = {
                                + [_c.c_size_t, _vp]),
     "ner_mrc_span_decode_workspace_bytes": (_c.c_size_t, [_i, _i]),
     "ner_mrc_span_decode": (_i, [_vp] * 3 + [_i] + [_vp] * 5 + [_i] * 8 + [_vp] * 5 + [_c.c_size_t, _vp]),
+    "ner_gp_targets": (_i, [_vp] * 3 + [_i] * 3 + [_vp, _vp]),
+    "ner_gp_rope": (_i, [_vp, _i, _vp] + [_i] * 3 + [_vp] * 3),
+    "ner_gp_rope_bwd": (_i, [_vp, _vp] + [_i] * 3 + [_vp, _i, _vp]),
+    "ner_gp_loss_workspace_bytes": (_c.c_size_t, [_i] * 3),
+    "ner_gp_loss_fwd": (_i, [_vp] * 5 + [_i] * 3 + [_vp] * 3 + [_c.c_size_t, _vp]),
+    "ner_gp_loss_bwd": (_i, [_vp] * 5 + [_i] * 3 + [_c.c_float, _vp, _vp]),
+    "ner_gp_decode_workspace_bytes": (_c.c_size_t, [_i] * 3),
+    "ner_gp_decode": (_i, [_vp] * 5 + [_i] * 7 + [_vp] * 5 + [_c.c_size_t, _vp]),
     "ner_window_plan": (_i, [_vp] * 3 + [_i] * 5 + [_vp] * 6),
     "ner_layernorm_bwd": (_i, [_vp, _i] + [_vp] * 7 + [_i, _i, _c.c_float, _vp]),
     "ner_layernorm_dropout_bwd": (_i, [_vp, _i] + [_vp] * 7 + [_i, _i, _c.c_float, _c.c_float, _c.c_uint64, _vp]),

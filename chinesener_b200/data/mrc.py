@@ -63,19 +63,34 @@ def query_token_ids(params, names):
     return ids, tokenizer.vocab['[SEP]'] if tokenizer is not None else SEP_TOKEN_ID
 
 
-class MrcTable:
-    """Everything the bert_mrc graph needs about its queries: host sizes and the device tables of ner_mrc_pairs /
-    ner_mrc_merge."""
+class TypeTable:
+    """The entity types of params['idx2tag'] (entity_types) and the tag ids a per-type decode writes: names, T, type_tag
+    [T, 2] (B-X, I-X ids) on `device`, o_tag, and cls_tag / sep_tag (o_tag when idx2tag has no [CLS] / [SEP])."""
 
     def __init__(self, params, device='cuda'):
         idx2tag = params['idx2tag']
         types = entity_types(idx2tag)
         self.names = [n for n, _, _ in types]
-        ids, self.sep_id = query_token_ids(params, self.names)
         self.T = len(types)
+        self.L = int(params['max_seq_len'])
+        self.type_tag = torch.tensor([[b, i] for _, b, i in types], dtype=torch.int32).to(device)
+        tag2idx = {tag: i for i, tag in idx2tag.items()}
+        if 'O' not in tag2idx:
+            raise ValueError("idx2tag has no 'O' tag: the per-type decode writes it outside the entities")
+        self.o_tag = tag2idx['O']
+        self.cls_tag = tag2idx.get('[CLS]', self.o_tag)
+        self.sep_tag = tag2idx.get('[SEP]', self.o_tag)
+
+
+class MrcTable(TypeTable):
+    """Everything the bert_mrc graph needs about its queries: host sizes and the device tables of ner_mrc_pairs /
+    ner_mrc_merge, on top of the TypeTable."""
+
+    def __init__(self, params, device='cuda'):
+        super().__init__(params, device)
+        ids, self.sep_id = query_token_ids(params, self.names)
         self.query_lens = [len(q) for q in ids]
         self.qmax = max(self.query_lens)
-        self.L = int(params['max_seq_len'])
         self.L2 = self.qmax + 1 + self.L
         max_pos = bert.load_bert_config(params['pretrain_dir'])['max_position_embeddings']
         if self.L2 > max_pos:
@@ -87,13 +102,6 @@ class MrcTable:
             table[t, :len(q)] = torch.tensor(q, dtype=torch.int32)
         self.query_ids = table.to(device)
         self.query_len = torch.tensor(self.query_lens, dtype=torch.int32).to(device)
-        self.type_tag = torch.tensor([[b, i] for _, b, i in types], dtype=torch.int32).to(device)
-        tag2idx = {tag: i for i, tag in idx2tag.items()}
-        if 'O' not in tag2idx:
-            raise ValueError("bert_mrc: idx2tag has no 'O' tag")
-        self.o_tag = tag2idx['O']
-        self.cls_tag = tag2idx.get('[CLS]', self.o_tag)
-        self.sep_tag = tag2idx.get('[SEP]', self.o_tag)
 
     def pair_tokens(self, mask):
         """Real tokens of the B*T pairs of a batch, from the host counts Estimator.to_device attaches to its mask
@@ -111,3 +119,11 @@ def device_table(params):
     if 'mrc_table' not in cache:
         cache['mrc_table'] = MrcTable(params)
     return cache['mrc_table']
+
+
+def type_table(params):
+    """The TypeTable of a params dict, built once: what a plugin without queries (bert_global_pointer) needs."""
+    cache = params.setdefault('_device_consts', {})
+    if 'type_table' not in cache:
+        cache['type_table'] = TypeTable(params)
+    return cache['type_table']

@@ -712,6 +712,102 @@ def mrc_span_decode(start_logits, end_logits, uv, b1, w2, b2, seq_len, type_tag,
     return pred
 
 
+# --------------------------------------------------------------------------- GlobalPointer span head (bert_global_pointer)
+GP_HEAD = 64                                     # D, the head size of ner_gp_*
+
+
+def _gp_rows(rot, B, L, cu_seqlens):
+    """rot [rows, T, 2, D] bf16 -> T; rows must be B*L (padded) or the packed count (checked by the caller's layout)."""
+    require_cuda(rot, cu_seqlens)
+    assert rot.dtype == torch.bfloat16 and rot.dim() == 4 and rot.shape[2] == 2 and rot.shape[3] == GP_HEAD
+    assert cu_seqlens is not None or rot.shape[0] == B * L
+    return rot.shape[1]
+
+
+def gp_targets(label_ids, seq_len, type_tag):
+    """label_ids [B, L] -> span_end [B, T, L] i32 (ner_gp_targets)."""
+    require_cuda(label_ids, seq_len, type_tag)
+    B, L = label_ids.shape
+    T = type_tag.shape[0]
+    assert type_tag.dtype == torch.int32 and tuple(type_tag.shape) == (T, 2)
+    out = torch.empty((B, T, L), dtype=torch.int32, device=label_ids.device)
+    check(lib().ner_gp_targets(ptr(_i32(label_ids)), ptr(_i32(seq_len)), ptr(type_tag), B, T, L, ptr(out), stream()))
+    return out
+
+
+def gp_rope(proj, B, L, T, cu_seqlens=None, split=False):
+    """proj [rows, >= T*2D] f32 (q | k of each type) -> (hi, lo | None) bf16 [rows, T, 2, D]: the rotated operands, q
+    scaled by 1/sqrt(D) (ner_gp_rope).  split: lo = the bf16 rest of the fp32 value."""
+    _require_rows(proj)
+    require_cuda(cu_seqlens)
+    rows = proj.shape[0]
+    hi = torch.empty((rows, T, 2, GP_HEAD), dtype=torch.bfloat16, device=proj.device)
+    lo = torch.empty_like(hi) if split else None
+    check(lib().ner_gp_rope(ptr(proj), proj.stride(0), ptr(cu_seqlens), B, T, L, ptr(hi), ptr(lo), stream()))
+    return hi, lo
+
+
+def gp_rope_bwd(d_rot, B, L, cu_seqlens=None):
+    """d_rot [rows, T, 2, D] f32 -> d_proj [rows, T*2D] f32 (ner_gp_rope_bwd)."""
+    require_cuda(d_rot, cu_seqlens)
+    rows, T = d_rot.shape[:2]
+    d_proj = torch.empty((rows, T * 2 * GP_HEAD), dtype=torch.float32, device=d_rot.device)
+    check(lib().ner_gp_rope_bwd(ptr(d_rot), ptr(cu_seqlens), B, T, L, ptr(d_proj), d_proj.stride(0), stream()))
+    return d_proj
+
+
+def gp_loss_fwd(hi, lo, seq_len, span_end, L, cu_seqlens=None):
+    """-> (loss [] f32, lse [B, T, 2] f32) of the multilabel span cross-entropy (ner_gp_loss_fwd); lo None = bf16 scores."""
+    require_cuda(lo, seq_len, span_end)
+    B = seq_len.shape[0]
+    T = _gp_rows(hi, B, L, cu_seqlens)
+    assert tuple(span_end.shape) == (B, T, L) and span_end.dtype == torch.int32
+    dev = hi.device
+    loss = torch.zeros((), dtype=torch.float32, device=dev)
+    lse = torch.zeros((B, T, 2), dtype=torch.float32, device=dev)
+    nbytes = int(lib().ner_gp_loss_workspace_bytes(B, T, L))
+    ws = _span_scratch('gp_loss', nbytes, dev)
+    check(lib().ner_gp_loss_fwd(ptr(hi), ptr(lo), ptr(_i32(seq_len)), ptr(cu_seqlens), ptr(span_end), B, T, L, ptr(loss),
+                                ptr(lse), ptr(ws), nbytes, stream()))
+    return loss, lse
+
+
+def gp_loss_bwd(rot, seq_len, span_end, lse, L, d_loss=1.0, cu_seqlens=None):
+    """-> d_rot [rows, T, 2, D] f32, the gradient of d_loss * the loss w.r.t. the rotated operands (ner_gp_loss_bwd)."""
+    require_cuda(seq_len, span_end, lse)
+    B = seq_len.shape[0]
+    T = _gp_rows(rot, B, L, cu_seqlens)
+    d_rot = torch.zeros(rot.shape, dtype=torch.float32, device=rot.device)
+    check(lib().ner_gp_loss_bwd(ptr(rot), ptr(_i32(seq_len)), ptr(cu_seqlens), ptr(span_end), ptr(lse), B, T, L,
+                                float(d_loss), ptr(d_rot), stream()))
+    return d_rot
+
+
+def gp_decode(hi, lo, seq_len, type_tag, o_id, cls_id, sep_id, L, cu_seqlens=None, cap=None, want_scores=False):
+    """Rotated operands -> pred_ids [B, L] i32 carrying .spans [B, cap] i32, .span_probs [B, cap] f32 and .span_counts [B]
+    i32 (ner_gp_decode).  cap None = L.  want_scores: also return the scores [B, T, L, L] f32 (valid at the candidates
+    only; a view of the workspace, overwritten by the next call on this stream)."""
+    require_cuda(lo, seq_len, type_tag)
+    B = seq_len.shape[0]
+    T = _gp_rows(hi, B, L, cu_seqlens)
+    assert tuple(type_tag.shape) == (T, 2) and type_tag.dtype == torch.int32
+    cap = L if cap is None else int(cap)
+    dev = hi.device
+    pred = torch.empty((B, L), dtype=torch.int32, device=dev)
+    spans = torch.empty((B, cap), dtype=torch.int32, device=dev)
+    probs = torch.empty((B, cap), dtype=torch.float32, device=dev)
+    counts = torch.zeros((B,), dtype=torch.int32, device=dev)
+    nbytes = int(lib().ner_gp_decode_workspace_bytes(B, T, L))
+    ws = _span_scratch('gp_decode', nbytes, dev)
+    check(lib().ner_gp_decode(ptr(hi), ptr(lo), ptr(_i32(seq_len)), ptr(cu_seqlens), ptr(type_tag), B, T, L, int(o_id),
+                              int(cls_id), int(sep_id), cap, ptr(pred), ptr(spans), ptr(probs), ptr(counts), ptr(ws), nbytes,
+                              stream()))
+    pred.spans, pred.span_probs, pred.span_counts = spans, probs, counts
+    if want_scores:
+        return pred, ws[:nbytes].view(torch.float32).view(B, T, L, L)
+    return pred
+
+
 # --------------------------------------------------------------------------- document windows (BERT document mode)
 def window_plan(token_ids, segment_ids, seq_len, W, S, NW, n_doc, packed=False, padded=False):
     """[B, L] documents -> their W-token windows (ner_window_plan): dict of ids / segment_ids / mask [NW, W] i32 and the

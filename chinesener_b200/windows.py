@@ -16,6 +16,7 @@ REFUSED = {
     'bert_dice': "its PREDICT argmax covers [PAD] positions",
     'bert_mrc': "its query/context pairs would need the query repeated in every window",
     'bert_mrc_span': "its query/context pairs would need the query repeated in every window",
+    'bert_global_pointer': "its PREDICT decode keeps a [B, T, L, L] score tensor",
 }
 
 

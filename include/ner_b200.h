@@ -641,6 +641,57 @@ int ner_mrc_span_decode(const float* start_logits, const float* end_logits, cons
                         int I, int o_id, int cls_id, int sep_id, int cap, int32_t* pred_ids, int32_t* spans,
                         float* span_probs, int32_t* span_counts, void* workspace, size_t workspace_bytes,
                         ner_stream_t stream);
+/* model/bert_global_pointer.py: the GlobalPointer span head (Su, 2021; a restatement, not pinned to the reference) over the
+ * BertModel sequence output of B sentences, T entity types, head size D = 64.  The projection P [rows, T*2D] f32 (one
+ * GEMM) holds q of type t in columns [t*2D, t*2D + D) and k in [t*2D + D, (t+1)*2D).  Rows are addressed padded (row b*L + s,
+ * cu_seqlens NULL) or packed (row cu_seqlens[b] + s, cu_seqlens [B+1] from ner_seq_pack_plan), as ner_bilstm_recurrence.
+ * With len_b = clamp(seq_len[b], 0, L) and m_b = len_b - 2, the candidates are 1 <= i <= j <= m_b and
+ *   s[b,t,i,j] = q'_i . k'_j,   q' = RoPE_i(q) / 8,  k' = RoPE_j(k),
+ * RoPE_s rotating each pair (2i, 2i+1) by the angle s * 10000^(-2i/D).  Common rules: T in [1, 32] and L <= 512, else
+ * NER_ERR_UNSUPPORTED; B*T*L*L < 2^31; B = 0 is a no-op; every check runs before any CUDA call; no allocation, no float
+ * atomics, bit-identical repeats.
+ *
+ * Targets: label_ids [B,L] i32, type_tag [T,2] (tag ids of B-X_t, I-X_t) -> span_end [B,T,L] i32 = for a B-X_t at s < len_b
+ * the end of the I-X_t run after it (s itself without one), else -1; an I-run without a B gives no span.  One launch. */
+int ner_gp_targets(const int32_t* label_ids, const int32_t* seq_len, const int32_t* type_tag, int B, int T, int L,
+                   int32_t* span_end, ner_stream_t stream);
+/* RoPE: proj [rows, ld_proj] f32 (ld_proj >= 2*D*T, even, 8-byte aligned) -> rot_hi bf16 [rows, T, 2, D] (q' then k' of
+ * each type, 16-byte aligned; the column of an element is its column in proj) and, when rot_lo is not NULL, the bf16 rest
+ * rot_lo = bf16(x - rot_hi) (ner_split_bf16's rule).  The angles are computed in double.  Rows: every (b, s < L) padded,
+ * every (b, s < cu[b+1] - cu[b]) packed.  One launch. */
+int ner_gp_rope(const float* proj, int ld_proj, const int32_t* cu_seqlens, int B, int T, int L, void* rot_hi, void* rot_lo,
+                ner_stream_t stream);
+/* Its backward: d_rot [rows, T, 2, D] f32 (16-byte aligned) -> d_proj [rows, ld_dproj] f32 = the transposed rotation (and
+ * the 1/8 of q), on the rows ner_gp_rope writes.  One launch. */
+int ner_gp_rope_bwd(const float* d_rot, const int32_t* cu_seqlens, int B, int T, int L, float* d_proj, int ld_dproj,
+                    ner_stream_t stream);
+/* Loss (bert4keras' global_pointer_crossentropy): per (b, t), with (i, j) positive iff j = span_end[b,t,i],
+ *   lse_neg = log(1 + sum over negative candidates e^s),  lse_pos = log(1 + sum over positive candidates e^-s),
+ * loss [1] = mean over B*T of lse_neg + lse_pos (0 for a (b, t) without candidates); lse [B*T, 2] f32 receives (lse_neg,
+ * lse_pos), which ner_gp_loss_bwd reads.  S = Q'K'^T on mma.sync (bf16 -> fp32); rot_lo not NULL adds hi.lo + lo.hi
+ * (fp32-accurate scores).  Per-tile partials in workspace (>= ner_gp_loss_workspace_bytes) merged in index order by a
+ * second launch. */
+size_t ner_gp_loss_workspace_bytes(int B, int T, int L);
+int ner_gp_loss_fwd(const void* rot_hi, const void* rot_lo, const int32_t* seq_len, const int32_t* cu_seqlens,
+                    const int32_t* span_end, int B, int T, int L, float* loss, float* lse, void* workspace,
+                    size_t workspace_bytes, ner_stream_t stream);
+/* Its backward for loss * d_loss: S recomputed from rot (bf16), dS = g e^(s - lse_neg) on negatives, -g e^(-s - lse_pos) on
+ * positives, 0 off the candidates, g = d_loss / (B*T); d_rot [rows, T, 2, D] f32 = (dS K' | dS^T Q') on every row of the
+ * layout (0 off the candidate rows).  Two launches: one owns query tiles, one key tiles. */
+int ner_gp_loss_bwd(const void* rot, const int32_t* seq_len, const int32_t* cu_seqlens, const int32_t* span_end,
+                    const float* lse, int B, int T, int L, float d_loss, float* d_rot, ner_stream_t stream);
+/* PREDICT / EVAL decode.  s is computed on the tensor cores (split as ner_gp_loss_fwd when rot_lo is not NULL) into the
+ * workspace (>= ner_gp_decode_workspace_bytes): after the call its first B*T*L*L floats hold s[b,t,i,j] at index
+ * ((b*T + t)*L + i)*L + j for every candidate (other entries are not written).  A span (i, j, t) is kept when s > 0, with
+ * span_probs = sigmoid(s) (a monotone score, not a calibrated probability).  spans [B, cap] i32 = i | (j + 1) << 12 | t << 24,
+ * ordered by (start, end, type); span_counts [B] = the true count (slots past the count are 0).  pred_ids [B, L] = the greedy
+ * non-overlapping projection of ner_mrc_span_decode (descending s, then lower type, start, end), with its tag rules.  cap >= 0
+ * (spans / span_probs may be NULL when cap = 0).  Two launches, no host synchronisation. */
+size_t ner_gp_decode_workspace_bytes(int B, int T, int L);
+int ner_gp_decode(const void* rot_hi, const void* rot_lo, const int32_t* seq_len, const int32_t* cu_seqlens,
+                  const int32_t* type_tag, int B, int T, int L, int o_id, int cls_id, int sep_id, int cap, int32_t* pred_ids,
+                  int32_t* spans, float* span_probs, int32_t* span_counts, void* workspace, size_t workspace_bytes,
+                  ner_stream_t stream);
 /* Window plan of the BERT plugins' document mode (documents longer than the position table).  Document b of the [B,L]
  * batch has n_b = clamp(seq_len[b], 0, L) tokens ([CLS] ... [SEP]), m = n_b - 2 content tokens; C = W - 2.
  *   n_b = 0: no window;  n_b <= W: one window, the document itself (its rows past n_b are [PAD]);
