@@ -175,6 +175,9 @@ SIGNATURES["ner_lexicon_create"] = (_vp, [_vp, _vp, _vp, _i])
 SIGNATURES["ner_lexicon_destroy"] = (None, [_vp])
 SIGNATURES["ner_lexicon_num_nodes"] = (_c.c_int64, [_vp])
 SIGNATURES["ner_lexicon_build"] = (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _i])
+SIGNATURES["ner_lexicon_build_lattice"] = (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _i])
+SIGNATURES["ner_lattice_recurrence"] = (_i, [_vp] * 9 + [_i] * 4 + [_vp] * 8)
+SIGNATURES["ner_lattice_recurrence_bwd"] = (_i, [_vp] * 16 + [_i] * 4 + [_vp])
 
 # return values of ner_crf_viterbi_plan, by enum value (include/ner_b200.h: NER_VIT_*)
 VIT_PLANS = ("small", "tma", "parked", "onchip_128", "onchip_32", "small_any_b", "none")

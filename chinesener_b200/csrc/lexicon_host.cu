@@ -230,3 +230,77 @@ extern "C" int ner_lexicon_build(const ner_lexicon* lx, const uint32_t* codepoin
   }
   return failed.load() ? NER_ERR_UNSUPPORTED : NER_OK;
 }
+
+namespace {
+// Lattice lists of one sentence: per start b, the 2..10-character vocabulary words at [b, b + n), trie order (increasing
+// length), cut to the Kw most frequent (stable).  -> number of matches the cut dropped.
+int64_t build_lattice_one(const ner_lexicon& lx, const uint32_t* cp, int n, int L, int Kw, int32_t* ids, int32_t* lens) {
+  const int32_t pad_id = lx.n_words + 1;
+  for (int s = 0; s < L * Kw; ++s) { ids[s] = pad_id; lens[s] = 0; }
+  const int n_keep = std::min(n, L);
+  int64_t dropped = 0;
+  std::pair<int32_t, int32_t> found[kMaxWordLen];   // (word id, length)
+  for (int b = 0; b < n_keep; ++b) {
+    int cnt = 0;
+    int32_t node = 0;
+    const int jend = std::min(b + kMaxWordLen, n_keep);
+    for (int j = b; j < jend; ++j) {
+      node = lx.find(node, cp[j]);
+      if (node < 0) break;
+      const int32_t w = lx.node_word[node];
+      if (w >= 0 && j > b) found[cnt++] = {w, j - b + 1};
+    }
+    if (cnt > Kw) {
+      std::stable_sort(found, found + cnt, [&](const std::pair<int32_t, int32_t>& a, const std::pair<int32_t, int32_t>& c) {
+        return lx.freq[a.first] > lx.freq[c.first];
+      });
+      dropped += cnt - Kw;
+      cnt = Kw;
+    }
+    for (int k = 0; k < cnt; ++k) { ids[b * Kw + k] = found[k].first; lens[b * Kw + k] = found[k].second; }
+  }
+  return dropped;
+}
+}  // namespace
+
+extern "C" int ner_lexicon_build_lattice(const ner_lexicon* lx, const uint32_t* codepoints_host,
+                                         const int64_t* sent_offsets_host, int n_sent, int max_seq_len, int Kw,
+                                         int32_t* ids_out_host, int32_t* lens_out_host, int64_t* dropped_out_host,
+                                         int n_threads) {
+  if (!lx || !sent_offsets_host || !ids_out_host || !lens_out_host || n_sent < 0 || max_seq_len < 1) return NER_ERR_INVALID_ARG;
+  if (Kw < 1 || Kw > 8) return NER_ERR_INVALID_ARG;
+  if (dropped_out_host) *dropped_out_host = 0;
+  if (n_sent == 0) return NER_OK;
+  if (!codepoints_host && sent_offsets_host[n_sent] > 0) return NER_ERR_INVALID_ARG;
+  const size_t row = (size_t)max_seq_len * Kw;
+  int nt = n_threads > 0 ? n_threads : (int)std::thread::hardware_concurrency();
+  nt = std::max(1, std::min(nt, std::min(n_sent, 256)));
+  std::atomic<int> next(0);
+  std::atomic<int64_t> dropped(0);
+  auto work = [&]() {
+    int64_t mine = 0;
+    for (;;) {
+      const int s0 = next.fetch_add(64);
+      if (s0 >= n_sent) break;
+      for (int s = s0; s < std::min(s0 + 64, n_sent); ++s) {
+        const int64_t a = sent_offsets_host[s], b = sent_offsets_host[s + 1];
+        mine += build_lattice_one(*lx, codepoints_host + a, (int)(b - a), max_seq_len, Kw, ids_out_host + s * row,
+                                  lens_out_host + s * row);
+      }
+    }
+    dropped.fetch_add(mine);
+  };
+  if (nt == 1) {
+    work();
+  } else {
+    std::vector<std::thread> pool;
+    try {
+      for (int t = 0; t < nt; ++t) pool.emplace_back(work);
+    } catch (...) {   // could not start every thread: the started ones (or this thread, below) finish the job
+    }
+    for (auto& th : pool) th.join();
+    if (pool.empty()) work();
+  }
+  if (dropped_out_host) *dropped_out_host = dropped.load();
+  return NER_OK;
+}

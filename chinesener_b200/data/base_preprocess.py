@@ -8,16 +8,17 @@ import torch
 
 from .tokenizer import TokenizerBert, TokenizerGiga
 
-SoftWord, ExSoftWord, SoftLexicon, BiChar = 'softword', 'ex_softword', 'softlexicon', 'bichar'
-WordEnhanceMethod = [SoftWord, ExSoftWord, SoftLexicon, BiChar]
+SoftWord, ExSoftWord, SoftLexicon, BiChar, Lattice = 'softword', 'ex_softword', 'softlexicon', 'bichar', 'lattice'
+WordEnhanceMethod = [SoftWord, ExSoftWord, SoftLexicon, BiChar, Lattice]
 
 
 def extract_prefix_surfix(model_name):
     """-> (word_enhance, tokenizer_type) from the model name (reference :25-36): a name containing 'bert' uses the BERT
-    tokenizer, else giga; the word-enhance method is the first of softword / softlexicon / ex_softword / bichar the
-    alternation finds (leftmost match, alternatives tried in that order — 'ex_softword' names match 'softword' only
-    when no earlier position matches, exactly as the reference's regex does)."""
-    m = re.search('({})|({})|({})|({})'.format(SoftWord, SoftLexicon, ExSoftWord, BiChar), model_name)
+    tokenizer, else giga; the word-enhance method is the first of softword / softlexicon / ex_softword / bichar / lattice
+    the alternation finds (leftmost match, alternatives tried in that order — 'ex_softword' names match 'softword' only
+    when no earlier position matches, exactly as the reference's regex does; 'lattice' comes last, so every name without
+    it maps as the reference maps it)."""
+    m = re.search('({})|({})|({})|({})|({})'.format(SoftWord, SoftLexicon, ExSoftWord, BiChar, Lattice), model_name)
     word_enhance = m.group() if m else None
     tokenizer_type = TokenizerBert if re.search('({})'.format(TokenizerBert), model_name) else TokenizerGiga
     return word_enhance, tokenizer_type
@@ -26,14 +27,15 @@ def extract_prefix_surfix(model_name):
 def get_instance(tokenizer_type, max_seq_len, tag2idx, tokenizer, word_enhance=None, **kwargs):
     """reference :75-93 — the processor class for a word-enhance method (None -> BasicProc, softlexicon ->
     SoftLexiconProc(vocab), bichar -> BiCharProc(bichar_tokenizer), softword -> SoftWordProc(cut), ex_softword ->
-    ExSoftWordProc(vocab)); the tokenizer object and the method's keyword arguments are passed in instead of being
-    looked up by name because vocabularies / vectors live wherever the caller keeps them."""
+    ExSoftWordProc(vocab), lattice -> LatticeProc(vocab, word_embedding)); the tokenizer object and the method's keyword
+    arguments are passed in instead of being looked up by name because vocabularies / vectors live wherever the caller
+    keeps them."""
     assert word_enhance in [None] + WordEnhanceMethod, 'word_enhance must in {}'.format(','.join(WordEnhanceMethod))
     if word_enhance is None:
         return BasicProc(tokenizer_type, max_seq_len, tag2idx, tokenizer)
     from . import word_enhance as we
     cls = {SoftLexicon: we.SoftLexiconProc, BiChar: we.BiCharProc, SoftWord: we.SoftWordProc,
-           ExSoftWord: we.ExSoftWordProc}[word_enhance]
+           ExSoftWord: we.ExSoftWordProc, Lattice: we.LatticeProc}[word_enhance]
     return cls(tokenizer_type, max_seq_len, tag2idx, tokenizer, **kwargs)
 
 
@@ -86,7 +88,7 @@ def features_to_batch(features, pin_memory=False):
     out['seq_len'] = torch.tensor([f['seq_len'] for f in features], dtype=torch.int32)
     out['label_ids'] = torch.tensor([f.get('label_ids', [0] * L) for f in features], dtype=torch.int32)
     # optional per-plugin features (dataset.py:29-36, MultiDataset.add_discriminator :88-90)
-    for k in ('softlexicon_ids', 'bichar_ids', 'softword_ids'):
+    for k in ('softlexicon_ids', 'bichar_ids', 'softword_ids', 'lattice_ids', 'lattice_lens'):
         if k in features[0]:
             out[k] = torch.tensor([f[k] for f in features], dtype=torch.int32)
     for k in ('softlexicon_weights', 'ex_softword_ids'):

@@ -10,16 +10,16 @@ TFRecords.
     python -m chinesener_b200.data.preprocess --src <dir with train/ val/ test/> --out datasets/msra \
         --tokenizer giga --giga_vec <gigaword .vec>  [--bert_vocab <vocab.txt>]
         [--word_enhance bichar --bichar_vec <bigram .vec> | --word_enhance ex_softword --word_vec <word .vec>
-         | --word_enhance softword]
+         | --word_enhance lattice --word_vec <word .vec> | --word_enhance softword]
 """
 import argparse
 import os
 import pickle
 
-from .base_preprocess import BiChar, ExSoftWord, SoftWord, get_instance
+from .base_preprocess import BiChar, ExSoftWord, Lattice, SoftWord, get_instance
 from .records import write_records
 from .tokenizer import TextVectors, TokenizerBert, TokenizerGiga, get_bert_tokenizer, get_giga_tokenizer
-from .word_enhance import WordVocab
+from .word_enhance import WordVocab, lattice_word_embedding
 
 # data/msra/preprocess.py:7-27 (people_daily uses the same tag set and length)
 MSRA_TAG2IDX = {'[PAD]': 0, 'O': 1, 'B-ORG': 2, 'I-ORG': 3, 'B-PER': 4, 'I-PER': 5, 'B-LOC': 6, 'I-LOC': 7, '[CLS]': 8, '[SEP]': 9}
@@ -105,12 +105,13 @@ def main(argv=None):
     ap.add_argument('--max_seq_len', type=int, default=MSRA_MAX_SEQ_LEN)
     ap.add_argument('--seed', type=int, default=1234, help='seed of the two add-on embedding rows ([PAD], [UNK])')
     ap.add_argument('--format', default='ner', choices=['ner', 'msr'], help="'msr': word-segmented msr_<split>.utf8 files (CWS tags)")
-    ap.add_argument('--word_enhance', default=None, choices=[BiChar, SoftWord, ExSoftWord],
+    ap.add_argument('--word_enhance', default=None, choices=[BiChar, SoftWord, ExSoftWord, Lattice],
                     help='extra input of the bilstm_crf_<word_enhance> plugins (giga tokenizer); softword segments with jieba')
     ap.add_argument('--bichar_vec', default='./pretrain_model/giga/gigaword_chn.all.a2b.bi.ite50.vec',
                     help='bigram vectors (giga .vec format) for --word_enhance bichar')
     ap.add_argument('--word_vec', default='./pretrain_model/ctb50/ctb.50d.vec',
-                    help='word vectors (giga .vec format) whose vocabulary is the lexicon of --word_enhance ex_softword')
+                    help='word vectors (giga .vec format) whose vocabulary is the lexicon of --word_enhance ex_softword / '
+                         'lattice (lattice also keeps the vectors as the word table)')
     args = ap.parse_args(argv)
     if args.tokenizer == TokenizerGiga:
         tok = get_giga_tokenizer(args.giga_vec)
@@ -125,12 +126,18 @@ def main(argv=None):
     elif args.word_enhance == ExSoftWord:
         words = TextVectors(args.word_vec).index2word
         kwargs['vocab'] = WordVocab(words, dict.fromkeys(words, 1))
+    elif args.word_enhance == Lattice:
+        vec = TextVectors(args.word_vec)
+        kwargs['vocab'] = WordVocab(vec.index2word, dict.fromkeys(vec.index2word, 1))
+        kwargs['word_embedding'] = lattice_word_embedding(vec, args.seed)
     proc = get_instance(args.tokenizer, args.max_seq_len, MSR_TAG2IDX if msr else MSRA_TAG2IDX, tok,
                         word_enhance=args.word_enhance, **kwargs)
     for file in (MSR_MAPPING if msr else MAPPING):
         print('Dumping records for {} tokenizer = {}'.format(file, args.tokenizer))
         dump_records(proc, args.src, args.out, file, mapping=MSR_MAPPING if msr else MAPPING, embedding=emb,
                      load_data=load_msr_data if msr else None, word_enhance=args.word_enhance, bichar_embedding=bichar_emb)
+        if args.word_enhance == Lattice:
+            print('lattice words dropped by the max_lattice_words cap so far: {}'.format(proc.dropped))
 
 
 if __name__ == '__main__':

@@ -25,6 +25,7 @@ from .tokenizer import TokenizerBert
 MaxWordLen = 10
 MaxLexiconLen = 10      # only keep top-n words per B/M/E/S set
 SoftKeys = ('B', 'M', 'E', 'S')
+MaxLatticeWords = 4     # lattice words kept per start character (the most frequent)
 
 
 class WordVocab(object):
@@ -102,6 +103,22 @@ class NativeLexicon(object):
             None if toff is None else toff.ctypes.data, max_seq_len, 1 if bert else 0, ids.ctypes.data, wts.ctypes.data, n_threads))
         _lib.LAUNCHES -= 1          # host call, not a kernel launch
         return ids, wts
+
+    def build_lattice(self, sentences, max_seq_len, max_words=MaxLatticeWords, n_threads=0):
+        """Lattice word lists (ner_lexicon_build_lattice): sentences are lists of characters (or strings, one character per
+        position).  -> (ids int32 [n, max_seq_len * max_words], lens int32 [n, max_seq_len * max_words], number of matches
+        the max_words cap dropped)."""
+        from .. import _lib
+        n = len(sentences)
+        cps, offs = _utf32([''.join(s) for s in sentences])
+        ids = np.empty((n, max_seq_len * max_words), np.int32)
+        lens = np.empty(ids.shape, np.int32)
+        dropped = np.zeros(1, np.int64)
+        _lib.check(self._lib.ner_lexicon_build_lattice(
+            self._h, cps.ctypes.data if cps.size else None, offs.ctypes.data, n, max_seq_len, max_words, ids.ctypes.data,
+            lens.ctypes.data, dropped.ctypes.data, n_threads))
+        _lib.LAUNCHES -= 1          # host call, not a kernel launch
+        return ids, lens, int(dropped[0])
 
 
 class SoftLexiconProc(BasicProc):
@@ -207,6 +224,50 @@ class ExSoftWordProc(BasicProc):
 
     def build_seq_feature(self, sentence):
         return self.build_seq_features([sentence], n_threads=1)[0]
+
+
+class LatticeProc(BasicProc):
+    """BasicProc + lattice_ids / lattice_lens [L * max_lattice_words] int32: for each character the vocabulary words of
+    2..10 characters starting there (the giga tokenizer's characters, whitespace dropped), the most frequent
+    max_lattice_words of them (NativeLexicon.build_lattice).  `word_embedding` (the [n_word + 3, Ew] table whose rows
+    follow `vocab`) initialises the plugin's trainable word table.  `dropped` counts the matches the cap discarded."""
+
+    def __init__(self, tokenizer_type, max_seq_len, tag2idx, tokenizer, vocab, word_embedding=None, vocabfreq=None,
+                 max_lattice_words=MaxLatticeWords):
+        _reject_bert(tokenizer_type, 'LatticeProc')
+        super(LatticeProc, self).__init__(tokenizer_type, max_seq_len, tag2idx, tokenizer)
+        self.vocab, self.word_embedding, self.max_lattice_words = vocab, word_embedding, int(max_lattice_words)
+        self.word_enhance = 'lattice'
+        self.lexicon = NativeLexicon(vocab, vocabfreq)
+        self.dropped = 0
+
+    def build_seq_features(self, sentences, n_threads=0):
+        feats = [super(LatticeProc, self).build_seq_feature(s) for s in sentences]
+        chars = [[c for c in s if c.strip()] for s in sentences]
+        ids, lens, dropped = self.lexicon.build_lattice(chars, self.max_seq_len, self.max_lattice_words, n_threads)
+        self.dropped += dropped
+        for f, i, n in zip(feats, ids, lens):
+            f['lattice_ids'], f['lattice_lens'] = i.tolist(), n.tolist()
+        return feats
+
+    def build_seq_feature(self, sentence):
+        return self.build_seq_features([sentence], n_threads=1)[0]
+
+    def build_data_params(self, n_sample):
+        params = super(LatticeProc, self).build_data_params(n_sample)
+        params.update({'max_lattice_words': self.max_lattice_words, 'vocab2idx': self.vocab.vocab2idx,
+                       'word_embedding': self.word_embedding})
+        return params
+
+
+def lattice_word_embedding(vectors, seed=1234):
+    """[n_word + 3, Ew] float32 table for a WordVocab over `vectors` (TextVectors): the word vectors, then N(0, 1) rows for
+    <None> and <eos> and a zero row for <PAD> (the id of empty lattice slots)."""
+    rng = np.random.RandomState(seed)
+    v = np.asarray(vectors.vectors, np.float32)
+    extra = rng.normal(0, 1, size=(3, v.shape[1])).astype(np.float32)
+    extra[1] = 0.0
+    return np.vstack([v, extra]).astype(np.float32)
 
 
 def softword_labels(words):

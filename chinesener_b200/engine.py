@@ -14,7 +14,7 @@ import torch
 from . import autodiff, variables
 
 _DEVICE_KEYS = ('token_ids', 'mask', 'segment_ids', 'label_ids', 'seq_len', 'softlexicon_ids', 'softlexicon_weights',
-                'bichar_ids', 'softword_ids', 'ex_softword_ids', 'task_ids')
+                'bichar_ids', 'softword_ids', 'ex_softword_ids', 'task_ids', 'lattice_ids', 'lattice_lens')
 
 
 def load_plugin(model_name):

@@ -306,6 +306,53 @@ def bigru_recurrence_bwd(d_out, gates, hstate, wh_fw, wh_bw, seq_len, B, L, H, a
     return d_xproj
 
 
+# --------------------------------------------------------------------------- Lattice LSTM
+def lattice_recurrence(xproj, wproj, lat_len, wrec_fw, wrec_bw, wac_fw, wac_bw, seq_len, B, L, H, Kw,
+                       save_for_backward=False):
+    """Lattice LSTM recurrence of both directions (ner_lattice_recurrence): xproj [B*L, 8H], wproj [B*L*Kw, 6H],
+    lat_len int32 [B, L*Kw], wrec_* [H, 6H], wac_* [H, H] -> out [B, L, 2H]; with save_for_backward also the dict of
+    saved tensors lattice_recurrence_bwd reads (gates, cstate, norm, wgates, cw, aw, hw)."""
+    require_cuda(xproj, wproj, lat_len, wrec_fw, wrec_bw, wac_fw, wac_bw, seq_len)
+    assert xproj.dtype == torch.float32 and xproj.shape == (B * L, 8 * H)
+    assert wproj.dtype == torch.float32 and wproj.shape == (B * L * Kw, 6 * H)
+    assert lat_len.dtype == torch.int32 and lat_len.numel() == B * L * Kw
+    assert wrec_fw.shape == (H, 6 * H) and wrec_bw.shape == (H, 6 * H) and wac_fw.shape == (H, H) and wac_bw.shape == (H, H)
+    dev = xproj.device
+    out = torch.empty((B, L, 2 * H), dtype=torch.float32, device=dev)
+    sv = None
+    if save_for_backward:
+        sv = dict(gates=torch.zeros((B * L, 6 * H), dtype=torch.float32, device=dev),
+                  cstate=torch.zeros((B, L, 2 * H), dtype=torch.float32, device=dev),
+                  norm=torch.zeros((B, L, 2 * H), dtype=torch.float32, device=dev),
+                  wgates=torch.zeros((B * L * Kw, 6 * H), dtype=torch.float32, device=dev),
+                  cw=torch.zeros((B * L * Kw, 2 * H), dtype=torch.float32, device=dev),
+                  aw=torch.zeros((B * L * Kw, 2 * H), dtype=torch.float32, device=dev),
+                  hw=torch.zeros((B * L * Kw, 2 * H), dtype=torch.float32, device=dev))
+    s = sv or {}
+    check(lib().ner_lattice_recurrence(ptr(xproj), ptr(wproj), ptr(lat_len), ptr(wrec_fw), ptr(wrec_bw), ptr(wac_fw),
+                                       ptr(wac_bw), ptr(_i32(seq_len)), ptr(out), B, L, H, Kw, ptr(s.get('gates')),
+                                       ptr(s.get('cstate')), ptr(s.get('norm')), ptr(s.get('wgates')), ptr(s.get('cw')),
+                                       ptr(s.get('aw')), ptr(s.get('hw')), stream()))
+    return (out, sv) if save_for_backward else out
+
+
+def lattice_recurrence_bwd(d_out, saved, lat_len, wrec_fw, wrec_bw, wac_fw, wac_bw, seq_len, B, L, H, Kw):
+    """-> (d_xproj [B*L, 8H], d_wproj [B*L*Kw, 6H], d_alpha [B*L*Kw, 2H]): the gradients of the two hoisted projections
+    and of each word's alpha pre-activation (zero on empty slots)."""
+    require_cuda(d_out, lat_len, wrec_fw, wrec_bw, wac_fw, wac_bw, seq_len)
+    assert d_out.shape == (B, L, 2 * H) and d_out.dtype == torch.float32
+    dev = d_out.device
+    d_xproj = torch.empty((B * L, 8 * H), dtype=torch.float32, device=dev)
+    d_wproj = torch.zeros((B * L * Kw, 6 * H), dtype=torch.float32, device=dev)
+    d_alpha = torch.zeros((B * L * Kw, 2 * H), dtype=torch.float32, device=dev)
+    s = saved
+    check(lib().ner_lattice_recurrence_bwd(ptr(d_out), ptr(s['gates']), ptr(s['cstate']), ptr(s['norm']), ptr(s['wgates']),
+                                           ptr(s['cw']), ptr(s['aw']), ptr(lat_len), ptr(wrec_fw), ptr(wrec_bw),
+                                           ptr(wac_fw), ptr(wac_bw), ptr(_i32(seq_len)), ptr(d_xproj), ptr(d_wproj),
+                                           ptr(d_alpha), B, L, H, Kw, stream()))
+    return d_xproj, d_wproj, d_alpha
+
+
 # --------------------------------------------------------------------------- SoftLexicon
 def softlexicon_pool(table, ids, weights, G=4, S=10, out=None):
     """ids/weights [..., G*S] -> [..., G*E]; `out` may be a wider [n_tok, >=G*E] buffer (concat target)."""

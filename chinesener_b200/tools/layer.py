@@ -367,6 +367,126 @@ def _rnn_layer_train(embedding, cell, i, scope, activation, H, keep, seq_len):
     return out
 
 
+LATTICE_PARTS = ("char_cell", "word_cell", "alpha")
+
+
+def _lattice_variables(store, scope, Ec, Ew, H):
+    """{d: {part: (kernel, bias)}} of the lattice layer, created fw then bw: char_cell [Ec+H, 3H] (i, o, g), word_cell
+    [Ew+H, 3H] (f, i, g), alpha [Ec+H, H]; glorot-uniform kernels, zero biases."""
+    names = {}
+    for d in ("fw", "bw"):
+        names[d] = {}
+        for part, din, n in (("char_cell", Ec, 3 * H), ("word_cell", Ew, 3 * H), ("alpha", Ec, H)):
+            k, b = f"{scope}/{d}/{part}/kernel", f"{scope}/{d}/{part}/bias"
+            store.get_variable(k, (din + H, n), variables.glorot_uniform)
+            store.get_variable(b, (n,), variables.zeros)
+            names[d][part] = (k, b)
+    return names
+
+
+def _pack_kn(w, b):
+    """[K, N] f32 kernel + [N] bias -> (bf16 [Np, Kp] GEMM operand, f32 [Np] bias, Kp, Np): K padded to 8, N to 32."""
+    K, N = w.shape
+    Kp, Np = (K + 7) // 8 * 8, (N + 31) // 32 * 32
+    w = torch.nn.functional.pad(w, (0, Np - N, 0, Kp - K))
+    return ops.pack_weight_bf16(w.contiguous()), torch.nn.functional.pad(b, (0, Np - N)).contiguous(), Kp, Np
+
+
+def _lattice_pack(store, names, Ec, Ew, H):
+    def build():
+        v = store.vars
+        k = {d: {p: v[names[d][p][0]] for p in LATTICE_PARTS} for d in ("fw", "bw")}
+        b = {d: {p: v[names[d][p][1]] for p in LATTICE_PARTS} for d in ("fw", "bw")}
+        wx = torch.cat([torch.cat([k[d]["char_cell"][:Ec], k[d]["alpha"][:Ec]], 1) for d in ("fw", "bw")], 1)   # [Ec, 8H]
+        bx = torch.cat([torch.cat([b[d]["char_cell"], b[d]["alpha"]]) for d in ("fw", "bw")])
+        ww = torch.cat([k[d]["word_cell"][:Ew] for d in ("fw", "bw")], 1)                                      # [Ew, 6H]
+        bw = torch.cat([b[d]["word_cell"] for d in ("fw", "bw")])
+        xc, xcb, Kc, _ = _pack_kn(wx, bx)
+        xw, xwb, Kw_, _ = _pack_kn(ww, bw)
+        return dict(wx=wx, ww=ww, xc=xc, xcb=xcb, Kc=Kc, xw=xw, xwb=xwb, Kw=Kw_,
+                    wrec={d: torch.cat([k[d]["char_cell"][Ec:], k[d]["word_cell"][Ew:]], 1).contiguous() for d in ("fw", "bw")},
+                    wac={d: k[d]["alpha"][Ec:].contiguous() for d in ("fw", "bw")})
+    return store.cached(("lattice_pack", names["fw"]["char_cell"][0], Ec, Ew), build)
+
+
+def _proj(x2d, w16, bias, Kp, N):
+    """x [M, K] f32 @ packed weight + bias -> f32 [M, N] (bf16 operands, fp32 accumulate)."""
+    y = ops.gemm_bf16(ops.cast_pad_bf16(x2d, Kp), w16, bias, epilogue=ops.EPI_F32)
+    return y if y.shape[1] == N else y[:, :N].contiguous()
+
+
+def _input_grad(dy, w_kn):
+    """dx [M, K] = dy [M, N] · w [K, N]^T on the tensor cores."""
+    K, N = w_kn.shape
+    Np, Kp = (N + 7) // 8 * 8, (K + 31) // 32 * 32
+    wt = torch.nn.functional.pad(w_kn, (0, Np - N, 0, Kp - K)).to(torch.bfloat16).contiguous()
+    return ops.gemm_bf16(ops.cast_pad_bf16(dy, Np), wt, None, epilogue=ops.EPI_F32)[:, :K]
+
+
+def lattice_lstm(char_input, word_input, lattice_lens, hidden_units, seq_len, is_training):
+    """Bidirectional Lattice LSTM (Zhang & Yang, ACL 2018) as defined in model/lattice_lstm_crf.py -> [B, L, 2H] f32.
+
+    char_input [B, L, Ec] f32; word_input [B*L, Kw*Ew] f32: the embedding of word slot (b, p, k) in row b*L + p, columns
+    k*Ew.. (zero rows for empty slots are fine); lattice_lens int32 [B, L*Kw]: slot lengths, a slot is empty when its length
+    is outside [2, 10] or the word reaches past seq_len.  The char/alpha and word-cell input projections are bf16 GEMMs
+    (fp32 accumulate) for both directions; the recurrence is ner_lattice_recurrence.  TRAIN records the backward:
+    ner_lattice_recurrence_bwd, then every weight and bias gradient as a GEMM over its outputs (no float atomics)."""
+    B, L, Ec = char_input.shape
+    H = int(hidden_units)
+    Kw = lattice_lens.shape[1] // L
+    Ew = word_input.shape[1] // Kw
+    store = variables.default_store()
+    names = _lattice_variables(store, variables.scoped("lattice_layer"), Ec, Ew, H)
+    pk = _lattice_pack(store, names, Ec, Ew, H)
+    x2d = char_input.reshape(B * L, Ec).contiguous()
+    w2d = word_input.reshape(B * L * Kw, Ew).contiguous()
+    xproj = _proj(x2d, pk["xc"], pk["xcb"], pk["Kc"], 8 * H)
+    wproj = _proj(w2d, pk["xw"], pk["xwb"], pk["Kw"], 6 * H)
+    lens = lattice_lens.to(torch.int32).contiguous()
+    args = (lens, pk["wrec"]["fw"], pk["wrec"]["bw"], pk["wac"]["fw"], pk["wac"]["bw"], seq_len, B, L, H, Kw)
+    tape = autodiff.current() if is_training else None
+    if tape is None:
+        return ops.lattice_recurrence(xproj, wproj, *args)
+    out, saved = ops.lattice_recurrence(xproj, wproj, *args, save_for_backward=True)
+    need_dc, need_dw = tape.needs_grad(char_input), tape.needs_grad(word_input)
+
+    def bwd(g):
+        if g is None:
+            return
+        dxp, dwp, dal = ops.lattice_recurrence_bwd(g.contiguous(), saved, *args)
+        gr = store.grad
+        dwx = ops.wgrad_gemm(x2d, dxp)            # [Ec, 8H]
+        dww = ops.wgrad_gemm(w2d, dwp)            # [Ew, 6H]
+        db_x = ops.wgrad_gemm(torch.ones((B * L, 8), dtype=torch.float32, device=out.device), dxp)
+        db_w = ops.wgrad_gemm(torch.ones((B * L * Kw, 8), dtype=torch.float32, device=out.device), dwp)
+        for di, d in enumerate(("fw", "bw")):
+            nm = names[d]
+            c0, w0 = di * 4 * H, di * 3 * H
+            hprev = torch.zeros((B, L, H), dtype=torch.float32, device=out.device)
+            if di == 0:
+                hprev[:, 1:] = out[:, :-1, :H]
+            else:
+                hprev[:, :-1] = out[:, 1:, H:]
+            dz_c, da_x, dz_w = dxp[:, c0:c0 + 3 * H], dxp[:, c0 + 3 * H:c0 + 4 * H], dwp[:, w0:w0 + 3 * H]
+            # bias gradients as GEMMs against a ones operand: fixed summation order, so repeats are bit-identical
+            gr(nm["char_cell"][1]).add_(db_x[0, c0:c0 + 3 * H])
+            gr(nm["alpha"][1]).add_(db_x[0, c0 + 3 * H:c0 + 4 * H])
+            gr(nm["word_cell"][1]).add_(db_w[0, w0:w0 + 3 * H])
+            gc, gw, ga = gr(nm["char_cell"][0]), gr(nm["word_cell"][0]), gr(nm["alpha"][0])
+            gc[:Ec] += dwx[:, c0:c0 + 3 * H]
+            ga[:Ec] += dwx[:, c0 + 3 * H:c0 + 4 * H]
+            gw[:Ew] += dww[:, w0:w0 + 3 * H]
+            gc[Ec:] += ops.wgrad_gemm(hprev.view(B * L, H), dz_c)                                   # h_prev^T dz
+            gw[Ew:] += ops.wgrad_gemm(saved["hw"][:, di * H:(di + 1) * H], dz_w)                    # h_start^T dz_w
+            ga[Ec:] += ops.wgrad_gemm(saved["cw"][:, di * H:(di + 1) * H], dal[:, di * H:(di + 1) * H])   # C^w^T da
+        if need_dc:
+            tape.add_grad(char_input, _input_grad(dxp, pk["wx"]).reshape(B, L, Ec).contiguous())
+        if need_dw:
+            tape.add_grad(word_input, _input_grad(dwp, pk["ww"]).reshape(word_input.shape).contiguous())
+    tape.record(out, bwd)
+    return out
+
+
 def cnn_layer(embedding, filter_list, kernel_size_list, activation, drop_out, is_training):
     """reference tools/layer.py:44-60 — tf.layers.conv1d(padding='SAME') per kernel size (+ dropout), concatenated.
     A kernel-k convolution over [B, L, C] is the label-projection kernel (ner_dense_small_n, filters <= 32) applied to the

@@ -843,6 +843,43 @@ int64_t ner_lexicon_num_nodes(const ner_lexicon* lexicon);
 int ner_lexicon_build(const ner_lexicon* lexicon, const uint32_t* codepoints_host, const int64_t* sent_offsets_host,
                       int n_sent, const int32_t* tok_len_host, const int64_t* tok_offsets_host, int max_seq_len,
                       int bert_mode, int32_t* ids_out_host, float* weights_out_host, int n_threads);
+/* Lattice word lists of the lattice_lstm_crf plugin (giga characters only), same trie walk and thread pool as
+ * ner_lexicon_build.  For each start character b < max_seq_len, the vocabulary words of 2..10 characters that match the
+ * sentence at [b, b + n) fill the Kw slots [b * Kw, (b + 1) * Kw): at most Kw of them, the most frequent first (stable
+ * over the trie's discovery order, i.e. increasing length).  A word must end inside the first max_seq_len characters.
+ * Empty slots: id <PAD> (n_words + 1), length 0.  ids_out / lens_out: [n_sent, max_seq_len * Kw] int32.
+ * dropped_out (may be NULL): number of matches the Kw cap discarded over all sentences.  1 <= Kw <= 8. */
+int ner_lexicon_build_lattice(const ner_lexicon* lexicon, const uint32_t* codepoints_host, const int64_t* sent_offsets_host,
+                              int n_sent, int max_seq_len, int Kw, int32_t* ids_out_host, int32_t* lens_out_host,
+                              int64_t* dropped_out_host, int n_threads);
+
+/* ------------------------------------------------------------------------ *
+ * Lattice LSTM recurrence (Zhang & Yang, ACL 2018) — model/lattice_lstm_crf.py.  Padded layout [B, L].
+ * ------------------------------------------------------------------------ */
+/* Word slots: lat_len [B, L * Kw] int32, slot (b, p, k) = a word of lat_len characters starting at position p.  A slot is
+ * empty when its length is outside [2, 10] or the word would reach past seq_len[b].  Per direction d (fw = 0, bw = 1):
+ *   xproj [B*L, 8H]: columns d*4H + (z_i, z_o, z_g, x-part of alpha) = x_t W + b of the char cell and alpha;
+ *   wproj [B*L*Kw, 6H]: columns d*3H + (z_f, z_i, z_g) = x^w W_x + b of the word cell of slot (b, p, k);
+ *   wrec_d [H, 6H] = [char_cell kernel[Ec:] | word_cell kernel[Ew:]];  wac_d [H, H] = alpha kernel[Ec:].
+ * out [B, L, 2H] (fw | bw, zero for t >= seq_len).  The backward direction runs right to left and merges a word at its
+ * first character; its cell is computed at the word's last character.  Training saves (all NULL or all given):
+ *   gates [B*L, 6H] (sigmoid i, sigmoid o, tanh g per direction), cstate [B, L, 2H], norm [B, L, 2H] (e^i + sum e^a, 0 at
+ *   steps without words), wgates [B*L*Kw, 6H] (sigmoid f, sigmoid i, tanh g), cw / aw / hw [B*L*Kw, 2H] (word cell,
+ *   alpha gate, h the word cell read).  Slot outputs are written for filled slots only: the caller zeroes them.
+ * Limits: Kw <= 8; H small enough for the recurrent weights to fit on a cluster of at most 8 CTAs (H <= 240). */
+int ner_lattice_recurrence(const float* xproj, const float* wproj, const int32_t* lat_len, const float* wrec_fw,
+                           const float* wrec_bw, const float* wac_fw, const float* wac_bw, const int32_t* seq_len,
+                           float* out, int B, int L, int H, int Kw, float* gates, float* cstate, float* norm,
+                           float* wgates, float* cw, float* aw, float* hw, ner_stream_t stream);
+/* Back-propagation through time of ner_lattice_recurrence, from its saved tensors.  Writes d_xproj [B*L, 8H] (every row;
+ * zero for t >= seq_len), and for filled slots only d_wproj [B*L*Kw, 6H] and d_alpha [B*L*Kw, 2H] (the gradient of the
+ * alpha pre-activation of each word): the caller zeroes those two.  Weight gradients are GEMMs over them:
+ * dW_rec = [h_prev^T dz_char | hw^T d_wproj], dW_ac = cw^T d_alpha, dW_x = x^T d_xproj, d_bias = column sums. */
+int ner_lattice_recurrence_bwd(const float* d_out, const float* gates, const float* cstate, const float* norm,
+                               const float* wgates, const float* cw, const float* aw, const int32_t* lat_len,
+                               const float* wrec_fw, const float* wrec_bw, const float* wac_fw, const float* wac_bw,
+                               const int32_t* seq_len, float* d_xproj, float* d_wproj, float* d_alpha, int B, int L,
+                               int H, int Kw, ner_stream_t stream);
 
 #ifdef __cplusplus
 }
