@@ -18,7 +18,7 @@ using namespace crf;
 constexpr int TAGP = 12;
 
 template <int K, int NT>
-size_t bwd_smem_bytes() {
+constexpr size_t bwd_smem_bytes() {
   using Gm = Geom<K>;
   size_t words = 3 * Gm::KK4 + 32 + NT + 2 * (size_t)NSTAGE * NT * Gm::P + (size_t)NSTAGE * NT * TAGP;
   return words * 4;
@@ -335,7 +335,9 @@ template <int K>
 int launch_bwd(const float* logits, const int32_t* tags, const int32_t* seq_len, const float* trans,
                const float* alpha_ws, const float* logz, const float* d_ll, float scale, float* d_logits,
                float* d_trans, int B, int L, cudaStream_t st) {
-  if (B > ner_num_sms() * 64 * 2)
+  // 64-thread CTAs need twice the staging ring of 32-thread ones: past K = 26 that is more shared memory than a CTA
+  // can have, so those K stay on 32-thread CTAs at every B
+  if (bwd_smem_bytes<K, 64>() <= kMaxSmem && B > ner_num_sms() * 64 * 2)
     return launch_bwd_nt<K, 64>(logits, tags, seq_len, trans, alpha_ws, logz, d_ll, scale, d_logits, d_trans, B, L, st);
   return launch_bwd_nt<K, 32>(logits, tags, seq_len, trans, alpha_ws, logz, d_ll, scale, d_logits, d_trans, B, L, st);
 }

@@ -446,6 +446,9 @@ def crf_loglik_bwd(logits, tags, seq_len, trans, alpha, logz, d_ll=None, scale=1
     """-> d_logits [B,L,K], d_trans [K,K] for g_b = (d_ll|1) * scale."""
     require_cuda(logits, tags, seq_len, trans, alpha, logz, d_ll)
     B, L, K = logits.shape
+    assert all(t.dtype == torch.float32 for t in (logits, trans, alpha, logz) + ((d_ll,) if d_ll is not None else ()))
+    assert trans.shape == (K, K) and alpha.shape == (B, L, K) and logz.shape == (B,)
+    assert d_ll is None or d_ll.shape == (B,)
     d_logits = torch.empty_like(logits)
     d_trans = torch.zeros_like(trans)
     check(lib().ner_crf_loglik_bwd(ptr(logits), ptr(_i32(tags)), ptr(_i32(seq_len)), ptr(trans), ptr(alpha), ptr(logz),

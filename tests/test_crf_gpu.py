@@ -8,10 +8,15 @@ import pytest
 import torch
 
 from chinesener_b200 import ops
-from chinesener_b200._lib import VIT_PLANS, lib
+from chinesener_b200._lib import VIT_PLANS, check, lib, ptr, stream
 from oracle import crf
 
+from _crf_grad_oracle import crf_grad_ref
+
 pytestmark = pytest.mark.gpu
+
+# |alpha - ref| <= ALPHA_RTOL |ref| + ALPHA_ATOL at every valid step, and the same for log Z
+ALPHA_RTOL, ALPHA_ATOL = 5e-6, 5e-6
 
 
 def _case(B, L, K, seed, ragged=True, scale=2.0):
@@ -157,6 +162,79 @@ def test_viterbi_large_batch_kernels_bit_exact(B, L, K, aligned, plan):
     tags, best = ops.crf_viterbi(xd, torch.from_numpy(lens).cuda(), torch.from_numpy(tr).cuda(), return_score=True)
     np.testing.assert_array_equal(tags.cpu().numpy(), ref_tags)
     np.testing.assert_array_equal(best.cpu().numpy(), ref_best.astype(np.float32))
+
+
+def fwd_route(B, forced=False):
+    """The kernel ner_crf_loglik_fwd runs for B sequences: the lane-per-tag kernel of crf_small.cu up to
+    NER_CRF_SMALL_B unless flags bit 1 forces the throughput kernel; that one runs 4-step chunks in 64-thread CTAs
+    above 128 sequences per SM and 8-step chunks in 32-thread CTAs below (launch_fwd, crf_loglik.cu:344)."""
+    if B <= 4096 and not forced:
+        return "lanes"
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    return "t4_nt64" if B > 128 * sms else "t8_nt32"
+
+
+def _loglik_fwd_flags(xd, td, ld, trd, flags):
+    """ner_crf_loglik_fwd with raw flags (bit 0: exact path, bit 1: throughput kernel at any B)."""
+    B, L, K = xd.shape
+    ll = torch.empty(B, dtype=torch.float32, device="cuda")
+    logz = torch.empty(B, dtype=torch.float32, device="cuda")
+    alpha = torch.full((B, L, K), float("nan"), dtype=torch.float32, device="cuda")
+    check(lib().ner_crf_loglik_fwd(ptr(xd), ptr(td), ptr(ld), ptr(trd), ptr(ll), ptr(logz), ptr(alpha), B, L, K, flags,
+                                   stream()))
+    return ll, logz, alpha
+
+
+# (B: "big" above 128 sequences per SM, "mid" between NER_CRF_SMALL_B and that, or a small B forced onto the throughput
+# kernel; L, K, mode, logits 16-byte aligned).  mode "wide" spans the transitions over >= 30 nats, "inf" forbids an
+# edge, "flag" asks for the exact path through flags bit 0.
+_FWD_CASES = [
+    ("big", 40, 10, "fast", True), ("big", 37, 7, "inf", True), ("big", 33, 13, "wide", False),
+    ("big", 24, 32, "fast", True), ("big", 30, 13, "fast", False), ("big", 9, 4, "flag", True),
+    ("mid", 40, 10, "fast", True), ("mid", 9, 11, "wide", True), ("mid", 37, 20, "inf", False),
+    ("mid", 17, 4, "fast", True), ("mid", 33, 7, "fast", False), ("mid", 512, 10, "fast", True),
+    (37, 31, 10, "fast", True), (5, 1, 4, "flag", True), (70, 45, 13, "wide", False), (3, 9, 1, "fast", True),
+    (33, 16, 32, "inf", True), (40, 21, 7, "fast", False), (64, 128, 10, "fast", True),
+]
+
+
+@pytest.mark.parametrize("Bs,L,K,mode,aligned", _FWD_CASES)
+def test_loglik_alpha_workspace_throughput_kernels(Bs, L, K, mode, aligned):
+    """alpha at every valid step and log Z of the throughput forward (the alpha the backward consumes) against float64,
+    on both chunkings, fast and exact, vector and scalar staging."""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    B = {"big": 128 * sms + 301, "mid": 5003}.get(Bs, Bs)
+    forced = not isinstance(Bs, str)
+    assert fwd_route(B, forced) == ("t4_nt64" if Bs == "big" else "t8_nt32")
+    gen = torch.Generator().manual_seed(B + L + K)
+    x = torch.randn(B, L, K, generator=gen) * 2
+    tr = torch.randn(K, K, generator=gen)
+    lens = torch.randint(0, L + 1, (B,), generator=gen, dtype=torch.int32)
+    lens[0] = L
+    if B > 2:
+        lens[1], lens[2] = 1, 0
+    tags = torch.randint(0, K, (B, L), generator=gen, dtype=torch.int32)
+    if mode == "wide":
+        tr[0, 1] = tr.max() - 35.0
+    elif mode == "inf":
+        tr[0, 1] = -float("inf")
+    if aligned:
+        xd = x.cuda()
+    else:                                                # the same logits 4 bytes past a 16-byte boundary
+        flat = torch.empty(x.numel() + 1, dtype=torch.float32, device="cuda")
+        xd = flat[1:].view(B, L, K)
+        xd.copy_(x)
+    assert (xd.data_ptr() % 16 == 0) == aligned
+    td, ld, trd = tags.cuda(), lens.cuda(), tr.cuda()
+    flags = 2 * forced + (mode == "flag")
+    _, logz, alpha = _loglik_fwd_flags(xd, td, ld, trd, flags)
+    ref = crf_grad_ref(xd, td, ld, trd)
+    valid = (torch.arange(L, device="cuda")[None, :] < ld[:, None].long())[:, :, None].expand(B, L, K)
+    got, want = alpha.double()[valid], ref.alpha[valid]
+    assert torch.isfinite(got).all()
+    assert ((got - want).abs() <= ALPHA_RTOL * want.abs() + ALPHA_ATOL).all(), \
+        f"alpha error {((got - want).abs() - ALPHA_RTOL * want.abs()).max().item():.3e}"
+    assert ((logz.double() - ref.logz).abs() <= ALPHA_RTOL * ref.logz.abs() + ALPHA_ATOL).all()
 
 
 @pytest.mark.parametrize("B", [19000, 5000])             # 64-thread CTAs with 4-step chunks / 32-thread CTAs
