@@ -1,6 +1,6 @@
 """Stand-alone kernel timings (CUDA events) used while tuning; not the driver's bench.py.
 
-usage: python scripts/bench_kernels.py [crf] [gemm] [--lib OTHER/libner_b200.so]
+usage: python scripts/bench_kernels.py [crf] [gemm] [attn] [wgrad] [--lib OTHER/libner_b200.so]
 """
 import json
 import os
@@ -153,6 +153,70 @@ def bench_gemm(lib_path=None, iters=20):
     return out
 
 
+def _attention_fn(lib_path):
+    """ner_bert_attention (packed mode, inference) of the package's library, or of another build of it (`--lib`)."""
+    import ctypes
+    from chinesener_b200 import _lib
+    if lib_path is None:
+        fn = _lib.lib().ner_bert_attention
+    else:
+        fn = ctypes.CDLL(os.path.abspath(lib_path)).ner_bert_attention
+        fn.restype, fn.argtypes = _lib.SIGNATURES["ner_bert_attention"]
+
+    def call(qkv, cu, ctx, B, L, NH):
+        rc = fn(qkv.data_ptr(), None, ctx.data_ptr(), B, L, NH, 64, 0.125, -10000.0, cu.data_ptr(), qkv.shape[0], 1.0, 0,
+                _lib.stream())
+        if rc != 0:
+            raise RuntimeError(f"{lib_path}: ner_bert_attention returned {rc}")
+        return ctx
+    return call
+
+
+def bench_attention(lib_path=None, rounds=3):
+    """wgmma attention vs the mma.sync kernel at the bench shapes: one MSRA-shaped 64-sentence batch and four stacked.
+    With `lib_path` the same call of that library ("ref") is timed alternately with this one, round by round, and the
+    contexts (written over NaN) are compared byte for byte."""
+    from chinesener_b200 import synthetic
+    import numpy as np
+    libs = {"new": _attention_fn(None)}
+    if lib_path:
+        libs["ref"] = _attention_fn(lib_path)
+    out = {"card": device_card()}
+    NH, D = 12, 64
+    for B in (64, 256):
+        lens = synthetic.msra_lengths(B, 128, np.random.default_rng(1234))
+        T = int(lens.sum())
+        qkv = torch.randn(T, 3 * NH * D, device="cuda").to(torch.bfloat16)
+        cu = torch.tensor([0] + list(np.cumsum(lens)), dtype=torch.int32, device="cuda")
+        ctx = torch.full((T, NH * D), float("nan"), device="cuda", dtype=torch.bfloat16)
+        flops = 4.0 * float((lens.astype(np.float64) ** 2).sum()) * NH * D
+        row = {"tokens": T}
+        outs = {}
+        for tag, fn in libs.items():
+            outs[tag] = fn(qkv, cu, ctx.clone(), B, 128, NH)
+        row["finite"] = bool(torch.isfinite(outs["new"].float()).all())
+        if "ref" in outs:
+            row["bytes_equal_ref"] = bool(torch.equal(outs["new"].view(torch.uint8), outs["ref"].view(torch.uint8)))
+            row["max_abs_diff_ref"] = float((outs["new"].float() - outs["ref"].float()).abs().max())
+        runs = [(tag, fn, None) for tag, fn in libs.items()] + [("mma_sync", libs["new"], "1")]
+        meds = {name: [] for name, _, _ in runs}
+        for _ in range(rounds):
+            for name, fn, var in runs:
+                if var:
+                    os.environ["NER_ATTN_VARIANT"] = var
+                try:
+                    meds[name].append(timeit(lambda: fn(qkv, cu, ctx, B, 128, NH), iters=30)[0] * 1e3)
+                finally:
+                    os.environ.pop("NER_ATTN_VARIANT", None)
+        for name, ts in meds.items():
+            us = min(ts)
+            row[name] = dict(us=round(us, 2), round_us=[round(t, 2) for t in ts], TFLOPs=round(flops / us / 1e6, 1))
+        if "ref" in meds:
+            row["speedup_vs_ref"] = round(row["ref"]["us"] / row["new"]["us"], 2)
+        out[f"B{B}"] = row
+    return out
+
+
 def print_gemm_table(res):
     print(f"# card: {res['card']}")
     tags = [t for t in ("new", "ref") if any(f"{t}_TFLOPs" in r for r in res["rows"].values())]
@@ -178,7 +242,7 @@ def print_gemm_table(res):
 if __name__ == "__main__":
     argv = sys.argv[1:]
     lib_path = None
-    if "--lib" in argv:                 # --lib PATH: time / compare ner_gemm_bf16 of another libner_b200.so as well
+    if "--lib" in argv:                 # --lib PATH: time / compare gemm / attn of another libner_b200.so as well
         i = argv.index("--lib")
         lib_path = argv[i + 1]
         del argv[i:i + 2]
@@ -189,33 +253,9 @@ if __name__ == "__main__":
     if "gemm" in which:
         res["gemm"] = bench_gemm(lib_path)
         print_gemm_table(res["gemm"])
+    if "attn" in which:
+        res["attention"] = bench_attention(lib_path)
     print(json.dumps(res, indent=1))
-
-
-def bench_attention():
-    """wgmma attention vs the mma.sync kernel at the bench shapes: one MSRA-shaped 64-sentence batch and four stacked."""
-    import os
-    from chinesener_b200 import synthetic
-    import numpy as np
-    out = {}
-    NH, D = 12, 64
-    for B in (64, 256):
-        lens = synthetic.msra_lengths(B, 128, np.random.default_rng(1234))
-        T = int(lens.sum())
-        qkv = torch.randn(T, 3 * NH * D, device="cuda").to(torch.bfloat16)
-        cu = torch.tensor([0] + list(np.cumsum(lens)), dtype=torch.int32, device="cuda")
-        for name, var in (("wgmma", None), ("mma_sync", "1")):
-            if var:
-                os.environ["NER_ATTN_VARIANT"] = var
-            med, best = timeit(lambda: ops.bert_attention(qkv, None, B, 128, NH, D, cu_seqlens=cu), iters=30)
-            os.environ.pop("NER_ATTN_VARIANT", None)
-            flops = 4.0 * float((lens.astype(np.float64) ** 2).sum()) * NH * D
-            out[f"{name}_B{B}"] = dict(us=round(med * 1e3, 2), best_us=round(best * 1e3, 2), tokens=T, TFLOPs=round(flops / med / 1e9, 1))
-    return out
-
-
-if __name__ == "__main__" and "attn" in sys.argv[1:]:
-    print(json.dumps({"attention": bench_attention()}, indent=1))
 
 
 def bench_wgrad(rows=3150):
