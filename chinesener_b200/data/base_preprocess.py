@@ -39,7 +39,37 @@ def get_instance(tokenizer_type, max_seq_len, tag2idx, tokenizer, word_enhance=N
     return cls(tokenizer_type, max_seq_len, tag2idx, tokenizer, **kwargs)
 
 
+SPECIAL_TAGS = ('[PAD]', '[CLS]', '[SEP]')
+OPEN_TAG, TAG_SET_SEP = '?', '|'
+
+
+def tag_set_mask(tag, tag2idx):
+    """The allowed-tag bitmask of one partial label: '?' allows every tag a real token may carry (all but [PAD], [CLS]
+    and [SEP]), 'T1|T2|...' the listed tags.  A set naming an unknown or special tag raises ValueError.  Returned as a
+    signed int32 value (bit 31, tag id 31, is the sign bit)."""
+    if tag == OPEN_TAG:
+        ids = [i for t, i in tag2idx.items() if t not in SPECIAL_TAGS]
+    else:
+        names = tag.split(TAG_SET_SEP)
+        bad = [t for t in names if t not in tag2idx or t in SPECIAL_TAGS]
+        if bad:
+            raise ValueError('tag set {!r}: unknown or special tag {}'.format(tag, ', '.join(map(repr, bad))))
+        ids = [tag2idx[t] for t in names]
+    return _bits(ids)
+
+
+def _bits(ids):
+    """tag ids -> the int32 bitmask with those bits set (bit 31 as the sign bit)."""
+    if any(not 0 <= i < 32 for i in ids):
+        raise ValueError('a label_mask holds tag ids below 32 only, got {}'.format(sorted(ids)))
+    m = sum(1 << i for i in set(ids))
+    return m - (1 << 32) if m >= 1 << 31 else m
+
+
 class BasicProc(object):
+    # partial_labels: tags.txt may hold '?' / 'T1|T2|...' entries (build_tag_feature); set by the preprocess CLI
+    partial_labels = False
+
     def __init__(self, tokenizer_type, max_seq_len, tag2idx, tokenizer):
         assert tokenizer_type in (TokenizerBert, TokenizerGiga)
         self.tokenizer_type, self.max_seq_len, self.tag2idx, self.tokenizer = tokenizer_type, max_seq_len, tag2idx, tokenizer
@@ -65,9 +95,22 @@ class BasicProc(object):
         return {'tokens': tokens, 'token_ids': token_ids, 'segment_ids': segment_ids, 'mask': mask, 'seq_len': seq_len}
 
     def build_tag_feature(self, tag):
+        """With partial_labels, an entry of `tag` may be a tag set ('?' or 'T1|T2|...'): it gets label_id -1, and the
+        `label_mask` row holds every position's allowed-tag bitmask (the one-hot bit of its label_id elsewhere, [CLS],
+        [SEP] and [PAD] included)."""
         labels, label_len = self.format_sequence(tag.split(' '))
-        label_ids = [self.tag2idx[i] for i in labels]
-        return {'labels': labels, 'label_ids': label_ids, 'label_len': label_len}
+        if not self.partial_labels:
+            label_ids = [self.tag2idx[i] for i in labels]
+            return {'labels': labels, 'label_ids': label_ids, 'label_len': label_len}
+        label_ids, label_mask = [], []
+        for t in labels:
+            if t == OPEN_TAG or TAG_SET_SEP in t:
+                label_ids.append(-1)
+                label_mask.append(tag_set_mask(t, self.tag2idx))
+            else:
+                label_ids.append(self.tag2idx[t])
+                label_mask.append(_bits([label_ids[-1]]))
+        return {'labels': labels, 'label_ids': label_ids, 'label_mask': label_mask, 'label_len': label_len}
 
     def build_feature(self, sentence, tag):
         f_seq, f_label = self.build_seq_feature(sentence), self.build_tag_feature(tag)
@@ -87,6 +130,8 @@ def features_to_batch(features, pin_memory=False):
     out = {k: torch.tensor([f[k] for f in features], dtype=torch.int32) for k in ('token_ids', 'mask', 'segment_ids')}
     out['seq_len'] = torch.tensor([f['seq_len'] for f in features], dtype=torch.int32)
     out['label_ids'] = torch.tensor([f.get('label_ids', [0] * L) for f in features], dtype=torch.int32)
+    if 'label_mask' in features[0]:     # partially annotated sentences (BasicProc.build_tag_feature)
+        out['label_mask'] = torch.tensor([f['label_mask'] for f in features], dtype=torch.int32)
     # optional per-plugin features (dataset.py:29-36, MultiDataset.add_discriminator :88-90)
     for k in ('softlexicon_ids', 'bichar_ids', 'softword_ids', 'lattice_ids', 'lattice_lens'):
         if k in features[0]:

@@ -10,7 +10,7 @@ TFRecords.
     python -m chinesener_b200.data.preprocess --src <dir with train/ val/ test/> --out datasets/msra \
         --tokenizer giga --giga_vec <gigaword .vec>  [--bert_vocab <vocab.txt>]
         [--word_enhance bichar --bichar_vec <bigram .vec> | --word_enhance ex_softword --word_vec <word .vec>
-         | --word_enhance lattice --word_vec <word .vec> | --word_enhance softword]
+         | --word_enhance lattice --word_vec <word .vec> | --word_enhance softword]  [--partial_labels]
 """
 import argparse
 import os
@@ -79,6 +79,9 @@ def dump_records(proc, src_dir, out_dir, file_name, mapping=MAPPING, word_enhanc
             n_invalid += 1
             if verbose:
                 print(e)
+    if not any(-1 in f['label_ids'] for f in feats if 'label_mask' in f):
+        for f in feats:             # a split without open positions is written exactly as without --partial_labels
+            f.pop('label_mask', None)
     os.makedirs(out_dir, exist_ok=True)
     stem = '_'.join(filter(None, [proc.tokenizer_type, mapping[file_name], word_enhance]))
     write_records(os.path.join(out_dir, stem + '.nerrec'), feats, proc.max_seq_len)
@@ -112,6 +115,9 @@ def main(argv=None):
     ap.add_argument('--word_vec', default='./pretrain_model/ctb50/ctb.50d.vec',
                     help='word vectors (giga .vec format) whose vocabulary is the lexicon of --word_enhance ex_softword / '
                          'lattice (lattice also keeps the vectors as the word table)')
+    ap.add_argument('--partial_labels', action='store_true',
+                    help="tags.txt may leave a token's tag open: '?' (any tag) or a set 'T1|T2|...'; such splits get a "
+                         "label_mask column and label_id -1 at the open positions, for the CRF plugins")
     args = ap.parse_args(argv)
     if args.tokenizer == TokenizerGiga:
         tok = get_giga_tokenizer(args.giga_vec)
@@ -132,6 +138,7 @@ def main(argv=None):
         kwargs['word_embedding'] = lattice_word_embedding(vec, args.seed)
     proc = get_instance(args.tokenizer, args.max_seq_len, MSR_TAG2IDX if msr else MSRA_TAG2IDX, tok,
                         word_enhance=args.word_enhance, **kwargs)
+    proc.partial_labels = args.partial_labels
     for file in (MSR_MAPPING if msr else MAPPING):
         print('Dumping records for {} tokenizer = {}'.format(file, args.tokenizer))
         dump_records(proc, args.src, args.out, file, mapping=MSR_MAPPING if msr else MAPPING, embedding=emb,

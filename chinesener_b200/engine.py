@@ -14,7 +14,7 @@ import torch
 from . import autodiff, variables
 
 _DEVICE_KEYS = ('token_ids', 'mask', 'segment_ids', 'label_ids', 'seq_len', 'softlexicon_ids', 'softlexicon_weights',
-                'bichar_ids', 'softword_ids', 'ex_softword_ids', 'task_ids', 'lattice_ids', 'lattice_lens')
+                'bichar_ids', 'softword_ids', 'ex_softword_ids', 'task_ids', 'lattice_ids', 'lattice_lens', 'label_mask')
 
 
 def load_plugin(model_name):
@@ -55,7 +55,10 @@ class Estimator:
 
     def predict_device(self, dev_features):
         """PREDICT on device-resident features -> pred_ids (device).  One fused C call when the plugin has an
-        executor in fastpath.FUSED_PREDICT (same kernels as build_graph, see fastpath.py), else build_graph."""
+        executor in fastpath.FUSED_PREDICT (same kernels as build_graph, see fastpath.py), else build_graph.  A
+        `label_mask` (partial labels) is dropped: decoding does not read labels."""
+        if 'label_mask' in dev_features:
+            dev_features = {k: v for k, v in dev_features.items() if k != 'label_mask'}
         if self.params.get('fused_predict', True):
             from . import fastpath
             fn = fastpath.FUSED_PREDICT.get(self.model_name)

@@ -9,6 +9,8 @@ evaluation.py:48-55,86-93 prints.
 import pickle
 from collections import defaultdict
 
+import numpy as np
+
 from .tools.predict_utils import process_prediction
 
 
@@ -95,6 +97,10 @@ class SingleEval(object):
             with open(prediction, 'rb') as f:
                 prediction = pickle.load(f)
         self.idx2tag = idx2tag
+        for i in prediction:
+            if (np.asarray(i['label_ids']) < 0).any():
+                raise ValueError('SingleEval needs gold tags at every position; this prediction carries partial labels '
+                                 '(label_id -1 at open positions), whose gold entities are unknown')
         self.prediction = [process_prediction(dict(i), idx2tag) for i in prediction]
         self.verbose = verbose
 

@@ -110,7 +110,7 @@ def predict_to_list(estimator, input_fn):
 
 def singletask_train(args):
     from . import checkpoint, engine
-    from .data.records import NerDataset
+    from .data.records import NerDataset, RecordFile
     model_name = args.rename if args.rename else args.model_name
     model_dir = os.path.join(args.checkpoint_root, 'ner_{}_{}'.format(args.data, model_name))
     data_dir = args.data_dir or './data/{}'.format(args.data)
@@ -152,12 +152,20 @@ def singletask_train(args):
         pickle.dump(prediction, f)
     print('{} sentences -> {}'.format(len(prediction), out_pkl))
 
-    from .evaluation import SingleEval
-    tag_rep, ent_rep = SingleEval(prediction, TRAIN_PARAMS['idx2tag']).gen_report()
-    summary = {'model': model_name, 'data': args.data, 'history': history, 'n_predict': len(prediction), 'seed': args.seed,
-               'entity_micro_f1': ent_rep['micro avg']['f1-score'], 'entity_weighted_f1': ent_rep['weighted avg']['f1-score'],
-               'entity_report': ent_rep, 'tag_weighted_f1': tag_rep['weighted avg']['f1-score']}
-    print('entity micro-F1 = {:.4f}  weighted-F1 = {:.4f}'.format(summary['entity_micro_f1'], summary['entity_weighted_f1']))
+    summary = {'model': model_name, 'data': args.data, 'history': history, 'n_predict': len(prediction), 'seed': args.seed}
+    if 'label_mask' in RecordFile(input_pipe.file_path('predict')).names():
+        # partially labelled: the gold entities are unknown, only the labelled positions (label_id > 0) can be scored
+        real = [(int(a), int(b)) for i in prediction for a, b in zip(i['label_ids'], i['pred_ids']) if a > 0]
+        summary['tag_accuracy'] = sum(a == b for a, b in real) / max(len(real), 1)
+        print('entity report skipped: the predict split is partially labelled, so its gold entities are unknown; '
+              'tag accuracy over the labelled positions = {:.4f}'.format(summary['tag_accuracy']))
+    else:
+        from .evaluation import SingleEval
+        tag_rep, ent_rep = SingleEval(prediction, TRAIN_PARAMS['idx2tag']).gen_report()
+        summary.update({'entity_micro_f1': ent_rep['micro avg']['f1-score'],
+                        'entity_weighted_f1': ent_rep['weighted avg']['f1-score'],
+                        'entity_report': ent_rep, 'tag_weighted_f1': tag_rep['weighted avg']['f1-score']})
+        print('entity micro-F1 = {:.4f}  weighted-F1 = {:.4f}'.format(summary['entity_micro_f1'], summary['entity_weighted_f1']))
     if args.report:
         with open(args.report, 'w') as f:
             json.dump(summary, f, indent=1, default=float)

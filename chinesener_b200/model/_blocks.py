@@ -85,9 +85,19 @@ def segmentation_embedding(features, params, is_training, ids=None, weights=None
 
 
 def crf_head(hidden, features, params, is_training, name='logits'):
-    """Label projection + CRF: -> (mean negative log-likelihood, Viterbi tags)."""
+    """Label projection + CRF: -> (mean negative log-likelihood, Viterbi tags).  A batch with a `label_mask` feature
+    (partially annotated sentences) is trained and evaluated with the partial-annotation CRF loss."""
     n_tags, lengths = params['label_size'], features['seq_len']
     emissions = L.dense(hidden, units=n_tags, name=name, is_training=is_training)
-    transitions, log_lik = L.crf_layer(emissions, features['label_ids'], lengths, n_tags, is_training)
+    transitions, log_lik = L.crf_layer(emissions, features['label_ids'], lengths, n_tags, is_training,
+                                       label_mask=features.get('label_mask'))
     tags = L.crf_decode(emissions, transitions, lengths, params['idx2tag'], is_training)
     return (-log_lik).mean(), tags
+
+
+def refuse_label_mask(features, plugin):
+    """Plugins that read label_ids as complete gold labels cannot train on partially annotated batches: refuse one
+    before anything is launched."""
+    if features.get('label_ids') is not None and features.get('label_mask') is not None:
+        raise ValueError(f"{plugin} cannot use partial labels (a 'label_mask' feature); train it on fully labelled "
+                         f"data, or use a CRF plugin")

@@ -19,6 +19,7 @@ def build_graph(features, labels, params, is_training):
     all task share bert embedding, and has its own bilstm+crf layer
     Equal weight for all task, with lambda weight for discriminator
     """
+    nn.refuse_label_mask(features, 'bert_bilstm_crf_adv')
     input_ids = features['token_ids']
     label_ids = features['label_ids']
     input_mask = features['mask']

@@ -28,6 +28,7 @@ def build_graph(features, labels, params, is_training):
     asymmetry=False, all task share bert embedding, and has its own bilstm+crf tower
     asymmetry=True, task2 is the main task, 2 task share bert embedding, task2 use task 1 hidden state also
     """
+    nn.refuse_label_mask(features, 'bert_bilstm_crf_mtl')
     input_ids = features['token_ids']
     label_ids = features['label_ids']
     input_mask = features['mask']

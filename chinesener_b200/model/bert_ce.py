@@ -14,6 +14,7 @@ from . import _blocks as nn
 
 
 def build_graph(features, labels, params, is_training):
+    nn.refuse_label_mask(features, 'bert_ce')
     hidden = nn.bert_sequence(features, params, is_training, packed=is_training)
     logits = L.dense(hidden, units=params['label_size'], name='logits', is_training=is_training)
     loss = cross_entropy_loss(logits, features.get('label_ids'), features['seq_len'], params['max_seq_len'], is_training)

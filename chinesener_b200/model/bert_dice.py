@@ -11,6 +11,7 @@ from . import _blocks as nn
 
 
 def build_graph(features, labels, params, is_training):
+    nn.refuse_label_mask(features, 'bert_dice')
     hidden = nn.bert_sequence(features, params, is_training, packed=is_training)
     logits = L.dense(hidden, units=params['label_size'], name='logits', is_training=is_training)
     loss = dice_loss(logits, features.get('label_ids'), features['seq_len'], params['max_seq_len'], params['dice_alpha'],

@@ -94,6 +94,7 @@ def span_loss(proj, hi, lo, label_ids, seq_len, type_tag, B, Lq, cu, is_training
 
 
 def build_graph(features, labels, params, is_training):
+    nn.refuse_label_mask(features, 'bert_global_pointer')
     table = mrc.type_table(params)
     check_supported(params, table)
     B, Lq = features['token_ids'].shape

@@ -40,6 +40,7 @@ def sentence_rows(hidden, align, n_pairs, max_seq_len, is_training):
 
 
 def build_graph(features, labels, params, is_training):
+    nn.refuse_label_mask(features, 'bert_mrc')
     table = mrc.device_table(params)
     B, max_seq_len = features['token_ids'].shape
     pairs = ops.mrc_pairs(features['token_ids'], features['seq_len'], table.query_ids, table.query_len, table.type_tag,

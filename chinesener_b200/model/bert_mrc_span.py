@@ -110,6 +110,7 @@ def match_loss(uv, b1, w2, b2, pair_seq_len, span_end, L_sent, keep, is_training
 
 
 def build_graph(features, labels, params, is_training):
+    nn.refuse_label_mask(features, 'bert_mrc_span')
     table = mrc.device_table(params)
     I, keep = check_supported(params, table)
     B, max_seq_len = features['token_ids'].shape

@@ -60,7 +60,8 @@ def build_graph(features, labels, params, is_training):
 
     logits = dense(transformer_output, units=params['label_size'], name='logits', is_training=is_training)
 
-    trans, log_likelihood = crf_layer(logits, label_ids, seq_len, params['label_size'], is_training)
+    trans, log_likelihood = crf_layer(logits, label_ids, seq_len, params['label_size'], is_training,
+                                      label_mask=features.get('label_mask'))
     pred_ids = crf_decode(logits, trans, seq_len, params['idx2tag'], is_training)
     crf_loss = (-log_likelihood).mean()
 

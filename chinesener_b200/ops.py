@@ -456,6 +456,37 @@ def crf_loglik_bwd(logits, tags, seq_len, trans, alpha, logz, d_ll=None, scale=1
     return d_logits, d_trans
 
 
+def crf_partial_loglik_fwd(logits, label_mask, seq_len, trans, want_alpha=False, exact=False):
+    """Partial-annotation CRF log-likelihood (ner_crf_partial_loglik_fwd): label_mask [B,L] int32 bitmasks of the
+    allowed tags. -> ll [B], logz [B,2] (logZ_A, logZ), alpha [2,B,L,K] | None."""
+    require_cuda(logits, label_mask, seq_len, trans)
+    assert logits.dtype == torch.float32 and trans.dtype == torch.float32
+    B, L, K = logits.shape
+    assert trans.shape == (K, K) and label_mask.shape == (B, L)
+    label_mask, seq_len = _i32(label_mask), _i32(seq_len)
+    ll = torch.empty((B,), dtype=torch.float32, device=logits.device)
+    logz = torch.empty((B, 2), dtype=torch.float32, device=logits.device)
+    alpha = torch.empty((2, B, L, K), dtype=torch.float32, device=logits.device) if want_alpha else None
+    check(lib().ner_crf_partial_loglik_fwd(ptr(logits), ptr(label_mask), ptr(seq_len), ptr(trans), ptr(ll), ptr(logz),
+                                           ptr(alpha), B, L, K, 1 if exact else 0, stream()))
+    return ll, logz, alpha
+
+
+def crf_partial_loglik_bwd(logits, label_mask, seq_len, trans, alpha, logz, d_ll=None, scale=1.0):
+    """-> d_logits [B,L,K], d_trans [K,K] of sum_b g_b ll_b, g_b = (d_ll|1) * scale (ner_crf_partial_loglik_bwd)."""
+    require_cuda(logits, label_mask, seq_len, trans, alpha, logz, d_ll)
+    B, L, K = logits.shape
+    assert all(t.dtype == torch.float32 for t in (logits, trans, alpha, logz) + ((d_ll,) if d_ll is not None else ()))
+    assert trans.shape == (K, K) and alpha.shape == (2, B, L, K) and logz.shape == (B, 2)
+    assert label_mask.shape == (B, L) and (d_ll is None or d_ll.shape == (B,))
+    d_logits = torch.empty_like(logits)
+    d_trans = torch.zeros_like(trans)
+    check(lib().ner_crf_partial_loglik_bwd(ptr(logits), ptr(_i32(label_mask)), ptr(_i32(seq_len)), ptr(trans),
+                                           ptr(alpha), ptr(logz), ptr(d_ll), scale, ptr(d_logits), ptr(d_trans),
+                                           B, L, K, stream()))
+    return d_logits, d_trans
+
+
 # --------------------------------------------------------------------------- fp32-accurate dense (split bf16)
 def split_bf16(x2d, Dp=None):
     """f32 [M,D] -> (hi, lo) bf16 [M,Dp] with hi + lo ~= x to 2^-17."""

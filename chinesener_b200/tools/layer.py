@@ -581,29 +581,36 @@ def dense(inputs, units, name='logits', is_training=False):
     return out.view(*lead, units)
 
 
-def crf_layer(logits, label_ids, seq_len, label_size, is_training):
-    """reference tools/layer.py:112-131 -> (trans, log_likelihood [B])."""
+def crf_layer(logits, label_ids, seq_len, label_size, is_training, label_mask=None):
+    """reference tools/layer.py:112-131 -> (trans, log_likelihood [B]).
+
+    label_mask [B, L] int32 (partially annotated batches): bit j of label_mask[b, t] allows tag j at t, and the
+    log-likelihood is that of the partial-annotation CRF (ner_crf_partial_loglik_fwd); label_ids is then not read."""
     tname = variables.scoped("crf_layer/transitions")
     trans = variables.get_variable(tname, (label_size, label_size), variables.xavier)
     if label_ids is None:
         return trans, None
+    if label_mask is None:
+        fwd, bwd_op, labels = ops.crf_loglik_fwd, ops.crf_loglik_bwd, label_ids
+    else:
+        fwd, bwd_op, labels = ops.crf_partial_loglik_fwd, ops.crf_partial_loglik_bwd, label_mask
     tape = autodiff.current()
     if is_training and tape is not None:
         store = variables.default_store()
         lg = logits.contiguous()
-        ll, logz, alpha = ops.crf_loglik_fwd(lg, label_ids, seq_len, trans, want_alpha=True)
+        ll, logz, alpha = fwd(lg, labels, seq_len, trans, want_alpha=True)
 
         def bwd(g):
             # g = d loss / d ll  [B]; the plugins use loss = mean(-ll)  ->  g = -1/B
             B = lg.shape[0]
             d_ll = g if g is not None else torch.full((B,), -1.0 / B, dtype=torch.float32, device=lg.device)
-            d_logits, d_trans = ops.crf_loglik_bwd(lg, label_ids, seq_len, trans, alpha, logz, d_ll.contiguous(), 1.0)
+            d_logits, d_trans = bwd_op(lg, labels, seq_len, trans, alpha, logz, d_ll.contiguous(), 1.0)
             store.grad(tname).add_(d_trans)
             tape.add_grad(logits, d_logits)
         tape.record(ll, bwd)
         return trans, ll
     # EVAL / PREDICT: built lazily — evaluated when the loss is fetched (EVAL), never in PREDICT
-    return trans, variables.Deferred(lambda: ops.crf_loglik_fwd(logits, label_ids, seq_len, trans)[0])
+    return trans, variables.Deferred(lambda: fwd(logits, labels, seq_len, trans)[0])
 
 
 def concat(tensors, is_training=False):

@@ -91,6 +91,27 @@ int ner_crf_loglik_bwd(const float* logits, const int32_t* tags, const int32_t* 
                        const float* d_ll, float scale, float* d_logits, float* d_trans, int B,
                        int L, int K, ner_stream_t stream);
 
+/* Partial-annotation CRF (Tsuboi et al., COLING 2008) in place of tools/layer.py:122-127's crf_log_likelihood when
+ * the gold path is only known as a set of allowed tags per position.  label_mask [B,L] i32: bit j of label_mask[b,t]
+ * allows tag j at t (bits >= K ignored, t >= seq_len ignored).
+ *   ll[b] = logZ_A - logZ,  logZ_A = log-sum over the paths inside the allowed sets of exp(score)
+ * A one-hot mask gives ner_crf_loglik_fwd's ll; a row whose every position allows all K tags gives exactly 0.0; an
+ * empty set at some t < seq_len gives -inf; seq_len <= 0 gives 0.
+ * logz: NULL or [B,2] f32 (logZ_A, logZ).  alpha_ws: NULL or [2,B,L,K] f32 (alpha_A, alpha) for the backward.
+ * flags: bit0 = force the exact (per-column max) logsumexp path. */
+int ner_crf_partial_loglik_fwd(const float* logits, const int32_t* label_mask, const int32_t* seq_len,
+                               const float* trans, float* ll, float* logz, float* alpha_ws, int B, int L, int K,
+                               int flags, ner_stream_t stream);
+
+/* Gradient of ner_crf_partial_loglik_fwd's ll, for g_b = (d_ll ? d_ll[b] : 1) * scale:
+ *   d_logits[b,t,j] = g_b * (P_A(y_t=j) - P(y_t=j))                  (0 beyond seq_len, 0 for a row with ll = -inf)
+ *   d_trans[i,j]   += sum_b g_b * sum_t (P_A(y_{t-1}=i,y_t=j) - P(y_{t-1}=i,y_t=j))
+ * alpha_ws [2,B,L,K] and logz [B,2] come from ner_crf_partial_loglik_fwd.  d_logits is fully written, d_trans is
+ * accumulated into, as for ner_crf_loglik_bwd. */
+int ner_crf_partial_loglik_bwd(const float* logits, const int32_t* label_mask, const int32_t* seq_len,
+                               const float* trans, const float* alpha_ws, const float* logz, const float* d_ll,
+                               float scale, float* d_logits, float* d_trans, int B, int L, int K, ner_stream_t stream);
+
 
 /* ------------------------------------------------------------------------ *
  * Dense layers on wgmma tensor cores — replaces tf.layers.dense /
