@@ -9,12 +9,26 @@ to the device inside `predict` — that copy is part of the end-to-end number be
 import contextlib
 import importlib
 
+import numpy as np
 import torch
 
 from . import autodiff, variables
 
 _DEVICE_KEYS = ('token_ids', 'mask', 'segment_ids', 'label_ids', 'seq_len', 'softlexicon_ids', 'softlexicon_weights',
                 'bichar_ids', 'softword_ids', 'ex_softword_ids', 'task_ids', 'lattice_ids', 'lattice_lens', 'label_mask')
+
+
+# Plugins that refuse params['crf_nbest'] > 1, with the reason (checked by Estimator.crf_nbest before anything is launched)
+NBEST_REFUSED = {
+    'bert_ce': "it has no CRF: its tags are a per-token argmax",
+    'bert_dice': "it has no CRF: its tags are a per-token argmax",
+    'bert_mrc': "it has no CRF: its tags come from per-type span pointers",
+    'bert_mrc_span': "it has no CRF: its tags come from span scores",
+    'bert_global_pointer': "it has no CRF: its tags come from span scores",
+    'bert_bilstm_crf_mtl': "its pred_ids are a per-task selection of several CRF decodes",
+    'bert_bilstm_crf_adv': "its pred_ids are a per-task selection of several CRF decodes",
+}
+NBEST_MAX = 16
 
 
 def load_plugin(model_name):
@@ -59,6 +73,7 @@ class Estimator:
         `label_mask` (partial labels) is dropped: decoding does not read labels."""
         if 'label_mask' in dev_features:
             dev_features = {k: v for k, v in dev_features.items() if k != 'label_mask'}
+        self.crf_nbest()
         if self.params.get('fused_predict', True):
             from . import fastpath
             fn = fastpath.FUSED_PREDICT.get(self.model_name)
@@ -78,17 +93,29 @@ class Estimator:
         max_pos = bert.load_bert_config(self.params.get('pretrain_dir', ''))["max_position_embeddings"]
         return windows.settings(self.params.get('bert_window'), self.params.get('bert_window_stride'), max_pos)
 
+    def crf_nbest(self):
+        """params['crf_nbest'] (default 1): how many best CRF paths PREDICT / EVAL decode.  ValueError outside
+        1..NBEST_MAX, or above 1 for a plugin in NBEST_REFUSED."""
+        n = self.params.get('crf_nbest', 1)
+        if isinstance(n, bool) or not isinstance(n, (int, np.integer)) or not 1 <= n <= NBEST_MAX:
+            raise ValueError(f"crf_nbest must be an integer in 1..{NBEST_MAX} (got {n!r})")
+        if n > 1 and self.model_name in NBEST_REFUSED:
+            raise ValueError(f"{self.model_name} cannot decode crf_nbest = {n} paths: {NBEST_REFUSED[self.model_name]}")
+        return int(n)
+
     @contextlib.contextmanager
     def _layer_settings(self, dev_features):
         """The module settings of tools/layer.py this Estimator's params select, checked before anything is launched."""
         from . import windows
         from .tools import layer
+        nbest = self.crf_nbest()
         ws = self.document_window()
         if ws is not None and torch.is_tensor(dev_features.get('token_ids')):
             windows.check_batch(self.model_name, dev_features['token_ids'].shape[1], ws[0])
-        keys = ('BERT_PRECISION', 'BERT_WINDOW', 'BERT_WINDOW_STRIDE', 'DOCUMENT_REFUSAL')
+        keys = ('BERT_PRECISION', 'BERT_WINDOW', 'BERT_WINDOW_STRIDE', 'DOCUMENT_REFUSAL', 'CRF_NBEST')
         saved = {k: getattr(layer, k) for k in keys}
         layer.BERT_PRECISION = self.params.get('bert_precision', saved['BERT_PRECISION'])
+        layer.CRF_NBEST = nbest
         if ws is not None:
             layer.BERT_WINDOW, layer.BERT_WINDOW_STRIDE = ws
             if self.model_name in windows.REFUSED:
@@ -106,14 +133,19 @@ class Estimator:
 
     def predict(self, features):
         """PREDICT mode on one host batch -> dict(pred_ids int32 [B,L] on host, label_ids, tokens), and 'pred_spans' (per
-        sentence a list of (type name, start, end_exclusive, probability)) when the plugin's pred_ids carries spans."""
+        sentence a list of (type name, start, end_exclusive, probability)) when the plugin's pred_ids carries spans, and
+        'pred_nbest' (per sentence a list of (tags int32 [L], score, probability), best first, empty for seq_len <= 0) when
+        params['crf_nbest'] > 1."""
         dev = self.to_device(features)
         pred_ids = self.predict_device(dev)
         out = {'pred_ids': pred_ids.cpu(), 'label_ids': features.get('label_ids'), 'tokens': features.get('tokens')}
-        from .tools.infer_utils import span_lists
+        from .tools.infer_utils import nbest_lists, span_lists
         spans = span_lists(pred_ids)
         if spans is not None:
             out['pred_spans'] = spans
+        nbest = nbest_lists(pred_ids, features['seq_len']) if 'seq_len' in features else None
+        if nbest is not None:
+            out['pred_nbest'] = nbest
         return out
 
     def stack_to_device(self, feature_list):

@@ -33,6 +33,8 @@ def bert_bilstm_crf_predict(est, dev):
         return None
     if params.get('cell_type', 'lstm').lower() != 'lstm' or params.get('cell_size', 1) != 1:
         return None
+    if params.get('crf_nbest', 1) > 1:
+        return None                                    # N-best decoding: build_graph's crf_decode attaches the paths
     if dev['token_ids'].shape[1] > est.document_window()[0]:
         return None                                    # document mode: build_graph stitches the windows
     Hl, K = params['hidden_units_list'][0], params['label_size']

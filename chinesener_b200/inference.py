@@ -51,6 +51,24 @@ class InferHelper(object):
             return span_entities([feature['tokens']], out['pred_spans'])[0]
         return self.decode_prediction(out['pred_ids'].numpy())
 
+    def infer_nbest(self, text):
+        """The estimator's params['crf_nbest'] best CRF paths of one sentence -> a list of (entity dict, probability), best
+        first, one entry per path; the first entity dict is infer(text).  Entries are not merged: two paths that give the
+        same entities (for example paths that differ only at [CLS] / [SEP]) are two entries, each with its own
+        probability exp(score - log Z)."""
+        import torch
+        from .tools.infer_utils import extract_entity_device
+        feature = self.make_feature(text)
+        out = self.estimator.predict(features_to_batch([feature]))
+        if 'pred_nbest' not in out:
+            raise ValueError(f"infer_nbest needs a CRF plugin run with params['crf_nbest'] > 1 ({self.model_name})")
+        paths = out['pred_nbest'][0]
+        if not paths:
+            return []
+        rows = torch.from_numpy(np.stack([p[0] for p in paths])).to(self.estimator.device)
+        ents = extract_entity_device([feature['tokens']] * len(paths), rows, self.idx2tag)
+        return [(e, p[2]) for e, p in zip(ents, paths)]
+
     def infer_batch(self, texts):
         """Many sentences per call: one PREDICT batch, the tag scan of extract_entity on the GPU (ner_extract_spans) —
         the tag tensor stays on the device, only the spans come back.  -> one entity dict per text, as infer() gives.

@@ -108,6 +108,37 @@ def predict_to_list(estimator, input_fn):
     return out
 
 
+def predict_nbest_to_list(estimator, input_fn):
+    """predict_to_list with params['crf_nbest'] > 1, batch by batch through Estimator.predict: each sentence's dict also
+    holds its candidate paths, best first, as nbest_ids int32 [count, L], nbest_scores f32 [count] and nbest_probs f32
+    [count].  -> (that list, seq_len of every sentence)."""
+    out, lens = [], []
+    for feats in input_fn():
+        res = estimator.predict(feats)
+        pred, lab, tok = res['pred_ids'].numpy(), feats['label_ids'].numpy(), feats['tokens']
+        L = pred.shape[1]
+        lens.extend(int(n) for n in feats['seq_len'])
+        for b, paths in enumerate(res['pred_nbest']):
+            out.append({'pred_ids': pred[b].astype(np.int32), 'label_ids': lab[b].astype(np.int32),
+                        'tokens': np.array([t.encode('utf-8') if isinstance(t, str) else t for t in tok[b]], dtype=object),
+                        'nbest_ids': np.array([p[0] for p in paths], dtype=np.int32).reshape(len(paths), L),
+                        'nbest_scores': np.array([p[1] for p in paths], dtype=np.float32),
+                        'nbest_probs': np.array([p[2] for p in paths], dtype=np.float32)})
+    return out, lens
+
+
+def exact_match_rates(prediction, lens):
+    """-> (exact_match_at_1, exact_match_at_n): the share of sentences whose gold label_ids over t < seq_len equal the
+    best candidate path / one of the candidate paths."""
+    at1 = atn = 0
+    for p, n in zip(prediction, lens):
+        hits = [np.array_equal(c[:n], p['label_ids'][:n]) for c in p['nbest_ids']] if n > 0 else []
+        at1 += bool(hits and hits[0])
+        atn += any(hits)
+    total = max(len(prediction), 1)
+    return at1 / total, atn / total
+
+
 def singletask_train(args):
     from . import checkpoint, engine
     from .data.records import NerDataset, RecordFile
@@ -126,6 +157,8 @@ def singletask_train(args):
     if args.batch_size:
         TRAIN_PARAMS['batch_size'] = args.batch_size
     _window_params(TRAIN_PARAMS, args)
+    if args.crf_nbest != 1:
+        TRAIN_PARAMS['crf_nbest'] = args.crf_nbest
     input_pipe = NerDataset(data_dir, TRAIN_PARAMS['batch_size'], TRAIN_PARAMS['epoch_size'], model_name, seed=args.seed)
     TRAIN_PARAMS.update(input_pipe.params)       # label_size, max_seq_len, num_train_steps ... (main.py:25)
     print('=' * 10 + 'TRAIN PARAMS' + '=' * 10)
@@ -134,6 +167,7 @@ def singletask_train(args):
     print(RUN_CONFIG)
 
     estimator = engine.Estimator(args.model_name, TRAIN_PARAMS)
+    nbest = estimator.crf_nbest()                # ValueError before training: out of range, or a plugin without one CRF
     estimator.store.gen.manual_seed(args.seed)
     warm = checkpoint.latest_checkpoint(model_dir)
     if warm:
@@ -146,13 +180,21 @@ def singletask_train(args):
     if not args.predict_only:
         history = train_and_evaluate(estimator, input_pipe, model_dir, max_steps=args.max_steps)
 
-    prediction = predict_to_list(estimator, input_pipe.build_input_fn('predict', is_predict=True))
+    if nbest > 1:
+        prediction, lens = predict_nbest_to_list(estimator, input_pipe.build_input_fn('predict', is_predict=True))
+    else:
+        prediction = predict_to_list(estimator, input_pipe.build_input_fn('predict', is_predict=True))
     out_pkl = os.path.join(data_dir, '{}_predict.pkl'.format(model_name))
     with open(out_pkl, 'wb') as f:
         pickle.dump(prediction, f)
     print('{} sentences -> {}'.format(len(prediction), out_pkl))
 
     summary = {'model': model_name, 'data': args.data, 'history': history, 'n_predict': len(prediction), 'seed': args.seed}
+    if nbest > 1:
+        summary['crf_nbest'] = nbest
+        summary['exact_match_at_1'], summary['exact_match_at_n'] = exact_match_rates(prediction, lens)
+        print('exact match of the gold tags: {:.4f} at 1, {:.4f} within {} paths'.format(
+            summary['exact_match_at_1'], summary['exact_match_at_n'], nbest))
     if 'label_mask' in RecordFile(input_pipe.file_path('predict')).names():
         # partially labelled: the gold entities are unknown, only the labelled positions (label_id > 0) can be scored
         real = [(int(a), int(b)) for i in prediction for a, b in zip(i['label_ids'], i['pred_ids']) if a > 0]
@@ -181,6 +223,9 @@ def multitask_train(args):
     model_name = args.rename if args.rename else args.model_name
     data_list = args.data.split(',')
     joined = '_'.join(data_list)
+    if args.crf_nbest != 1:
+        raise ValueError('--crf_nbest is for single-task plugins: the multi-task pred_ids are a per-task selection of '
+                         'several CRF decodes')
     model_dir = os.path.join(args.checkpoint_root, 'ner_{}_{}'.format(joined, model_name))
     data_root = args.data_dir or './data'
     if args.clear_model:
@@ -258,6 +303,9 @@ def build_parser():
                         'longer batches as overlapping windows of this many tokens (default max_position_embeddings)')
     parser.add_argument('--bert_window_stride', type=int, default=0, help='override params["bert_window_stride"]: content '
                         'tokens between window starts (default (bert_window - 2) // 2)')
+    parser.add_argument('--crf_nbest', type=int, default=1, help='CRF plugins: decode the N best tag paths (1..16) at '
+                        'PREDICT; the pickle gains nbest_ids / nbest_scores / nbest_probs and the summary exact_match_at_1 / '
+                        'exact_match_at_n')
     return parser
 
 

@@ -36,6 +36,29 @@ def crf_viterbi(logits, seq_len, trans, return_score=False):
     return (tags, score) if return_score else tags
 
 
+NBEST_MAX = 16                                   # largest n of crf_viterbi_nbest
+
+
+def crf_viterbi_nbest(logits, seq_len, trans, n):
+    """N-best tf.contrib.crf.crf_decode (ner_crf_viterbi_nbest) -> (tags [B,n,L] int32, scores [B,n] f32, counts [B]
+    int32).  Rank 0 is crf_viterbi's path and best_score; ranks past counts[b] are zero tags with score -inf."""
+    require_cuda(logits, seq_len, trans)
+    assert logits.dtype == torch.float32 and trans.dtype == torch.float32
+    B, L, K = logits.shape
+    assert trans.shape == (K, K)
+    n = int(n)
+    seq_len = _i32(seq_len)
+    dev = logits.device
+    tags = torch.empty((B, n, L), dtype=torch.int32, device=dev)
+    scores = torch.empty((B, n), dtype=torch.float32, device=dev)
+    counts = torch.zeros((B,), dtype=torch.int32, device=dev)
+    nbytes = int(lib().ner_crf_viterbi_nbest_workspace_bytes(B, L, K, n))
+    ws = torch.empty((max(nbytes, 16),), dtype=torch.uint8, device=dev)
+    check(lib().ner_crf_viterbi_nbest(ptr(logits), ptr(seq_len), ptr(trans), n, ptr(tags), ptr(scores), ptr(counts),
+                                      ptr(ws), nbytes, B, L, K, stream()))
+    return tags, scores, counts
+
+
 def crf_loglik_fwd(logits, tags, seq_len, trans, want_alpha=False, exact=False):
     """tf.contrib.crf.crf_log_likelihood forward (reference tools/layer.py:122). -> ll [B], logz [B], alpha|None."""
     require_cuda(logits, tags, seq_len, trans)

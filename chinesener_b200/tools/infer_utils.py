@@ -2,6 +2,8 @@
 (`extract_entity`, `fix_tokens`), which `inference.InferHelper.infer` applies to the PREDICT output."""
 from collections import defaultdict
 
+import numpy as np
+
 _SPECIAL_TOKENS = frozenset(('[PAD]', '[CLS]', '[SEP]'))
 
 
@@ -49,6 +51,24 @@ def fix_tokens(sentence, tokens):
             tok = tokens[k] = tok.replace('##', '')
         cursor += len(tok)
     return tokens
+
+
+def nbest_lists(pred_ids, seq_len):
+    """The N best paths a CRF plugin attaches to its device pred_ids when params['crf_nbest'] > 1 (tools/layer.py
+    crf_decode) -> per sentence a list of (tags int32 [L], score, probability), best first, counts[b] long (empty for
+    seq_len <= 0); probability = exp(score - log Z).  None when pred_ids carries no N-best paths."""
+    ids = getattr(pred_ids, 'nbest_ids', None)
+    if ids is None:
+        return None
+    ids, scores = ids.cpu().numpy(), pred_ids.nbest_scores.cpu().numpy()
+    counts, logz = pred_ids.nbest_counts.cpu().numpy(), pred_ids.nbest_logz.cpu().numpy()
+    lens = np.asarray(seq_len.cpu() if hasattr(seq_len, 'cpu') else seq_len).reshape(-1)
+    out = []
+    for b in range(ids.shape[0]):
+        c = int(counts[b]) if lens[b] > 0 else 0
+        probs = np.exp(scores[b, :c].astype(np.float64) - float(logz[b]))
+        out.append([(ids[b, r], float(scores[b, r]), float(probs[r])) for r in range(c)])
+    return out
 
 
 def span_lists(pred_ids):

@@ -28,6 +28,9 @@ BERT_PRECISION = os.environ.get("NER_B200_BERT_PRECISION", "bf16")
 BERT_WINDOW = None
 BERT_WINDOW_STRIDE = None
 DOCUMENT_REFUSAL = None
+# N-best decoding: with CRF_NBEST > 1, crf_decode outside TRAIN also returns the CRF_NBEST best paths (as attributes of
+# pred_ids, whose values stay the Viterbi path).  Estimator sets it from params['crf_nbest'] around build_graph.
+CRF_NBEST = 1
 
 
 class TrainingPathNotBuilt(NotImplementedError):
@@ -676,5 +679,15 @@ def masked_task_loss(log_likelihoods, masks, weights, batch_size, is_training):
 
 
 def crf_decode(logits, trans, seq_len, idx2tag, is_training, mask=None):
-    """reference tools/layer.py:134-149 -> pred_ids [B,L] int32, zero beyond seq_len."""
-    return ops.crf_viterbi(logits, seq_len, trans)
+    """reference tools/layer.py:134-149 -> pred_ids [B,L] int32, zero beyond seq_len.
+
+    CRF_NBEST > 1 (PREDICT / EVAL): pred_ids is rank 0 of ops.crf_viterbi_nbest, the same tags, and carries the
+    CRF_NBEST best paths as .nbest_ids [B,N,L] int32, .nbest_scores [B,N] f32, .nbest_counts [B] int32 and .nbest_logz
+    [B] f32 (log Z of ner_crf_loglik_fwd), so that path r has probability exp(nbest_scores[:, r] - nbest_logz)."""
+    if CRF_NBEST <= 1 or is_training:
+        return ops.crf_viterbi(logits, seq_len, trans)
+    tags, scores, counts = ops.crf_viterbi_nbest(logits, seq_len, trans, CRF_NBEST)
+    pred = tags[:, 0].contiguous()
+    logz = ops.crf_loglik_fwd(logits, pred, seq_len, trans)[1]
+    pred.nbest_ids, pred.nbest_scores, pred.nbest_counts, pred.nbest_logz = tags, scores, counts, logz
+    return pred

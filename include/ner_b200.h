@@ -112,6 +112,24 @@ int ner_crf_partial_loglik_bwd(const float* logits, const int32_t* label_mask, c
                                const float* trans, const float* alpha_ws, const float* logz, const float* d_ll,
                                float scale, float* d_logits, float* d_trans, int B, int L, int K, ner_stream_t stream);
 
+/* N-best extension of tools/layer.py:140-142's tf.contrib.crf.crf_decode: the N highest-scoring tag paths of every
+ * sequence, best first (list Viterbi, csrc/crf_nbest.cu).  Row b decodes n = min(max(seq_len[b], 1), L) positions, as
+ * ner_crf_viterbi does.  A path's score is the fp32 left-to-right sum s_0 = x[0][y_0],
+ * s_t = (s_{t-1} + trans[y_{t-1}][y_t]) + x[t][y_t].  Ties: at each step the candidates (predecessor i, its rank r) are
+ * ordered by s + trans descending, then lower i, then lower r; the final lists by score, then lower last tag, then
+ * lower rank.  So rank 0 is ner_crf_viterbi's path and best_score bit for bit, and the N scores are the N largest
+ * path scores.
+ *   tags_out [B,N,L] i32: rank r of row b at tags_out[(b*N + r)*L ...], zero past n and in empty ranks;
+ *   scores_out [B,N] f32: -inf in empty ranks;  count_out [B] i32 or NULL: min(N, K^n), the ranks filled.
+ * workspace: backpointers, at least ner_crf_viterbi_nbest_workspace_bytes(B, L, K, N) = B*L*K*N*2 bytes (0 for B = 0).
+ * Returns NER_ERR_UNSUPPORTED outside 1 <= K <= 32, 1 <= N <= 16; NER_ERR_INVALID_ARG for B < 0, L < 1 or a null
+ * logits / seq_len / trans / tags_out / scores_out; NER_ERR_WORKSPACE for a missing or short workspace; B = 0 is a
+ * no-op.  All checked before any CUDA call. */
+size_t ner_crf_viterbi_nbest_workspace_bytes(int B, int L, int K, int N);
+int ner_crf_viterbi_nbest(const float* logits, const int32_t* seq_len, const float* trans, int N, int32_t* tags_out,
+                          float* scores_out, int32_t* count_out, void* workspace, size_t workspace_bytes, int B, int L,
+                          int K, ner_stream_t stream);
+
 
 /* ------------------------------------------------------------------------ *
  * Dense layers on wgmma tensor cores — replaces tf.layers.dense /
