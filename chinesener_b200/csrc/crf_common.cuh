@@ -1,12 +1,17 @@
-// Shared pieces of the CRF dynamic-programming kernels (Viterbi, forward-alpha, backward).
+// Shared pieces of the CRF dynamic-programming kernels (Viterbi, forward-alpha, backward), and the device code of the
+// two CRF losses: the ordinary one (crf_loglik.cu, crf_bwd.cu, the loss kernels of crf_small.cu) and the
+// partial-annotation one (crf_partial.cu).  Each loss kernel keeps its own loop body; the staging, the recursion
+// steps, the prologues, the stores and the shared-memory sizes below are the one implementation both use.
 //
-// Work decomposition (all three kernels): ONE THREAD PER SEQUENCE, NT sequences per CTA.
+// Work decomposition of the throughput kernels: ONE THREAD PER SEQUENCE, NT sequences per CTA.
 // The K-wide DP state lives in registers; emission logits are streamed HBM -> smem with
 // cp.async in chunks of T=8 time steps per sequence (coalesced 16-byte requests over the
 // CTA's contiguous [NT, L*K] slab), then each thread reads its own row back with LDS.128.
 // Row pitch P = 8K+4 floats makes P/4 odd, so the 8 threads of a quarter-warp hit 8
 // distinct 16-byte bank groups (conflict-free).
 #pragma once
+#include <cfloat>
+
 #include "common.cuh"
 
 namespace crf {
@@ -15,6 +20,10 @@ using namespace nerdev;
 
 constexpr int T_CHUNK = 8;  // time steps staged per chunk
 constexpr int NSTAGE = 2;   // cp.async ring depth
+constexpr int LABP = 12;    // pitch (ints) of a row's staged labels: 3 x 16B, odd -> conflict-free LDS.128
+
+constexpr float kLog2e = 1.4426950408889634f;
+constexpr float kLn2 = 0.6931471805599453f;
 
 template <int K, int TT = T_CHUNK>
 struct Geom {
@@ -26,6 +35,7 @@ struct Geom {
   static constexpr int GQ = G * K / 4;                                // float4 per step group
   static constexpr bool UNROLL = (K <= 12);                           // registers vs local arrays
   static constexpr int KK4 = (K * K + 3) & ~3;
+  static constexpr bool ACC_REGS = (K <= 10);  // backward: the K*K pair-marginal accumulators fit in registers
 };
 
 // Stage chunk `c` (time steps [t0, t0+T)) of the CTA's rows into dst[NT][P].
@@ -72,6 +82,26 @@ __device__ __forceinline__ void stage_logits(float* dst, const float* __restrict
         const int rem = min(ne, (s_len[r] - t0) * K);
         if (e < rem) cp_async4(dst + r * Gm::P + e, gbase + (size_t)r * LK + (size_t)t0 * K + e);
       }
+    }
+  }
+}
+
+// Stage chunk [t0, t0+TT) of the CTA's int32 label rows (gold tags, or allowed-tag masks) into dst[NT][LABP]; steps at
+// t >= s_len[r] are not fetched.
+template <int NT, int TT = T_CHUNK>
+__device__ __forceinline__ void stage_labels(int* dst, const int32_t* __restrict__ gbase, int L, int t0, int nv,
+                                             const int* s_len, int vec16) {
+  const int steps = min(TT, L - t0);
+  if (vec16) {
+    for (int idx = threadIdx.x; idx < NT * (TT / 4); idx += NT) {
+      const int r = idx / (TT / 4), q = idx - r * (TT / 4);
+      if (r < nv && 4 * q < min(steps, s_len[r] - t0))
+        cp_async16(dst + r * LABP + 4 * q, gbase + (size_t)r * L + t0 + 4 * q);
+    }
+  } else {
+    for (int idx = threadIdx.x; idx < NT * TT; idx += NT) {
+      const int r = idx / TT, e = idx - r * TT;
+      if (r < nv && e < min(steps, s_len[r] - t0)) cp_async4(dst + r * LABP + e, gbase + (size_t)r * L + t0 + e);
     }
   }
 }
@@ -145,12 +175,364 @@ __device__ __forceinline__ void store_tags_coalesced(int32_t* obase, int nv, int
   }
 }
 
-// Lane-per-tag kernels (crf_small.cu): a group of GS lanes holds the K-wide state of one sequence.
+// Can the scaled-probability (fast) path run on this transition matrix?  Only when its entries span < 30 nats and are
+// finite (a NaN fails every test).  hi gets the largest entry.
+__device__ __forceinline__ bool trans_is_narrow(const float* s_tr, int KK, float& hi) {
+  float lo = INFINITY;
+  hi = -INFINITY;
+  for (int e = 0; e < KK; ++e) {
+    lo = fminf(lo, s_tr[e]);
+    hi = fmaxf(hi, s_tr[e]);
+  }
+  return (hi - lo < 30.f) && (fabsf(hi) < 1e30f) && (fabsf(lo) < 1e30f);
+}
+
+// ------------------------------------------------------------------------------- loss forward, thread per sequence
+// State of one recursion: alpha_j = lacc + ln a[j] with a[] in the probability domain (fast path), or a[j] = alpha_j
+// (exact path).  Fast path, per step:
+//     a_t[j] = (sum_i a_{t-1}[i] * E[i][j]) * exp(x_t[j] - xm_t),   E = exp(trans - tmax),   lacc += xm_t + tmax
+// i.e. K*K FFMA + K ex2 instead of K*K exp and K log; renormalising a to max 1 adds one rcp and one lg2.
+
+// Shared memory of the thread-per-sequence forwards: trans, E, row lengths, and a ring of logit and label chunks.
+template <int K, int NT, int TT>
+constexpr size_t fwd_smem_bytes() {
+  using Gm = Geom<K, TT>;
+  return 4 * (2 * (size_t)Gm::KK4 + NT + (size_t)NSTAGE * NT * Gm::P + (size_t)NSTAGE * NT * LABP);
+}
+
+// max of x[0..K), in max3 steps
+template <int K>
+__device__ __forceinline__ float row_max(const float* x) {
+  constexpr int UNR = Geom<K>::UNROLL ? K : 1;
+  float m = x[0];
+  if (K > 1) {
+#pragma unroll UNR
+    for (int j = 1; j + 1 < K; j += 2) m = max3(m, x[j], x[j + 1]);
+    if (K % 2 == 0) m = fmaxf(m, x[K - 1]);
+  }
+  return m;
+}
+
+// E[i][2q], E[i][2q+1] (0 for the pad column of an odd K): from the packed registers E2[K][(K+1)/2], or from s_E.
+template <int K, bool EREG>
+__device__ __forceinline__ f32x2 e_pair(const f32x2* E2, const float* s_E, int i, int q) {
+  if (EREG) return E2[i * ((K + 1) / 2) + q];
+  return pk2(s_E[i * K + 2 * q], 2 * q + 1 < K ? s_E[i * K + 2 * q + 1] : 0.f);
+}
+
+// First step, fast path: a = exp(x - xm), lacc = xm.
+template <int K>
+__device__ __forceinline__ void fwd_fast_init(float* a, float& lacc, const float* x, float xm) {
+  constexpr int UNR = Geom<K>::UNROLL ? K : 1;
+#pragma unroll UNR
+  for (int j = 0; j < K; ++j) a[j] = fast_ex2((x[j] - xm) * kLog2e);
+  lacc = xm;
+}
+
+// a <- (a · E) * exp(x - xm);  lacc += xm + tmax;  with renorm, a is rescaled to max 1 (lacc += ln max a).  xm is the
+// step's emission maximum (row_max).  Per step: K*K/2 FFMA2 (a_i broadcast x column pair) + K ex2.  The rescaling
+// divides by max(max a, FLT_MIN): a row with no allowed path has a = 0, which stays 0 (alpha = -inf) instead of turning
+// into NaN.  Any other row has max a >= (max of the previous a) * min E, since the tag holding xm contributes
+// ex2(0) = 1: at least e^-60 when every second step renormalises.
+template <int K, bool EREG>
+__device__ __forceinline__ void fwd_fast_step(float* a, float& lacc, const float* x, float xm, float tmax,
+                                              const f32x2* E2, const float* s_E, bool renorm) {
+  constexpr int UNR = Geom<K>::UNROLL ? K : 1;
+  constexpr int KP = (K + 1) / 2;
+  const float nx2 = -xm * kLog2e;
+  // K/2 independent packed accumulators, i-outer: K/2-way ILP in the FFMA2 block
+  f32x2 ns[KP];
+#pragma unroll UNR
+  for (int q = 0; q < KP; ++q) ns[q] = mul2(pk2(a[0], a[0]), e_pair<K, EREG>(E2, s_E, 0, q));
+#pragma unroll UNR
+  for (int i = 1; i < K; ++i) {
+#pragma unroll UNR
+    for (int q = 0; q < KP; ++q) ns[q] = fma2(pk2(a[i], a[i]), e_pair<K, EREG>(E2, s_E, i, q), ns[q]);
+  }
+  lacc += xm + tmax;
+  float n[2 * KP];
+#pragma unroll UNR
+  for (int q = 0; q < KP; ++q) {
+    const f32x2 arg = fma2(pk2(x[2 * q], 2 * q + 1 < K ? x[2 * q + 1] : 0.f), pk2(kLog2e, kLog2e), pk2(nx2, nx2));
+    float lo, hi;
+    upk2(arg, lo, hi);
+    ns[q] = mul2(ns[q], pk2(fast_ex2(lo), fast_ex2(hi)));
+    if (renorm) upk2(ns[q], n[2 * q], n[2 * q + 1]);
+  }
+  if (renorm) {
+    const float m = fmaxf(row_max<K>(n), FLT_MIN);
+    const float r = __fdividef(1.f, m);
+    lacc = fmaf(kLn2, fast_lg2(m), lacc);
+#pragma unroll UNR
+    for (int q = 0; q < KP; ++q) ns[q] = mul2(ns[q], pk2(r, r));
+  }
+#pragma unroll UNR
+  for (int q = 0; q < KP; ++q) {
+    float lo, hi;
+    upk2(ns[q], lo, hi);
+    a[2 * q] = lo;
+    if (2 * q + 1 < K) a[2 * q + 1] = hi;
+  }
+}
+
+// Exact path: a[j] <- x[j] + logsumexp_i(a[i] + trans[i][j]), each column with its own max (reduce_logsumexp, with
+// its finite-max guard).
+template <int K>
+__device__ __forceinline__ void fwd_exact_step(float* a, const float* x, const float* s_tr) {
+  constexpr int UNR = Geom<K>::UNROLL ? K : 1;
+  float na[K];
+#pragma unroll UNR
+  for (int j = 0; j < K; ++j) {
+    float m = -INFINITY;
+#pragma unroll UNR
+    for (int i = 0; i < K; ++i) m = fmaxf(m, a[i] + s_tr[i * K + j]);
+    const float mm = (fabsf(m) <= 3.0e38f) ? m : 0.f;
+    float sum = 0.f;
+#pragma unroll UNR
+    for (int i = 0; i < K; ++i) sum += expf(a[i] + s_tr[i * K + j] - mm);
+    na[j] = x[j] + (logf(sum) + mm);
+  }
+#pragma unroll UNR
+  for (int j = 0; j < K; ++j) a[j] = na[j];
+}
+
+// alpha_t into the workspace row dst[K].
+template <int K>
+__device__ __forceinline__ void store_alpha(float* dst, const float* a, float lacc, bool fast) {
+  constexpr int UNR = Geom<K>::UNROLL ? K : 1;
+#pragma unroll UNR
+  for (int j = 0; j < K; ++j) dst[j] = fast ? fmaf(kLn2, fast_lg2(a[j]), lacc) : a[j];
+}
+
+// log Z = logsumexp_j alpha_j of the last step.
+template <int K>
+__device__ __forceinline__ float fwd_logz(const float* a, float lacc, bool fast) {
+  constexpr int UNR = Geom<K>::UNROLL ? K : 1;
+  if (fast) {
+    float sum = 0.f;
+#pragma unroll UNR
+    for (int j = 0; j < K; ++j) sum += a[j];
+    return lacc + logf(sum);
+  }
+  float m = a[0];
+#pragma unroll UNR
+  for (int j = 1; j < K; ++j) m = fmaxf(m, a[j]);
+  const float mm = (fabsf(m) <= 3.0e38f) ? m : 0.f;
+  float sum = 0.f;
+#pragma unroll UNR
+  for (int j = 0; j < K; ++j) sum += expf(a[j] - mm);
+  return logf(sum) + mm;
+}
+
+// ------------------------------------------------------------------------------ loss backward, thread per sequence
+// One thread walks t = len-1 .. 0 with beta[K] in registers; logits, the forward's alpha and the labels are streamed
+// in reverse, and d_logits goes back through the logits' tile so the HBM store is coalesced.
+
+// Shared memory of the thread-per-sequence backwards: trans, E, the CTA's d_trans, row maxima [32], row lengths, and a
+// ring of NF staged float tensors (logits and the forward's alphas) plus the label chunks.
+template <int K, int NT, int NF>
+constexpr size_t bwd_smem_bytes() {
+  using Gm = Geom<K>;
+  return 4 * (3 * (size_t)Gm::KK4 + 32 + NT + (size_t)NF * NSTAGE * NT * Gm::P + (size_t)NSTAGE * NT * LABP);
+}
+
+// trans -> s_tr, s_dT = 0, row lengths -> s_len, E[i][j] = exp(trans[i][j] - rmax[i]) when the fast path applies.
+// Returns whether it does; bmax gets the CTA's longest row.
+template <int K, int NT>
+__device__ __forceinline__ bool bwd_prologue(const float* __restrict__ trans, int mylen, float* s_tr, float* s_E,
+                                             float* s_dT, float* s_rmax, int* s_len, int* scratch, int& bmax) {
+  const int tid = threadIdx.x;
+  for (int e = tid; e < K * K; e += NT) {
+    s_tr[e] = trans[e];
+    s_dT[e] = 0.f;
+  }
+  s_len[tid] = mylen;
+  bmax = block_max_int<NT>(mylen, scratch);
+  if (tid < K) {
+    float rm = -INFINITY;
+    for (int j = 0; j < K; ++j) rm = fmaxf(rm, s_tr[tid * K + j]);
+    s_rmax[tid] = rm;
+  }
+  __syncthreads();
+  float hi;
+  const bool fast = trans_is_narrow(s_tr, K * K, hi);
+  for (int e = tid; e < K * K; e += NT) s_E[e] = fast ? expf(s_tr[e] - s_rmax[e / K]) : 0.f;
+  __syncthreads();
+  return fast;
+}
+
+// d_logits of the chunks past the CTA's longest row (from chunk nchunk on) are zero.
+template <int K, int NT>
+__device__ __forceinline__ void zero_dlogits_tail(float* gd, int nv, int L, int nchunk) {
+  using Gm = Geom<K>;
+  const int LK = L * K;
+  for (int c = nchunk; c < (L + Gm::T - 1) / Gm::T; ++c) {
+    const int t0 = c * Gm::T;
+    const int ne = min(Gm::T, L - t0) * K;
+    for (int idx = threadIdx.x; idx < NT * Gm::CE; idx += NT) {
+      const int r = idx / Gm::CE, e = idx - r * Gm::CE;
+      if (r < nv && e < ne) gd[(size_t)r * LK + (size_t)t0 * K + e] = 0.f;
+    }
+  }
+}
+
+// beta[i] <- logsumexp_j(trans[i][j] + u[j]).  Fast path through E and the row maxima rmax, leaving q = exp(u - mq)
+// and mq for the next pair marginal; exact path with each row's own max, leaving uk = u (q and uk may be one array).
+template <int K>
+__device__ __forceinline__ void beta_step(bool fast, float* beta, float* q, float& mq, float* uk, const float* u,
+                                          const float* s_tr, const float* s_E, const float* rmax) {
+  constexpr int UNR = Geom<K>::UNROLL ? K : 1;
+  if (fast) {
+    float m = u[0];
+#pragma unroll UNR
+    for (int j = 1; j < K; ++j) m = fmaxf(m, u[j]);
+    mq = m;
+#pragma unroll UNR
+    for (int j = 0; j < K; ++j) q[j] = __expf(u[j] - m);
+#pragma unroll UNR
+    for (int i = 0; i < K; ++i) {
+      float sum = 0.f;
+#pragma unroll UNR
+      for (int j = 0; j < K; ++j) sum = fmaf(s_E[i * K + j], q[j], sum);
+      beta[i] = m + rmax[i] + __logf(sum);
+    }
+  } else {
+    float nb[K];
+#pragma unroll UNR
+    for (int i = 0; i < K; ++i) {
+      float m = -INFINITY;
+#pragma unroll UNR
+      for (int j = 0; j < K; ++j) m = fmaxf(m, s_tr[i * K + j] + u[j]);
+      const float mm = (fabsf(m) <= 3.0e38f) ? m : 0.f;
+      float sum = 0.f;
+#pragma unroll UNR
+      for (int j = 0; j < K; ++j) sum += expf(s_tr[i * K + j] + u[j] - mm);
+      nb[i] = logf(sum) + mm;
+    }
+#pragma unroll UNR
+    for (int i = 0; i < K; ++i) {
+      beta[i] = nb[i];
+      uk[i] = u[i];
+    }
+  }
+}
+
+// Coalesced store of chunk t0's d_logits from the staged tile sx[NT][P]; zero at t >= s_len[r].
+template <int K, int NT>
+__device__ __forceinline__ void store_dlogits_chunk(float* gd, const float* sx, const int* s_len, int nv, int L,
+                                                    int t0, int vec) {
+  using Gm = Geom<K>;
+  const int LK = L * K;
+  const int ne = min(Gm::T, L - t0) * K;
+  if (vec) {
+    for (int idx = threadIdx.x; idx < NT * Gm::NQ; idx += NT) {
+      const int r = idx / Gm::NQ, qq = idx - r * Gm::NQ;
+      if (r < nv && 4 * qq < ne) {
+        const int valid = (s_len[r] - t0) * K;  // elements [0, valid) carry gradients
+        float4 v = *reinterpret_cast<const float4*>(sx + r * Gm::P + 4 * qq);
+        if (4 * qq + 0 >= valid) v.x = 0.f;
+        if (4 * qq + 1 >= valid) v.y = 0.f;
+        if (4 * qq + 2 >= valid) v.z = 0.f;
+        if (4 * qq + 3 >= valid) v.w = 0.f;
+        *reinterpret_cast<float4*>(gd + (size_t)r * LK + (size_t)t0 * K + 4 * qq) = v;
+      }
+    }
+  } else {
+    for (int idx = threadIdx.x; idx < NT * Gm::CE; idx += NT) {
+      const int r = idx / Gm::CE, e = idx - r * Gm::CE;
+      if (r < nv && e < ne) {
+        const int valid = (s_len[r] - t0) * K;
+        gd[(size_t)r * LK + (size_t)t0 * K + e] = (e < valid) ? sx[r * Gm::P + e] : 0.f;
+      }
+    }
+  }
+}
+
+// d_trans += coef * acc * E (the per-thread register accumulators of the fast path, warp-reduced into s_dT) plus what
+// the CTA gathered in s_dT.
+template <int K, int NT>
+__device__ __forceinline__ void flush_dtrans(const float* acc, float coef, bool active, float* s_dT, const float* s_E,
+                                             float* d_trans) {
+  if constexpr (Geom<K>::ACC_REGS) {
+#pragma unroll
+    for (int e = 0; e < K * K; ++e) {
+      float v = active ? coef * acc[e] * s_E[e] : 0.f;
+      v = warp_sum(v);
+      if ((threadIdx.x & 31) == 0 && v != 0.f) atomicAdd(&s_dT[e], v);
+    }
+  }
+  __syncthreads();
+  for (int e = threadIdx.x; e < K * K; e += NT) {
+    const float v = s_dT[e];
+    if (v != 0.f) atomicAdd(&d_trans[e], v);
+  }
+}
+
+// The thread-per-sequence kernels run 64-thread CTAs above 128 rows per SM (a backward only where their shared memory
+// fits), 32-thread CTAs otherwise.
+inline bool use_cta64(int B) { return B > ner_num_sms() * 64 * 2; }
+
+// ----------------------------------------------------------------------------------------------- lane per tag
+// Lane-per-tag kernels (crf_small.cu, crf_partial.cu): a group of GS lanes holds the K-wide state of one sequence.
 template <int K>
 struct Lanes {
   static constexpr int GS = K <= 8 ? 8 : (K <= 16 ? 16 : 32);
   static constexpr int SPW = 32 / GS;  // sequences per warp
 };
+
+// The warp's longest row: the trip count of a lane-per-tag kernel's lock-step loop.
+__device__ __forceinline__ int lanes_wmax(int len) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) len = max(len, __shfl_xor_sync(0xffffffffu, len, o));
+  return len;
+}
+
+// x + logsumexp_i(a_i + trans[i][j]) over the group's lanes (tc[i] = trans[i][j] of this lane's tag j), exact with
+// its own max.
+template <int K>
+__device__ __forceinline__ float lanes_alpha_step(float a, float x, const float* tc, int g) {
+  constexpr int GS = Lanes<K>::GS;
+  float v[K];
+  float m = -INFINITY;
+#pragma unroll
+  for (int i = 0; i < K; ++i) {
+    v[i] = __shfl_sync(0xffffffffu, a, g * GS + i) + tc[i];
+    m = fmaxf(m, v[i]);
+  }
+  const float mm = (fabsf(m) <= 3.0e38f) ? m : 0.f;
+  float sum = 0.f;
+#pragma unroll
+  for (int i = 0; i < K; ++i) sum += __expf(v[i] - mm);
+  return x + (__logf(sum) + mm);
+}
+
+// logsumexp_j a_j over the group's lanes (every lane of the group gets it).
+template <int K>
+__device__ __forceinline__ float lanes_logsumexp(float a, bool tag_ok) {
+  constexpr int GS = Lanes<K>::GS;
+  float m = a;
+#pragma unroll
+  for (int o = GS / 2; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o, GS));
+  const float mm = (fabsf(m) <= 3.0e38f) ? m : 0.f;
+  float e = tag_ok ? expf(a - mm) : 0.f;
+#pragma unroll
+  for (int o = GS / 2; o > 0; o >>= 1) e += __shfl_xor_sync(0xffffffffu, e, o, GS);
+  return logf(e) + mm;
+}
+
+// Backward: v[j] = tr[j] + w_j, with w_j from lane j of the group (tr = row i of trans for this lane's tag i).
+// Returns max_j v[j].
+template <int K>
+__device__ __forceinline__ float lanes_gather(float* v, float w, const float* tr, int g) {
+  constexpr int GS = Lanes<K>::GS;
+  float m = -INFINITY;
+#pragma unroll
+  for (int j = 0; j < K; ++j) {
+    v[j] = tr[j] + __shfl_sync(0xffffffffu, w, g * GS + j);
+    m = fmaxf(m, v[j]);
+  }
+  return m;
+}
 
 // Shared memory of the lane-per-tag Viterbi kernel: backpointers [L][32] bytes + decoded tags [SPW][L] ints.
 template <int K>

@@ -11,43 +11,13 @@
 // i.e. K*K FFMA + K ex2 per step (+ one rcp / lg2 per two steps) instead of K*K exp and K log.  Chunks that lie completely inside a sequence (the common case) run a branch-free
 // unrolled body; only the first and the ragged last chunk take the checked path.  The exact path (flags bit0, or
 // chosen automatically for wide/inf transition matrices) evaluates every logsumexp with its
-// own max, exactly as the reference's reduce_logsumexp does.
+// own max, exactly as the reference's reduce_logsumexp does.  The steps themselves are crf_common.cuh's, shared with
+// the partial-annotation loss (crf_partial.cu).
 #include "crf_common.cuh"
 
 namespace {
 
 using namespace crf;
-
-constexpr float kLog2e = 1.4426950408889634f;
-constexpr float kLn2 = 0.6931471805599453f;
-constexpr int TAGP = 12;  // tag-chunk pitch (ints): 3 x 16B, odd -> conflict-free LDS.128
-
-template <int K, int NT, int TT>
-size_t loglik_smem_bytes() {
-  using Gm = Geom<K, TT>;
-  size_t words = 2 * Gm::KK4 + 32 + NT + (size_t)NSTAGE * NT * Gm::P + (size_t)NSTAGE * NT * TAGP;
-  return words * 4;
-}
-
-template <int NT, int TT>
-__device__ __forceinline__ void stage_tags(int* dst, const int32_t* __restrict__ gbase, int L, int t0,
-                                           int nv, const int* s_len, int vec16) {
-  constexpr int T = TT;
-  const int steps = min(T, L - t0);
-  if (vec16) {
-    for (int idx = threadIdx.x; idx < NT * (T / 4); idx += NT) {
-      const int r = idx / (T / 4), q = idx - r * (T / 4);
-      if (r < nv && 4 * q < min(steps, s_len[r] - t0))
-        cp_async16(dst + r * TAGP + 4 * q, gbase + (size_t)r * L + t0 + 4 * q);
-    }
-  } else {
-    for (int idx = threadIdx.x; idx < NT * T; idx += NT) {
-      const int r = idx / T, e = idx - r * T;
-      if (r < nv && e < min(steps, s_len[r] - t0))
-        cp_async4(dst + r * TAGP + e, gbase + (size_t)r * L + t0 + e);
-    }
-  }
-}
 
 template <int K, int NT, int TT, bool EREG, int MINB>
 __global__ void __launch_bounds__(NT, MINB)
@@ -58,14 +28,12 @@ crf_loglik_fwd_kernel(const float* __restrict__ logits, const int32_t* __restric
                       int force_exact) {
   using Gm = Geom<K, TT>;
   constexpr int T = Gm::T, G = Gm::G, P = Gm::P;
-  constexpr bool E_REGS = EREG;
   constexpr int UNR = Gm::UNROLL ? K : 1;
 
   extern __shared__ __align__(16) float smem[];
   float* s_tr = smem;                                   // raw trans [i][j]
-  float* s_E = s_tr + Gm::KK4;                          // exp(trans - cmax[j]) stored [i][j]
-  float* s_cmax = s_E + Gm::KK4;                        // [32]
-  int* s_len = reinterpret_cast<int*>(s_cmax + 32);     // [NT]
+  float* s_E = s_tr + Gm::KK4;                          // exp(trans - tmax) [i][j]
+  int* s_len = reinterpret_cast<int*>(s_E + Gm::KK4);   // [NT]
   float* s_stage = reinterpret_cast<float*>(s_len + NT);
   int* s_tags = reinterpret_cast<int*>(s_stage + NSTAGE * NT * P);
 
@@ -82,26 +50,9 @@ crf_loglik_fwd_kernel(const float* __restrict__ logits, const int32_t* __restric
   }
   s_len[tid] = mylen;
   const int bmax = block_max_int<NT>(tid < nv ? mylen : 1, reinterpret_cast<int*>(s_stage));
-
-  // column maxima, range test, E matrix (tiny; every thread helps)
-  if (tid < K) {
-    float cm = -INFINITY;
-    for (int i = 0; i < K; ++i) cm = fmaxf(cm, s_tr[i * K + tid]);
-    s_cmax[tid] = cm;
-  }
-  __syncthreads();
-  bool fast = !force_exact;
-  float tmax = 0.f;
-  {
-    float lo = INFINITY, hi = -INFINITY;
-    for (int e = 0; e < K * K; ++e) {
-      const float v = s_tr[e];
-      lo = fminf(lo, v);
-      hi = fmaxf(hi, v);
-    }
-    if (!(hi - lo < 30.f) || !(fabsf(hi) < 1e30f) || !(fabsf(lo) < 1e30f)) fast = false;  // also NaN/inf
-    tmax = fast ? hi : 0.f;
-  }
+  float tmax;
+  const bool fast = trans_is_narrow(s_tr, K * K, tmax) && !force_exact;
+  if (!fast) tmax = 0.f;
   for (int e = tid; e < K * K; e += NT) s_E[e] = fast ? expf(s_tr[e] - tmax) : 0.f;
   __syncthreads();
 
@@ -113,90 +64,26 @@ crf_loglik_fwd_kernel(const float* __restrict__ logits, const int32_t* __restric
   for (int s = 0; s < NSTAGE - 1; ++s) {
     if (s < nchunk) {
       stage_logits<K, NT, TT>(s_stage + s * NT * P, gbase, LK, s * T, L, nv, s_len, vec_logits);
-      stage_tags<NT, TT>(s_tags + s * NT * TAGP, tbase, L, s * T, nv, s_len, vec_tags);
+      stage_labels<NT, TT>(s_tags + s * NT * LABP, tbase, L, s * T, nv, s_len, vec_tags);
     }
     cp_async_commit();
   }
 
   // E as packed column pairs: E2[i][q] = (E[i][2q], E[i][2q+1]) (hi lane 0 for the pad column of an odd K)
   constexpr int KP = (K + 1) / 2;
-  f32x2 E2[E_REGS ? K * KP : 1];
-  if (E_REGS) {
+  f32x2 E2[EREG ? K * KP : 1];
+  if (EREG) {
 #pragma unroll
     for (int i = 0; i < K; ++i)
 #pragma unroll
       for (int q = 0; q < KP; ++q) E2[i * KP + q] = pk2(s_E[i * K + 2 * q], 2 * q + 1 < K ? s_E[i * K + 2 * q + 1] : 0.f);
   }
-  auto e2 = [&](int i, int q) -> f32x2 {
-    if (E_REGS) return E2[i * KP + q];
-    return pk2(s_E[i * K + 2 * q], 2 * q + 1 < K ? s_E[i * K + 2 * q + 1] : 0.f);
-  };
-  // Fast path state: alpha_j = lacc + ln(a[j]) with a[] kept in the PROBABILITY domain and
-  // renormalised (max -> 1) every other step; exact path state: a[j] = alpha_j.
   float a[K];
   float lacc = 0.f;
 #pragma unroll UNR
   for (int j = 0; j < K; ++j) a[j] = 0.f;
-  // a <- (a · E) * exp(x - max x);  lacc += max x + tmax   [+ renormalisation]
-  // per step: K*K/2 FFMA2 (a_i broadcast x column pair) + K ex2 (+ 1 rcp + 1 lg2 when renormalising)
   auto fast_step = [&](const float* x, bool renorm) {
-    float xm = x[0];
-    if (K > 1) {
-#pragma unroll UNR
-      for (int j = 1; j + 1 < K; j += 2) xm = max3(xm, x[j], x[j + 1]);
-      if (K % 2 == 0) xm = fmaxf(xm, x[K - 1]);
-    }
-    const float nx2 = -xm * kLog2e;
-    // K/2 independent packed accumulators, i-outer: K/2-way ILP in the FFMA2 block
-    f32x2 ns[KP];
-#pragma unroll UNR
-    for (int q = 0; q < KP; ++q) ns[q] = mul2(pk2(a[0], a[0]), e2(0, q));
-#pragma unroll UNR
-    for (int i = 1; i < K; ++i) {
-#pragma unroll UNR
-      for (int q = 0; q < KP; ++q) ns[q] = fma2(pk2(a[i], a[i]), e2(i, q), ns[q]);
-    }
-    lacc += xm + tmax;
-    float n[2 * KP];
-#pragma unroll UNR
-    for (int q = 0; q < KP; ++q) {
-      const f32x2 arg = fma2(pk2(x[2 * q], 2 * q + 1 < K ? x[2 * q + 1] : 0.f), pk2(kLog2e, kLog2e), pk2(nx2, nx2));
-      float lo, hi;
-      upk2(arg, lo, hi);
-      ns[q] = mul2(ns[q], pk2(fast_ex2(lo), fast_ex2(hi)));
-      if (renorm) upk2(ns[q], n[2 * q], n[2 * q + 1]);
-    }
-    if (renorm) {
-      float m = n[0];
-      if (K > 1) {
-#pragma unroll UNR
-        for (int j = 1; j + 1 < K; j += 2) m = max3(m, n[j], n[j + 1]);
-        if (K % 2 == 0) m = fmaxf(m, n[K - 1]);
-      }
-      const float r = __fdividef(1.f, m);
-      lacc = fmaf(kLn2, fast_lg2(m), lacc);
-#pragma unroll UNR
-      for (int q = 0; q < KP; ++q) ns[q] = mul2(ns[q], pk2(r, r));
-    }
-#pragma unroll UNR
-    for (int q = 0; q < KP; ++q) {
-      float lo, hi;
-      upk2(ns[q], lo, hi);
-      a[2 * q] = lo;
-      if (2 * q + 1 < K) a[2 * q + 1] = hi;
-    }
-  };
-  auto fast_init = [&](const float* x) {
-    float xm = x[0];
-#pragma unroll UNR
-    for (int j = 1; j < K; ++j) xm = fmaxf(xm, x[j]);
-#pragma unroll UNR
-    for (int j = 0; j < K; ++j) a[j] = fast_ex2((x[j] - xm) * kLog2e);
-    lacc = xm;
-  };
-  auto store_alpha = [&](float* dst) {
-#pragma unroll UNR
-    for (int j = 0; j < K; ++j) dst[j] = fast ? fmaf(kLn2, fast_lg2(a[j]), lacc) : a[j];
+    fwd_fast_step<K, EREG>(a, lacc, x, row_max<K>(x), tmax, E2, s_E, renorm);
   };
 
   float score = 0.f;
@@ -207,7 +94,7 @@ crf_loglik_fwd_kernel(const float* __restrict__ logits, const int32_t* __restric
     const int cn = c + NSTAGE - 1;
     if (cn < nchunk) {
       stage_logits<K, NT, TT>(s_stage + (cn % NSTAGE) * NT * P, gbase, LK, cn * T, L, nv, s_len, vec_logits);
-      stage_tags<NT, TT>(s_tags + (cn % NSTAGE) * NT * TAGP, tbase, L, cn * T, nv, s_len, vec_tags);
+      stage_labels<NT, TT>(s_tags + (cn % NSTAGE) * NT * LABP, tbase, L, cn * T, nv, s_len, vec_tags);
     }
     cp_async_commit();
     cp_async_wait<NSTAGE - 1>();
@@ -218,7 +105,7 @@ crf_loglik_fwd_kernel(const float* __restrict__ logits, const int32_t* __restric
       const float* rowp = s_stage + (c % NSTAGE) * NT * P + tid * P;
       int tg[T];
       {
-        const int4* tp = reinterpret_cast<const int4*>(s_tags + (c % NSTAGE) * NT * TAGP + tid * TAGP);
+        const int4* tp = reinterpret_cast<const int4*>(s_tags + (c % NSTAGE) * NT * LABP + tid * LABP);
 #pragma unroll
         for (int q = 0; q < T / 4; ++q) {
           const int4 v = tp[q];
@@ -241,7 +128,7 @@ crf_loglik_fwd_kernel(const float* __restrict__ logits, const int32_t* __restric
             score += rowp[tt * K + tag] + s_tr[prev * K + tag];
             prev = tag;
             fast_step(xs + gg * K, (tt & 1) != 0 || T < 2);
-            if (aws != nullptr) store_alpha(aws + (size_t)(t0 + tt) * K);
+            if (aws != nullptr) store_alpha<K>(aws + (size_t)(t0 + tt) * K, a, lacc, fast);
           }
         }
       } else
@@ -263,7 +150,7 @@ crf_loglik_fwd_kernel(const float* __restrict__ logits, const int32_t* __restric
               // ---- forward-alpha (crf_log_norm)
               if (t == 0) {
                 if (fast) {
-                  fast_init(xs + gg * K);
+                  fwd_fast_init<K>(a, lacc, xs + gg * K, row_max<K>(xs + gg * K));
                 } else {
 #pragma unroll UNR
                   for (int j = 0; j < K; ++j) a[j] = xs[gg * K + j];
@@ -271,22 +158,9 @@ crf_loglik_fwd_kernel(const float* __restrict__ logits, const int32_t* __restric
               } else if (fast) {
                 fast_step(xs + gg * K, true);
               } else {
-                float na[K];
-#pragma unroll UNR
-                for (int j = 0; j < K; ++j) {
-                  float m = -INFINITY;
-#pragma unroll UNR
-                  for (int i = 0; i < K; ++i) m = fmaxf(m, a[i] + s_tr[i * K + j]);
-                  const float mm = (fabsf(m) <= 3.0e38f) ? m : 0.f;  // reduce_logsumexp's finite-max guard
-                  float sum = 0.f;
-#pragma unroll UNR
-                  for (int i = 0; i < K; ++i) sum += expf(a[i] + s_tr[i * K + j] - mm);
-                  na[j] = xs[gg * K + j] + (logf(sum) + mm);
-                }
-#pragma unroll UNR
-                for (int j = 0; j < K; ++j) a[j] = na[j];
+                fwd_exact_step<K>(a, xs + gg * K, s_tr);
               }
-              if (aws != nullptr) store_alpha(aws + (size_t)t * K);
+              if (aws != nullptr) store_alpha<K>(aws + (size_t)t * K, a, lacc, fast);
             }
           }
         }
@@ -296,22 +170,7 @@ crf_loglik_fwd_kernel(const float* __restrict__ logits, const int32_t* __restric
   }
 
   if (tid < nv) {
-    float logz;
-    if (fast) {
-      float sum = 0.f;
-#pragma unroll UNR
-      for (int j = 0; j < K; ++j) sum += a[j];
-      logz = lacc + logf(sum);
-    } else {
-      float m = a[0];
-#pragma unroll UNR
-      for (int j = 1; j < K; ++j) m = fmaxf(m, a[j]);
-      const float mm = (fabsf(m) <= 3.0e38f) ? m : 0.f;
-      float sum = 0.f;
-#pragma unroll UNR
-      for (int j = 0; j < K; ++j) sum += expf(a[j] - mm);
-      logz = logf(sum) + mm;
-    }
+    float logz = fwd_logz<K>(a, lacc, fast);
     if (rawlen <= 0) {  // crf_log_norm / crf_sequence_score: zero for empty sequences
       logz = 0.f;
       score = 0.f;
@@ -325,7 +184,7 @@ template <int K, int NT, int TT, bool EREG, int MINB = 1>
 int launch_fwd_nt(const float* logits, const int32_t* tags, const int32_t* seq_len,
                   const float* trans, float* ll, float* logz, float* alpha_ws, int B, int L,
                   int flags, cudaStream_t st) {
-  const size_t smem = loglik_smem_bytes<K, NT, TT>();
+  const size_t smem = fwd_smem_bytes<K, NT, TT>();
   auto kern = crf_loglik_fwd_kernel<K, NT, TT, EREG, MINB>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
@@ -341,7 +200,7 @@ int launch_fwd(const float* logits, const int32_t* tags, const int32_t* seq_len,
                float* ll, float* logz, float* alpha_ws, int B, int L, int flags, cudaStream_t st) {
   constexpr bool ER = (K <= 10);
   // big batches: 4-step chunks (30 KB smem / CTA) and <= 170 registers: 6 CTAs = 12 warps per SM
-  if (B > ner_num_sms() * 64 * 2)
+  if (use_cta64(B))
     return launch_fwd_nt<K, 64, 4, ER, 6>(logits, tags, seq_len, trans, ll, logz, alpha_ws, B, L, flags, st);
   return launch_fwd_nt<K, 32, T_CHUNK, ER>(logits, tags, seq_len, trans, ll, logz, alpha_ws, B, L, flags, st);
 }
@@ -356,10 +215,8 @@ extern "C" int ner_crf_loglik_fwd(const float* logits, const int32_t* tags, cons
   if (!logits || !tags || !seq_len || !trans || !ll) return NER_ERR_INVALID_ARG;
   if (K > NER_MAX_TAGS) return NER_ERR_UNSUPPORTED;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (B <= NER_CRF_SMALL_B && !(flags & 2)) {  // flags bit1: force the throughput kernel (tests / benches)
-    const int rc = ner_crf_loglik_fwd_small(logits, tags, seq_len, trans, ll, logz_out, alpha_ws, B, L, K, st);
-    if (rc != NER_ERR_UNSUPPORTED) return rc;
-  }
+  if (B <= NER_CRF_SMALL_B && !(flags & 2))  // flags bit1: force the throughput kernel (tests / benches)
+    return ner_crf_loglik_fwd_small(logits, tags, seq_len, trans, ll, logz_out, alpha_ws, B, L, K, st);
 #define CALL(KK) return launch_fwd<KK>(logits, tags, seq_len, trans, ll, logz_out, alpha_ws, B, L, flags, st)
   NER_CRF_DISPATCH_K(K, CALL)
 #undef CALL

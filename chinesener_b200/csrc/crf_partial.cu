@@ -18,57 +18,22 @@
 //                         takes the thread-per-sequence kernel instead (tests).
 //   forward   thread per sequence; B > 128 * SMs: 64-thread CTAs, 4-step chunks; otherwise 32-thread CTAs, 8-step
 //             chunks.  Fast scaled-probability step when the transition matrix spans < 30 nats and is finite, exact
-//             per-column logsumexp otherwise or when flags bit0 is set (the rule of crf_loglik.cu).
+//             per-column logsumexp otherwise or when flags bit0 is set.
 //   backward  thread per sequence; 64-thread CTAs when B > 128 * SMs and their staging ring fits in shared memory
 //             (K <= 17), 32-thread CTAs otherwise.  Fast / exact as the forward, decided from trans alone.
+// The staging, recursion steps, prologues, stores, shared-memory sizes and routes are those of the ordinary loss, in
+// crf_common.cuh; the loop bodies here are what differs: two recursions, the allowed-set masks, P_A - P.
 // Workspace: alpha_ws [2][B][L][K] = (alpha_A, alpha); logz [B][2] = (logZ_A, logZ).
 #include "crf_common.cuh"
 
 namespace {
 
 using namespace crf;
-using crf::Lanes;
 
-constexpr float kLog2e = 1.4426950408889634f;
-constexpr float kLn2 = 0.6931471805599453f;
-
-// fast (scaled-probability) path possible for this transition matrix? (the test of crf_loglik.cu / crf_bwd.cu)
-__device__ __forceinline__ bool trans_is_narrow(const float* s_tr, int KK) {
-  float lo = INFINITY, hi = -INFINITY;
-  for (int e = 0; e < KK; ++e) {
-    lo = fminf(lo, s_tr[e]);
-    hi = fmaxf(hi, s_tr[e]);
-  }
-  return (hi - lo < 30.f) && (fabsf(hi) < 1e30f) && (fabsf(lo) < 1e30f);
-}
-
-constexpr int TAGP = 12;  // pitch (ints) of a row's staged masks: 3 x 16B, odd -> conflict-free LDS.128
-
-// Stage chunk [t0, t0+TT) of the CTA's label_mask rows into dst[NT][TAGP]; steps at t >= s_len[r] are not fetched.
-// (crf_loglik.cu / crf_bwd.cu stage their gold tags the same way.)
-template <int NT, int TT>
-__device__ __forceinline__ void stage_masks(int* dst, const int32_t* __restrict__ gbase, int L, int t0, int nv,
-                                            const int* s_len, int vec16) {
-  const int steps = min(TT, L - t0);
-  if (vec16) {
-    for (int idx = threadIdx.x; idx < NT * (TT / 4); idx += NT) {
-      const int r = idx / (TT / 4), q = idx - r * (TT / 4);
-      if (r < nv && 4 * q < min(steps, s_len[r] - t0))
-        cp_async16(dst + r * TAGP + 4 * q, gbase + (size_t)r * L + t0 + 4 * q);
-    }
-  } else {
-    for (int idx = threadIdx.x; idx < NT * TT; idx += NT) {
-      const int r = idx / TT, e = idx - r * TT;
-      if (r < nv && e < min(steps, s_len[r] - t0)) cp_async4(dst + r * TAGP + e, gbase + (size_t)r * L + t0 + e);
-    }
-  }
-}
-
-template <int K, int NT, int TT>
-size_t partial_fwd_smem_bytes() {
-  using Gm = Geom<K, TT>;
-  size_t words = 2 * Gm::KK4 + NT + (size_t)NSTAGE * NT * Gm::P + (size_t)NSTAGE * NT * TAGP;
-  return words * 4;
+// Does mask m allow none of the K tags?
+template <int K>
+__device__ __forceinline__ bool mask_empty(unsigned m) {
+  return (K < 32 ? (m & ((1u << (K & 31)) - 1u)) : m) == 0u;
 }
 
 // The forward state of one recursion: alpha_j = lacc + ln a[j] (fast) or a[j] = alpha_j (exact).
@@ -87,7 +52,6 @@ crf_partial_fwd_kernel(const float* __restrict__ logits, const int32_t* __restri
   using Gm = Geom<K, TT>;
   constexpr int T = Gm::T, G = Gm::G, P = Gm::P;
   constexpr int UNR = Gm::UNROLL ? K : 1;
-  constexpr int KP = (K + 1) / 2;
 
   extern __shared__ __align__(16) float smem[];
   float* s_tr = smem;                                // raw trans [i][j]
@@ -109,10 +73,9 @@ crf_partial_fwd_kernel(const float* __restrict__ logits, const int32_t* __restri
   }
   s_len[tid] = mylen;
   const int bmax = block_max_int<NT>(tid < nv ? mylen : 1, reinterpret_cast<int*>(s_stage));
-  const bool fast = !force_exact && trans_is_narrow(s_tr, K * K);
-  float tmax = 0.f;
-  if (fast)
-    for (int e = 0; e < K * K; ++e) tmax = e == 0 ? s_tr[0] : fmaxf(tmax, s_tr[e]);
+  float tmax;
+  const bool fast = trans_is_narrow(s_tr, K * K, tmax) && !force_exact;
+  if (!fast) tmax = 0.f;
   for (int e = tid; e < K * K; e += NT) s_E[e] = fast ? expf(s_tr[e] - tmax) : 0.f;
   __syncthreads();
 
@@ -124,109 +87,28 @@ crf_partial_fwd_kernel(const float* __restrict__ logits, const int32_t* __restri
   for (int s = 0; s < NSTAGE - 1; ++s) {
     if (s < nchunk) {
       stage_logits<K, NT, TT>(s_stage + s * NT * P, gbase, LK, s * T, L, nv, s_len, vec_logits);
-      stage_masks<NT, TT>(s_mask + s * NT * TAGP, mbase, L, s * T, nv, s_len, vec_mask);
+      stage_labels<NT, TT>(s_mask + s * NT * LABP, mbase, L, s * T, nv, s_len, vec_mask);
     }
     cp_async_commit();
   }
 
-  auto e2 = [&](int i, int q) -> f32x2 {
-    return pk2(s_E[i * K + 2 * q], 2 * q + 1 < K ? s_E[i * K + 2 * q + 1] : 0.f);
-  };
-  // a <- (a · E) * exp(x - max x);  lacc += max x + tmax;  renormalised (max -> 1) every step.  For the constrained
-  // recursion x holds -inf at the disallowed tags, so the max is taken over the allowed ones.
-  auto fast_step = [&](Alpha<K>& s, const float* x) {
-    float xm = x[0];
-#pragma unroll UNR
-    for (int j = 1; j < K; ++j) xm = fmaxf(xm, x[j]);
-    if (!(xm > -INFINITY)) xm = 0.f;  // empty set: the row's ll is -inf whatever this step computes
-    const float nx2 = -xm * kLog2e;
-    f32x2 ns[KP];
-#pragma unroll UNR
-    for (int q = 0; q < KP; ++q) ns[q] = mul2(pk2(s.a[0], s.a[0]), e2(0, q));
-#pragma unroll UNR
-    for (int i = 1; i < K; ++i) {
-#pragma unroll UNR
-      for (int q = 0; q < KP; ++q) ns[q] = fma2(pk2(s.a[i], s.a[i]), e2(i, q), ns[q]);
-    }
-    s.lacc += xm + tmax;
-    float n[2 * KP];
-#pragma unroll UNR
-    for (int q = 0; q < KP; ++q) {
-      float lo = fmaf(x[2 * q], kLog2e, nx2), hi = 2 * q + 1 < K ? fmaf(x[2 * q + 1], kLog2e, nx2) : 0.f;
-      ns[q] = mul2(ns[q], pk2(fast_ex2(lo), fast_ex2(hi)));
-      upk2(ns[q], n[2 * q], n[2 * q + 1]);
-    }
-    float m = n[0];
-#pragma unroll UNR
-    for (int j = 1; j < K; ++j) m = fmaxf(m, n[j]);
-    if (m > 0.f) {
-      const float r = __fdividef(1.f, m);
-      s.lacc = fmaf(kLn2, fast_lg2(m), s.lacc);
-#pragma unroll UNR
-      for (int j = 0; j < K; ++j) s.a[j] = n[j] * r;
-    } else {
-#pragma unroll UNR
-      for (int j = 0; j < K; ++j) s.a[j] = n[j];
-    }
-  };
-  auto fast_init = [&](Alpha<K>& s, const float* x) {
-    float xm = x[0];
-#pragma unroll UNR
-    for (int j = 1; j < K; ++j) xm = fmaxf(xm, x[j]);
-    if (!(xm > -INFINITY)) xm = 0.f;
-#pragma unroll UNR
-    for (int j = 0; j < K; ++j) s.a[j] = fast_ex2((x[j] - xm) * kLog2e);
-    s.lacc = xm;
-  };
-  auto exact_step = [&](Alpha<K>& s, const float* x) {
-    float na[K];
-#pragma unroll UNR
-    for (int j = 0; j < K; ++j) {
-      float m = -INFINITY;
-#pragma unroll UNR
-      for (int i = 0; i < K; ++i) m = fmaxf(m, s.a[i] + s_tr[i * K + j]);
-      const float mm = (fabsf(m) <= 3.0e38f) ? m : 0.f;
-      float sum = 0.f;
-#pragma unroll UNR
-      for (int i = 0; i < K; ++i) sum += expf(s.a[i] + s_tr[i * K + j] - mm);
-      na[j] = x[j] + (logf(sum) + mm);
-    }
-#pragma unroll UNR
-    for (int j = 0; j < K; ++j) s.a[j] = na[j];
-  };
+  // One step of either recursion.  For the constrained one x holds -inf at the disallowed tags, so the fast path's
+  // max is taken over the allowed ones; an empty set leaves xm = -inf, which is replaced by 0 (the row's ll is -inf
+  // whatever this step computes).  The fast path renormalises every step.
   auto step = [&](Alpha<K>& s, const float* x, int t) {
-    if (t == 0) {
-      if (fast) {
-        fast_init(s, x);
-      } else {
-#pragma unroll UNR
-        for (int j = 0; j < K; ++j) s.a[j] = x[j];
-      }
-    } else if (fast) {
-      fast_step(s, x);
-    } else {
-      exact_step(s, x);
-    }
-  };
-  auto store_alpha = [&](const Alpha<K>& s, float* dst) {
-#pragma unroll UNR
-    for (int j = 0; j < K; ++j) dst[j] = fast ? fmaf(kLn2, fast_lg2(s.a[j]), s.lacc) : s.a[j];
-  };
-  auto logsum = [&](const Alpha<K>& s) -> float {
     if (fast) {
-      float sum = 0.f;
+      float xm = row_max<K>(x);
+      if (!(xm > -INFINITY)) xm = 0.f;
+      if (t == 0)
+        fwd_fast_init<K>(s.a, s.lacc, x, xm);
+      else
+        fwd_fast_step<K, false>(s.a, s.lacc, x, xm, tmax, nullptr, s_E, true);
+    } else if (t == 0) {
 #pragma unroll UNR
-      for (int j = 0; j < K; ++j) sum += s.a[j];
-      return s.lacc + logf(sum);
+      for (int j = 0; j < K; ++j) s.a[j] = x[j];
+    } else {
+      fwd_exact_step<K>(s.a, x, s_tr);
     }
-    float m = s.a[0];
-#pragma unroll UNR
-    for (int j = 1; j < K; ++j) m = fmaxf(m, s.a[j]);
-    const float mm = (fabsf(m) <= 3.0e38f) ? m : 0.f;
-    float sum = 0.f;
-#pragma unroll UNR
-    for (int j = 0; j < K; ++j) sum += expf(s.a[j] - mm);
-    return logf(sum) + mm;
   };
 
   Alpha<K> sa, sf;  // constrained, free
@@ -241,7 +123,7 @@ crf_partial_fwd_kernel(const float* __restrict__ logits, const int32_t* __restri
     const int cn = c + NSTAGE - 1;
     if (cn < nchunk) {
       stage_logits<K, NT, TT>(s_stage + (cn % NSTAGE) * NT * P, gbase, LK, cn * T, L, nv, s_len, vec_logits);
-      stage_masks<NT, TT>(s_mask + (cn % NSTAGE) * NT * TAGP, mbase, L, cn * T, nv, s_len, vec_mask);
+      stage_labels<NT, TT>(s_mask + (cn % NSTAGE) * NT * LABP, mbase, L, cn * T, nv, s_len, vec_mask);
     }
     cp_async_commit();
     cp_async_wait<NSTAGE - 1>();
@@ -250,7 +132,7 @@ crf_partial_fwd_kernel(const float* __restrict__ logits, const int32_t* __restri
     const int t0 = c * T;
     if (tid < nv && t0 < mylen) {
       const float* rowp = s_stage + (c % NSTAGE) * NT * P + tid * P;
-      const int* rowm = s_mask + (c % NSTAGE) * NT * TAGP + tid * TAGP;
+      const int* rowm = s_mask + (c % NSTAGE) * NT * LABP + tid * LABP;
 #pragma unroll
       for (int g = 0; g < T / G; ++g) {
         if (t0 + g * G < mylen) {
@@ -266,12 +148,12 @@ crf_partial_fwd_kernel(const float* __restrict__ logits, const int32_t* __restri
               float xa[K];
 #pragma unroll UNR
               for (int j = 0; j < K; ++j) xa[j] = ((m >> j) & 1u) ? x[j] : -INFINITY;
-              empty |= (K < 32 ? (m & ((1u << (K & 31)) - 1u)) : m) == 0u;
+              empty |= mask_empty<K>(m);
               step(sa, xa, t);
               step(sf, x, t);
               if (aws_a != nullptr) {
-                store_alpha(sa, aws_a + (size_t)t * K);
-                store_alpha(sf, aws_f + (size_t)t * K);
+                store_alpha<K>(aws_a + (size_t)t * K, sa.a, sa.lacc, fast);
+                store_alpha<K>(aws_f + (size_t)t * K, sf.a, sf.lacc, fast);
               }
             }
           }
@@ -282,7 +164,7 @@ crf_partial_fwd_kernel(const float* __restrict__ logits, const int32_t* __restri
   }
 
   if (tid < nv) {
-    float lza = logsum(sa), lzf = logsum(sf);
+    float lza = fwd_logz<K>(sa.a, sa.lacc, fast), lzf = fwd_logz<K>(sf.a, sf.lacc, fast);
     if (empty) lza = -INFINITY;
     if (rawlen <= 0) lza = lzf = 0.f;  // empty sequence: ll = 0, nothing to differentiate
     ll[row0 + tid] = lza - lzf;
@@ -296,7 +178,7 @@ crf_partial_fwd_kernel(const float* __restrict__ logits, const int32_t* __restri
 template <int K, int NT, int TT, int MINB = 1>
 int launch_fwd_nt(const float* logits, const int32_t* mask, const int32_t* seq_len, const float* trans, float* ll,
                   float* logz, float* alpha_ws, int B, int L, int flags, cudaStream_t st) {
-  const size_t smem = partial_fwd_smem_bytes<K, NT, TT>();
+  const size_t smem = fwd_smem_bytes<K, NT, TT>();
   auto kern = crf_partial_fwd_kernel<K, NT, TT, MINB>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
@@ -315,19 +197,12 @@ int launch_fwd(const float* logits, const int32_t* mask, const int32_t* seq_len,
                float* logz, float* alpha_ws, int B, int L, int flags, cudaStream_t st) {
   if (B <= NER_CRF_SMALL_B && !(flags & 2))  // flags bit1: the throughput kernel at any B (tests)
     return launch_fwd_lanes<K>(logits, mask, seq_len, trans, ll, logz, alpha_ws, B, L, st);
-  if (B > ner_num_sms() * 64 * 2)
+  if (use_cta64(B))
     return launch_fwd_nt<K, 64, 4, 4>(logits, mask, seq_len, trans, ll, logz, alpha_ws, B, L, flags, st);
   return launch_fwd_nt<K, 32, T_CHUNK>(logits, mask, seq_len, trans, ll, logz, alpha_ws, B, L, flags, st);
 }
 
 // ---------------------------------------------------------------------------------------------------------- backward
-
-template <int K, int NT>
-constexpr size_t partial_bwd_smem_bytes() {
-  using Gm = Geom<K>;
-  size_t words = 3 * Gm::KK4 + 32 + NT + 3 * (size_t)NSTAGE * NT * Gm::P + (size_t)NSTAGE * NT * TAGP;
-  return words * 4;
-}
 
 // One reverse pass with beta_A and beta.  Pair marginals (fast path) accumulate per thread as
 // acc[i][j] += pa_A[i] q_A[j] - pa[i] q[j]  and are scaled by exp(trans - rowmax) once at the end.
@@ -341,7 +216,7 @@ crf_partial_bwd_kernel(const float* __restrict__ logits, const int32_t* __restri
   using Gm = Geom<K>;
   constexpr int T = Gm::T, G = Gm::G, P = Gm::P;
   constexpr int UNR = Gm::UNROLL ? K : 1;
-  constexpr bool ACC_REGS = (K <= 10);
+  constexpr bool ACC_REGS = Gm::ACC_REGS;
 
   extern __shared__ __align__(16) float smem[];
   float* s_tr = smem;                                // raw trans [i][j]
@@ -359,10 +234,6 @@ crf_partial_bwd_kernel(const float* __restrict__ logits, const int32_t* __restri
   const int nv = min(NT, B - row0);
   const int LK = L * K;
 
-  for (int e = tid; e < K * K; e += NT) {
-    s_tr[e] = trans[e];
-    s_dT[e] = 0.f;
-  }
   float lza = 0.f, lzf = 0.f, gcoef = 0.f;
   int mylen = 0;
   if (tid < nv) {
@@ -372,17 +243,8 @@ crf_partial_bwd_kernel(const float* __restrict__ logits, const int32_t* __restri
     gcoef = (d_ll != nullptr ? d_ll[row0 + tid] : 1.f) * scale;
     if (!(lza > -INFINITY)) mylen = 0;  // an empty allowed set: ll = -inf, the row adds no gradient
   }
-  s_len[tid] = mylen;
-  const int bmax = block_max_int<NT>(mylen, reinterpret_cast<int*>(s_x));
-  if (tid < K) {
-    float rm = -INFINITY;
-    for (int j = 0; j < K; ++j) rm = fmaxf(rm, s_tr[tid * K + j]);
-    s_rmax[tid] = rm;
-  }
-  __syncthreads();
-  const bool fast = trans_is_narrow(s_tr, K * K);
-  for (int e = tid; e < K * K; e += NT) s_E[e] = fast ? expf(s_tr[e] - s_rmax[e / K]) : 0.f;
-  __syncthreads();
+  int bmax;
+  const bool fast = bwd_prologue<K, NT>(trans, mylen, s_tr, s_E, s_dT, s_rmax, s_len, reinterpret_cast<int*>(s_x), bmax);
 
   const float* gx = logits + (size_t)row0 * LK;
   const float* gaa = alpha_ws + (size_t)row0 * LK;
@@ -390,22 +252,13 @@ crf_partial_bwd_kernel(const float* __restrict__ logits, const int32_t* __restri
   const int32_t* gm = label_mask + (size_t)row0 * L;
   float* gd = d_logits + (size_t)row0 * LK;
   const int nchunk = (bmax + T - 1) / T;
-  const int nchunk_all = (L + T - 1) / T;
-
-  for (int c = nchunk; c < nchunk_all; ++c) {  // chunks past the CTA's longest row: zero fill
-    const int t0 = c * T;
-    const int ne = min(T, L - t0) * K;
-    for (int idx = tid; idx < NT * Gm::CE; idx += NT) {
-      const int r = idx / Gm::CE, e = idx - r * Gm::CE;
-      if (r < nv && e < ne) gd[(size_t)r * LK + (size_t)t0 * K + e] = 0.f;
-    }
-  }
+  zero_dlogits_tail<K, NT>(gd, nv, L, nchunk);
 
   auto stage = [&](int c, int buf) {
     stage_logits<K, NT>(s_x + buf * NT * P, gx, LK, c * T, L, nv, s_len, vec_logits);
     stage_logits<K, NT>(s_aa + buf * NT * P, gaa, LK, c * T, L, nv, s_len, vec_logits);
     stage_logits<K, NT>(s_af + buf * NT * P, gaf, LK, c * T, L, nv, s_len, vec_logits);
-    stage_masks<NT, T_CHUNK>(s_mask + buf * NT * TAGP, gm, L, c * T, nv, s_len, vec_mask);
+    stage_labels<NT>(s_mask + buf * NT * LABP, gm, L, c * T, nv, s_len, vec_mask);
   };
 #pragma unroll
   for (int s = 0; s < NSTAGE - 1; ++s) {
@@ -424,43 +277,6 @@ crf_partial_bwd_kernel(const float* __restrict__ logits, const int32_t* __restri
     for (int e = 0; e < K * K; ++e) acc[e] = 0.f;
   }
 
-  // beta <- logsumexp_j(trans[i][j] + u[j]); fast: keeps q, mq for the next pair marginal, exact: q = u
-  auto beta_step = [&](float* beta, float* qv, float& mq, const float* u) {
-    if (fast) {
-      float m = u[0];
-#pragma unroll UNR
-      for (int j = 1; j < K; ++j) m = fmaxf(m, u[j]);
-      mq = m;
-#pragma unroll UNR
-      for (int j = 0; j < K; ++j) qv[j] = __expf(u[j] - m);
-#pragma unroll UNR
-      for (int i = 0; i < K; ++i) {
-        float sum = 0.f;
-#pragma unroll UNR
-        for (int j = 0; j < K; ++j) sum = fmaf(s_E[i * K + j], qv[j], sum);
-        beta[i] = m + s_rmax[i] + __logf(sum);
-      }
-    } else {
-      float nb[K];
-#pragma unroll UNR
-      for (int i = 0; i < K; ++i) {
-        float m = -INFINITY;
-#pragma unroll UNR
-        for (int j = 0; j < K; ++j) m = fmaxf(m, s_tr[i * K + j] + u[j]);
-        const float mm = (fabsf(m) <= 3.0e38f) ? m : 0.f;
-        float sum = 0.f;
-#pragma unroll UNR
-        for (int j = 0; j < K; ++j) sum += expf(s_tr[i * K + j] + u[j] - mm);
-        nb[i] = logf(sum) + mm;
-      }
-#pragma unroll UNR
-      for (int i = 0; i < K; ++i) {
-        beta[i] = nb[i];
-        qv[i] = u[i];
-      }
-    }
-  };
-
   for (int it = 0; it < nchunk; ++it) {
     const int c = nchunk - 1 - it;
     const int itn = it + NSTAGE - 1;
@@ -475,7 +291,7 @@ crf_partial_bwd_kernel(const float* __restrict__ logits, const int32_t* __restri
       float* rowx = s_x + buf * NT * P + tid * P;
       const float* rowaa = s_aa + buf * NT * P + tid * P;
       const float* rowaf = s_af + buf * NT * P + tid * P;
-      const int* rowm = s_mask + buf * NT * TAGP + tid * TAGP;
+      const int* rowm = s_mask + buf * NT * LABP + tid * LABP;
 #pragma unroll
       for (int g = T / G - 1; g >= 0; --g) {
         if (t0 + g * G < mylen) {
@@ -536,8 +352,8 @@ crf_partial_bwd_kernel(const float* __restrict__ logits, const int32_t* __restri
                   uf[j] = x[j] + bf[j];
                   ua[j] = ((m >> j) & 1u) ? x[j] + ba[j] : -INFINITY;
                 }
-                beta_step(ba, qa, mqa, ua);
-                beta_step(bf, qf, mqf, uf);
+                beta_step<K>(fast, ba, qa, mqa, qa, ua, s_tr, s_E, s_rmax);
+                beta_step<K>(fast, bf, qf, mqf, qf, uf, s_tr, s_E, s_rmax);
               }
             } else {
 #pragma unroll UNR
@@ -552,55 +368,18 @@ crf_partial_bwd_kernel(const float* __restrict__ logits, const int32_t* __restri
       }
     }
     __syncthreads();
-    {  // coalesced store of this chunk's d_logits (zeros at t >= len)
-      const float* sx = s_x + buf * NT * P;
-      const int ne = min(T, L - t0) * K;
-      if (vec_logits) {
-        for (int idx = tid; idx < NT * Gm::NQ; idx += NT) {
-          const int r = idx / Gm::NQ, qq = idx - r * Gm::NQ;
-          if (r < nv && 4 * qq < ne) {
-            const int valid = (s_len[r] - t0) * K;
-            float4 v = *reinterpret_cast<const float4*>(sx + r * P + 4 * qq);
-            if (4 * qq + 0 >= valid) v.x = 0.f;
-            if (4 * qq + 1 >= valid) v.y = 0.f;
-            if (4 * qq + 2 >= valid) v.z = 0.f;
-            if (4 * qq + 3 >= valid) v.w = 0.f;
-            *reinterpret_cast<float4*>(gd + (size_t)r * LK + (size_t)t0 * K + 4 * qq) = v;
-          }
-        }
-      } else {
-        for (int idx = tid; idx < NT * Gm::CE; idx += NT) {
-          const int r = idx / Gm::CE, e = idx - r * Gm::CE;
-          if (r < nv && e < ne) {
-            const int valid = (s_len[r] - t0) * K;
-            gd[(size_t)r * LK + (size_t)t0 * K + e] = (e < valid) ? sx[r * P + e] : 0.f;
-          }
-        }
-      }
-    }
+    store_dlogits_chunk<K, NT>(gd, s_x + buf * NT * P, s_len, nv, L, t0, vec_logits);
     __syncthreads();
   }
 
-  if constexpr (ACC_REGS) {
-#pragma unroll
-    for (int e = 0; e < K * K; ++e) {
-      float v = (tid < nv) ? gcoef * acc[e] * s_E[e] : 0.f;
-      v = warp_sum(v);
-      if ((tid & 31) == 0 && v != 0.f) atomicAdd(&s_dT[e], v);
-    }
-  }
-  __syncthreads();
-  for (int e = tid; e < K * K; e += NT) {
-    const float v = s_dT[e];
-    if (v != 0.f) atomicAdd(&d_trans[e], v);
-  }
+  flush_dtrans<K, NT>(acc, gcoef, tid < nv, s_dT, s_E, d_trans);
 }
 
 template <int K, int NT>
 int launch_bwd_nt(const float* logits, const int32_t* mask, const int32_t* seq_len, const float* trans,
                   const float* alpha_ws, const float* logz, const float* d_ll, float scale, float* d_logits,
                   float* d_trans, int B, int L, cudaStream_t st) {
-  const size_t smem = partial_bwd_smem_bytes<K, NT>();
+  const size_t smem = bwd_smem_bytes<K, NT, 3>();
   auto kern = crf_partial_bwd_kernel<K, NT>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
@@ -618,11 +397,6 @@ int launch_bwd_nt(const float* logits, const int32_t* mask, const int32_t* seq_l
 // tag j of both recursions, predecessors are exchanged with __shfl_sync, every logsumexp is exact with its own max.
 // The constrained and the free recursion run the same instructions on x_A and x, so a row with every tag allowed stays
 // exactly 0 here too.
-
-template <int K>
-__device__ __forceinline__ bool mask_empty(unsigned m) {
-  return (K < 32 ? (m & ((1u << (K & 31)) - 1u)) : m) == 0u;
-}
 
 template <int K>
 __global__ void __launch_bounds__(32)
@@ -643,9 +417,7 @@ crf_partial_fwd_lanes_kernel(const float* __restrict__ logits, const int32_t* __
     rawlen = seq_len[b];
     len = min(max(rawlen, 1), L);
   }
-  int wmax = len;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
+  const int wmax = lanes_wmax(len);
   __syncwarp();
   float tc[K];
 #pragma unroll
@@ -658,21 +430,6 @@ crf_partial_fwd_lanes_kernel(const float* __restrict__ logits, const int32_t* __
   float* wf = wa != nullptr ? wa + (size_t)B * L * K : nullptr;
   auto ld = [&](int t) -> float { return (seq_ok && tag_ok && t < len) ? xp[(size_t)t * K] : -INFINITY; };
   auto ldm = [&](int t) -> unsigned { return (seq_ok && t < len) ? (unsigned)mp[t] : 0u; };
-  // logsumexp_i(alpha_i + trans[i][j]) over the group, then + x
-  auto step = [&](float a, float x) -> float {
-    float v[K];
-    float m = -INFINITY;
-#pragma unroll
-    for (int i = 0; i < K; ++i) {
-      v[i] = __shfl_sync(0xffffffffu, a, g * GS + i) + tc[i];
-      m = fmaxf(m, v[i]);
-    }
-    const float mm = (fabsf(m) <= 3.0e38f) ? m : 0.f;
-    float sum = 0.f;
-#pragma unroll
-    for (int i = 0; i < K; ++i) sum += __expf(v[i] - mm);
-    return x + (__logf(sum) + mm);
-  };
 
   float af = ld(0);
   unsigned m0 = ldm(0);
@@ -698,8 +455,8 @@ crf_partial_fwd_lanes_kernel(const float* __restrict__ logits, const int32_t* __
       xq[u] = ld(t + PF);
       mq[u] = ldm(t + PF);
       if (t < wmax) {
-        const float nf = step(af, x);
-        const float na = step(aa, ((m >> j) & 1u) ? x : -INFINITY);
+        const float nf = lanes_alpha_step<K>(af, x, tc, g);
+        const float na = lanes_alpha_step<K>(aa, ((m >> j) & 1u) ? x : -INFINITY, tc, g);
         if (t < len) {
           af = tag_ok ? nf : -INFINITY;
           aa = tag_ok ? na : -INFINITY;
@@ -712,17 +469,7 @@ crf_partial_fwd_lanes_kernel(const float* __restrict__ logits, const int32_t* __
       }
     }
   }
-  auto logsum = [&](float a) -> float {
-    float m = a;
-#pragma unroll
-    for (int o = GS / 2; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o, GS));
-    const float mm = (fabsf(m) <= 3.0e38f) ? m : 0.f;
-    float e = tag_ok ? expf(a - mm) : 0.f;
-#pragma unroll
-    for (int o = GS / 2; o > 0; o >>= 1) e += __shfl_xor_sync(0xffffffffu, e, o, GS);
-    return logf(e) + mm;
-  };
-  float lza = logsum(aa), lzf = logsum(af);
+  float lza = lanes_logsumexp<K>(aa, tag_ok), lzf = lanes_logsumexp<K>(af, tag_ok);
   if (j == 0 && seq_ok) {
     if (empty) lza = -INFINITY;
     if (rawlen <= 0) lza = lzf = 0.f;
@@ -760,9 +507,7 @@ crf_partial_bwd_lanes_kernel(const float* __restrict__ logits, const int32_t* __
     gco = (d_ll != nullptr ? d_ll[b] : 1.f) * scale;
     if (!(lza > -INFINITY)) len = 0;  // no path inside the sets: ll = -inf, the row adds no gradient
   }
-  int wmax = len;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
+  const int wmax = lanes_wmax(len);
 
   float tr[K], acc[K];
 #pragma unroll
@@ -811,14 +556,8 @@ crf_partial_bwd_lanes_kernel(const float* __restrict__ logits, const int32_t* __
         const float wf_ = (tag_ok && live) ? x + bf : -INFINITY;
         const float wa_ = (tag_ok && live && ((m >> i) & 1u)) ? x + ba : -INFINITY;
         float vf[K], va[K];
-        float mf = -INFINITY, ma = -INFINITY;
-#pragma unroll
-        for (int jj = 0; jj < K; ++jj) {
-          vf[jj] = tr[jj] + __shfl_sync(0xffffffffu, wf_, g * GS + jj);
-          va[jj] = tr[jj] + __shfl_sync(0xffffffffu, wa_, g * GS + jj);
-          mf = fmaxf(mf, vf[jj]);
-          ma = fmaxf(ma, va[jj]);
-        }
+        const float mf = lanes_gather<K>(vf, wf_, tr, g);
+        const float ma = lanes_gather<K>(va, wa_, tr, g);
         if (live && t >= 1) {
           const float mmf = (fabsf(mf) <= 3.0e38f) ? mf : 0.f;
           const float mma = (fabsf(ma) <= 3.0e38f) ? ma : 0.f;
@@ -871,8 +610,8 @@ int launch_bwd(const float* logits, const int32_t* mask, const int32_t* seq_len,
   if (B <= NER_CRF_SMALL_B)
     return launch_bwd_lanes<K>(logits, mask, seq_len, trans, alpha_ws, logz, d_ll, scale, d_logits, d_trans, B, L, st);
   // 64-thread CTAs need a three-tensor staging ring twice as large: only up to K = 17 does it fit
-  if constexpr (partial_bwd_smem_bytes<K, 64>() <= kMaxSmem) {
-    if (B > ner_num_sms() * 64 * 2)
+  if constexpr (bwd_smem_bytes<K, 64, 3>() <= kMaxSmem) {
+    if (use_cta64(B))
       return launch_bwd_nt<K, 64>(logits, mask, seq_len, trans, alpha_ws, logz, d_ll, scale, d_logits, d_trans, B, L,
                                   st);
   }

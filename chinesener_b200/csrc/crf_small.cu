@@ -14,7 +14,7 @@
 namespace {
 
 using namespace nerdev;
-using crf::Lanes;
+using namespace crf;
 
 constexpr int PF = 4;  // emission prefetch depth (time steps)
 
@@ -120,9 +120,7 @@ crf_loglik_lanes_kernel(const float* __restrict__ logits, const int32_t* __restr
     rawlen = seq_len[b];
     len = min(max(rawlen, 1), L);
   }
-  int wmax = len;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
+  const int wmax = lanes_wmax(len);
   __syncwarp();
 
   float tc[K];
@@ -157,18 +155,7 @@ crf_loglik_lanes_kernel(const float* __restrict__ logits, const int32_t* __restr
       tq[u] = ldtag(t + PF);
       if (t < wmax) {
         // exact logsumexp_i(alpha_i + trans[i][j]) with its own max (tf.reduce_logsumexp)
-        float v[K];
-        float m = -INFINITY;
-#pragma unroll
-        for (int i = 0; i < K; ++i) {
-          v[i] = __shfl_sync(0xffffffffu, a, g * GS + i) + tc[i];
-          m = fmaxf(m, v[i]);
-        }
-        const float mm = (fabsf(m) <= 3.0e38f) ? m : 0.f;
-        float sum = 0.f;
-#pragma unroll
-        for (int i = 0; i < K; ++i) sum += __expf(v[i] - mm);
-        const float na = x + (__logf(sum) + mm);
+        const float na = lanes_alpha_step<K>(a, x, tc, g);
         const float xtag = __shfl_sync(0xffffffffu, x, g * GS + tag);
         if (t < len) {
           a = tag_ok ? na : -INFINITY;
@@ -179,16 +166,8 @@ crf_loglik_lanes_kernel(const float* __restrict__ logits, const int32_t* __restr
       }
     }
   }
-  // logZ = logsumexp_j alpha_j over the group
-  float m = a;
-#pragma unroll
-  for (int o = GS / 2; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o, GS));
-  const float mm = (fabsf(m) <= 3.0e38f) ? m : 0.f;
-  float e = tag_ok ? expf(a - mm) : 0.f;
-#pragma unroll
-  for (int o = GS / 2; o > 0; o >>= 1) e += __shfl_xor_sync(0xffffffffu, e, o, GS);
+  float logz = lanes_logsumexp<K>(a, tag_ok);
   if (j == 0 && seq_ok) {
-    float logz = logf(e) + mm;
     if (rawlen <= 0) {
       logz = 0.f;
       score = 0.f;
@@ -219,9 +198,7 @@ crf_loglik_bwd_lanes_kernel(const float* __restrict__ logits, const int32_t* __r
   const bool seq_ok = b < B;
   const bool tag_ok = i < K;
   const int len = seq_ok ? min(max(seq_len[b], 0), L) : 0;
-  int wmax = len;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
+  const int wmax = lanes_wmax(len);
 
   float tr[K];   // row i of the transition matrix
 #pragma unroll
@@ -275,14 +252,8 @@ crf_loglik_bwd_lanes_kernel(const float* __restrict__ logits, const int32_t* __r
           const float p = __expf(a_t + beta - lz);
           dp[(size_t)t * K] = gco * ((i == tag_t ? 1.f : 0.f) - p);
         }
-        const float w = (tag_ok && live) ? x + beta : -INFINITY;
         float v[K];
-        float m = -INFINITY;
-#pragma unroll
-        for (int jj = 0; jj < K; ++jj) {
-          v[jj] = tr[jj] + __shfl_sync(0xffffffffu, w, g * GS + jj);
-          m = fmaxf(m, v[jj]);
-        }
+        const float m = lanes_gather<K>(v, (tag_ok && live) ? x + beta : -INFINITY, tr, g);
         if (live && t >= 1) {
           const float mm = (fabsf(m) <= 3.0e38f) ? m : 0.f;
           const float am = a_prev - lz;

@@ -27,6 +27,24 @@ TOL = {
     "nt64": (0.0, 2.0, 2e-6),
 }
 
+SMALL_B = 4096          # NER_CRF_SMALL_B, crf_common.cuh
+
+
+def bwd_smem_bytes(K, NT, nf):
+    """bwd_smem_bytes<K, NT, NF> of crf_common.cuh: transitions x3, row maxima, row lengths, and a 2-stage ring of nf
+    8-step float chunks (logits and the forward's alphas) at a row pitch of 8K+4 floats plus label chunks of 12 ints."""
+    return 4 * (3 * ((K * K + 3) & ~3) + 32 + NT + nf * 2 * NT * (8 * K + 4) + 2 * NT * 12)
+
+
+def bwd_route(B, K, nf):
+    """The kernel a CRF loss backward staging nf float tensors (2: ner_crf_loglik_bwd, 3: ner_crf_partial_loglik_bwd)
+    runs for B sequences of K tags: lane per tag up to NER_CRF_SMALL_B, else thread per sequence with 64-thread CTAs
+    above 128 sequences per SM when their shared memory fits, and 32-thread CTAs otherwise."""
+    if B <= SMALL_B:
+        return "lanes"
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    return "nt64" if B > 128 * sms and bwd_smem_bytes(K, 64, nf) <= 227 * 1024 else "nt32"
+
 
 def crf_grad_ref(x, tags, lens, trans, g=None):
     """x [B,L,K], tags [B,L], lens [B], trans [K,K], g [B] (None: all ones).

@@ -1,9 +1,10 @@
 """GPU: the partial-annotation CRF kernels (ner_crf_partial_loglik_fwd / _bwd) against the float64 reference of
 tests/_crf_partial_oracle.py, their exactness properties, and the CRF plugins trained and evaluated on partial labels.
 
-`route` restates the kernels' choice (crf_partial.cu): lane per tag up to 4096 sequences, 64-thread CTAs above 128
-sequences per SM (the backward only while its staging ring fits in shared memory), 32-thread CTAs otherwise.  Every case weights its rows with a random
-d_ll and a scale != 1 and is judged by assert_close_to_ref with the bound of its route.
+`bwd_route` (tests/_crf_grad_oracle.py) restates the kernels' choice: lane per tag up to 4096 sequences, 64-thread CTAs
+above 128 sequences per SM (the backward only while its staging ring fits in shared memory), 32-thread CTAs otherwise.
+Every case weights its rows with a random d_ll and a scale != 1 and is judged by assert_close_to_ref with the bound of
+its route.
 """
 import os
 
@@ -13,7 +14,7 @@ import torch
 
 from chinesener_b200 import autodiff, engine, ops, synthetic, variables
 
-from _crf_grad_oracle import TOL as _ROUTE_TOL, _worst_ratio, grad_errors
+from _crf_grad_oracle import TOL as _ROUTE_TOL, _worst_ratio, bwd_route, grad_errors
 from _crf_partial_oracle import partial_grad_ref, partial_ll_torch
 
 pytestmark = pytest.mark.gpu
@@ -26,25 +27,16 @@ SCALE = 0.75
 # (test_existing_backward_meets_the_same_bound).  At L = 128 a skipped step is > 16 C_T U (test_crf_partial_oracle.py).
 TOL = _ROUTE_TOL
 C_T = 4.0
+NF = 3          # staged float tensors of the backward: logits, alpha_A, alpha (64-thread CTAs fit up to K = 17)
 
 
 def _sms():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-def _bwd_smem_bytes(K, NT):
-    return 4 * (3 * ((K * K + 3) & ~3) + 32 + NT + 3 * 2 * NT * (8 * K + 4) + 2 * NT * 12)
-
-
-def route(B, K):
-    if B <= 4096:                                             # NER_CRF_SMALL_B: lane per tag
-        return "lanes"
-    return "nt64" if B > 128 * _sms() and _bwd_smem_bytes(K, 64) <= 227 * 1024 else "nt32"
-
-
 def assert_close_to_ref(d_logits, d_trans, ref, B, K):
     """-> (d_logits error in u_b, d_trans error in U beyond tol_s S, d_trans error in S)."""
-    rtol, c_dl, tol_s = TOL[route(B, K)]
+    rtol, c_dl, tol_s = TOL[bwd_route(B, K, NF)]
     e_dl, e_s, e_g = grad_errors(d_logits, d_trans, ref.grad, rtol)
     assert e_dl <= c_dl, f"d_logits error {e_dl:.3g} u_b ({e_g:.3e} |g_b|) exceeds {c_dl:.3g} u_b"
     err = (d_trans.to(ref.grad.d_trans.device, torch.float64) - ref.grad.d_trans).abs()
@@ -107,7 +99,7 @@ def _check(x, mask, lens, tr, d_ll, B, K, exact=False):
     past = torch.arange(L, device="cuda")[None, :] >= lens.cuda().clamp(0, L)[:, None]
     assert (d_logits[past] == 0).all()
     e = assert_close_to_ref(d_logits, d_trans, ref, B, K)
-    print(f"B={B} L={L} K={K} route={route(B, K)}: d_logits {e[0]:.3g} u_b, d_trans {e[2]:.2e} S, {e[1]:.3g} U")
+    print(f"B={B} L={L} K={K} route={bwd_route(B, K, NF)}: d_logits {e[0]:.3g} u_b, d_trans {e[2]:.2e} S, {e[1]:.3g} U")
     return ll, d_logits, d_trans
 
 
