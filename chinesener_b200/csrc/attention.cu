@@ -10,31 +10,15 @@
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "mma_tile.cuh"
 
 namespace {
 
 using namespace nerdev;
+using namespace mma_tile;
 
-constexpr int D = 64;
-constexpr int PITCH = D + 8;  // bf16 elements per smem row (144 B)
 constexpr int QT = 64;        // query rows per CTA
 constexpr int KB = 64;        // keys per inner block
-
-__device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void ldmatrix_x2_trans(uint32_t& r0, uint32_t& r1, const void* smem_row) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];"
-               : "=r"(r0), "=r"(r1)
-               : "r"(smem_u32(smem_row)));
-}
-__device__ __forceinline__ uint32_t pack2(float a, float b) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&v);
-}
 
 // attention_probs dropout (training): z(b,h,q,k) in {0, 1/keep} from the shared counter hash; the
 // row sums keep the undropped probabilities (dropout follows the softmax in attention_layer()).
@@ -101,25 +85,14 @@ bert_attention_kernel(const __nv_bfloat16* __restrict__ qkv, const int32_t* __re
 
   constexpr float kLog2e = 1.4426950408889634f;
   float o[8][4];
-#pragma unroll
-  for (int dt = 0; dt < 8; ++dt) o[dt][0] = o[dt][1] = o[dt][2] = o[dt][3] = 0.f;
+  clear_tile(o);
   float m0 = -1e30f, m1 = -1e30f, l0 = 0.f, l1 = 0.f;
 
   if (q0 < L) {
     for (int kb = 0; kb < Lp; kb += KB) {
       float s[8][4];
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt) s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-#pragma unroll
-        for (int nt = 0; nt < 8; ++nt) {
-          const __nv_bfloat16* kp = Ks + (kb + nt * 8 + (lane >> 2)) * PITCH + ks * 16 + cq;
-          const uint32_t b0 = *reinterpret_cast<const uint32_t*>(kp);
-          const uint32_t b1 = *reinterpret_cast<const uint32_t*>(kp + 8);
-          mma_bf16_16816(s[nt], qa[ks], b0, b1);
-        }
-      }
+      clear_tile(s);
+      mma_a_bt(s, qa, Ks, kb, lane, cq);
       float mx0 = -1e30f, mx1 = -1e30f;
 #pragma unroll
       for (int nt = 0; nt < 8; ++nt) {
@@ -170,20 +143,7 @@ bert_attention_kernel(const __nv_bfloat16* __restrict__ qkv, const int32_t* __re
         o[dt][2] *= c1;
         o[dt][3] *= c1;
       }
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        uint32_t pa[4];
-        pa[0] = pack2(s[2 * kk][0], s[2 * kk][1]);
-        pa[1] = pack2(s[2 * kk][2], s[2 * kk][3]);
-        pa[2] = pack2(s[2 * kk + 1][0], s[2 * kk + 1][1]);
-        pa[3] = pack2(s[2 * kk + 1][2], s[2 * kk + 1][3]);
-#pragma unroll
-        for (int dt = 0; dt < 8; ++dt) {
-          uint32_t b0, b1;
-          ldmatrix_x2_trans(b0, b1, Vs + (kb + kk * 16 + (lane & 15)) * PITCH + dt * 8);
-          mma_bf16_16816(o[dt], pa, b0, b1);
-        }
-      }
+      mma_p_b(o, s, Vs, kb, lane);
     }
     l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
     l0 += __shfl_xor_sync(0xffffffffu, l0, 2);

@@ -12,71 +12,14 @@
 //           dV = P^T dO,  dK = scale * dS^T Q                               (no cross-warp reduction)
 // Longer sequences, where the head does not fit in shared memory, take the key-tiled kernels further down.
 #include "common.cuh"
+#include "mma_tile.cuh"
 
 namespace {
 
 using namespace nerdev;
+using namespace mma_tile;
 
-constexpr int D = 64;
-constexpr int PITCH = D + 8;  // bf16 per smem row (144 B): conflict-free fragment loads / ldmatrix
-constexpr int NW = 8;         // warps per CTA
-
-__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void ldsm_x2_trans(uint32_t& r0, uint32_t& r1, const void* p) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(smem_u32(p)));
-}
-__device__ __forceinline__ uint32_t pack2(float a, float b) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&v);
-}
-__device__ __forceinline__ uint32_t lds32(const __nv_bfloat16* p) { return *reinterpret_cast<const uint32_t*>(p); }
-
-// A-operand fragments (16 rows x 64 k) of rows r0 / r1 = r0 + 8 of a [rows][PITCH] smem matrix
-__device__ __forceinline__ void load_a_frags(uint32_t (&a)[4][4], const __nv_bfloat16* base, int r0, int cq) {
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks) {
-    a[ks][0] = lds32(base + r0 * PITCH + ks * 16 + cq);
-    a[ks][1] = lds32(base + (r0 + 8) * PITCH + ks * 16 + cq);
-    a[ks][2] = lds32(base + r0 * PITCH + ks * 16 + 8 + cq);
-    a[ks][3] = lds32(base + (r0 + 8) * PITCH + ks * 16 + 8 + cq);
-  }
-}
-// acc[nt] (16 x 64 cols in 8 n-tiles) = A(16 x 64) · Bm^T where Bm is a [cols][PITCH] smem matrix (rows = n index)
-__device__ __forceinline__ void mma_a_bt(float (&acc)[8][4], const uint32_t (&a)[4][4], const __nv_bfloat16* Bm, int n0,
-                                         int lane, int cq) {
-#pragma unroll
-  for (int nt = 0; nt < 8; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks)
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt) {
-      const __nv_bfloat16* p = Bm + (n0 + nt * 8 + (lane >> 2)) * PITCH + ks * 16 + cq;
-      mma16816(acc[nt], a[ks], lds32(p), lds32(p + 8));
-    }
-}
-// out[dt] (16 x 64 dims) += P(16 x 64, C-fragment layout in p) · Bm[n0 .. n0+64][dims]
-__device__ __forceinline__ void mma_p_b(float (&out)[8][4], const float (&p)[8][4], const __nv_bfloat16* Bm, int n0,
-                                        int lane) {
-#pragma unroll
-  for (int kk = 0; kk < 4; ++kk) {
-    uint32_t pa[4];
-    pa[0] = pack2(p[2 * kk][0], p[2 * kk][1]);
-    pa[1] = pack2(p[2 * kk][2], p[2 * kk][3]);
-    pa[2] = pack2(p[2 * kk + 1][0], p[2 * kk + 1][1]);
-    pa[3] = pack2(p[2 * kk + 1][2], p[2 * kk + 1][3]);
-#pragma unroll
-    for (int dt = 0; dt < 8; ++dt) {
-      uint32_t b0, b1;
-      ldsm_x2_trans(b0, b1, Bm + (n0 + kk * 16 + (lane & 15)) * PITCH + dt * 8);
-      mma16816(out[dt], pa, b0, b1);
-    }
-  }
-}
+constexpr int NW = 8;  // warps per CTA
 
 // Same attention_probs dropout factor as the forward kernel (attention.cu): z in {0, 1/keep}.
 // With O = (P o z) V:  dV = (P o z)^T dO,  dS = P o (z o dP - D),  D = rowsum(dO o O) unchanged.
@@ -176,6 +119,7 @@ bert_attention_bwd_kernel(const __nv_bfloat16* __restrict__ qkv, const int32_t* 
     float m0 = -1e30f, m1 = -1e30f, l0 = 0.f, l1 = 0.f;
     for (int kb = 0; kb < Lp; kb += 64) {
       float s[8][4];
+      clear_tile(s);
       mma_a_bt(s, qa, Ks, kb, lane, cq);
       float mx0 = -1e30f, mx1 = -1e30f;
 #pragma unroll
@@ -215,10 +159,11 @@ bert_attention_bwd_kernel(const __nv_bfloat16* __restrict__ qkv, const int32_t* 
     }
     // pass 2: dS and dQ
     float dq[8][4];
-#pragma unroll
-    for (int dt = 0; dt < 8; ++dt) dq[dt][0] = dq[dt][1] = dq[dt][2] = dq[dt][3] = 0.f;
+    clear_tile(dq);
     for (int kb = 0; kb < Lp; kb += 64) {
       float s[8][4], dp[8][4];
+      clear_tile(s);
+      clear_tile(dp);
       mma_a_bt(s, qa, Ks, kb, lane, cq);
       mma_a_bt(dp, da, Vs, kb, lane, cq);
 #pragma unroll
@@ -259,13 +204,12 @@ bert_attention_bwd_kernel(const __nv_bfloat16* __restrict__ qkv, const int32_t* 
     load_a_frags(va, Vs, k0, cq);
     const float ma0 = s_madd[k0], ma1 = s_madd[k1];
     float dk[8][4], dv[8][4];
-#pragma unroll
-    for (int dt = 0; dt < 8; ++dt) {
-      dk[dt][0] = dk[dt][1] = dk[dt][2] = dk[dt][3] = 0.f;
-      dv[dt][0] = dv[dt][1] = dv[dt][2] = dv[dt][3] = 0.f;
-    }
+    clear_tile(dk);
+    clear_tile(dv);
     for (int qb = 0; qb < Lp; qb += 64) {
       float st[8][4], dpt[8][4];
+      clear_tile(st);
+      clear_tile(dpt);
       mma_a_bt(st, ka, Qs, qb, lane, cq);   // S^T  = K Q^T      (rows: keys, cols: queries)
       mma_a_bt(dpt, va, Os, qb, lane, cq);  // dP^T = V dO^T
 #pragma unroll
@@ -412,6 +356,7 @@ bert_attention_bwd_stats_kernel(const __nv_bfloat16* __restrict__ qkv, const int
       cp_async_commit();
     }
     float s[8][4];
+    clear_tile(s);
     mma_a_bt(s, qa, Ks[buf], 0, lane, cq);
     float mx0 = -1e30f, mx1 = -1e30f;
 #pragma unroll
@@ -503,11 +448,8 @@ bert_attention_bwd_dkdv_kernel(const __nv_bfloat16* __restrict__ qkv, const int3
   load_a_frags(ka, Ks, kl0, cq);
   load_a_frags(va, Vs, kl0, cq);
   float dk[8][4], dv[8][4];
-#pragma unroll
-  for (int dt = 0; dt < 8; ++dt) {
-    dk[dt][0] = dk[dt][1] = dk[dt][2] = dk[dt][3] = 0.f;
-    dv[dt][0] = dv[dt][1] = dv[dt][2] = dv[dt][3] = 0.f;
-  }
+  clear_tile(dk);
+  clear_tile(dv);
   for (int t = 0; t < nqt; ++t) {
     const int buf = t & 1;
     if (t + 1 < nqt) {
@@ -518,6 +460,8 @@ bert_attention_bwd_dkdv_kernel(const __nv_bfloat16* __restrict__ qkv, const int3
     const __nv_bfloat16* Ob = Os + buf * TILE;
     const float2* stb = s_st + buf * TQ;
     float st[8][4], dpt[8][4];
+    clear_tile(st);
+    clear_tile(dpt);
     mma_a_bt(st, ka, Qb, 0, lane, cq);   // S^T  = K Q^T      (rows: keys, cols: queries)
     mma_a_bt(dpt, va, Ob, 0, lane, cq);  // dP^T = V dO^T
 #pragma unroll
@@ -613,8 +557,7 @@ bert_attention_bwd_dq_kernel(const __nv_bfloat16* __restrict__ qkv, const int32_
   load_a_frags(qa, Qs, rl0, cq);
   load_a_frags(da, Os, rl0, cq);
   float dq[8][4];
-#pragma unroll
-  for (int dt = 0; dt < 8; ++dt) dq[dt][0] = dq[dt][1] = dq[dt][2] = dq[dt][3] = 0.f;
+  clear_tile(dq);
   for (int t = 0; t < nkt; ++t) {
     const int buf = t & 1;
     if (t + 1 < nkt) {
@@ -625,6 +568,8 @@ bert_attention_bwd_dq_kernel(const __nv_bfloat16* __restrict__ qkv, const int32_
     const __nv_bfloat16* Vb = Vs + buf * TILE;
     const float* mb = s_madd + buf * TQ;
     float s[8][4], dp[8][4];
+    clear_tile(s);
+    clear_tile(dp);
     mma_a_bt(s, qa, Kb, 0, lane, cq);
     mma_a_bt(dp, da, Vb, 0, lane, cq);
 #pragma unroll

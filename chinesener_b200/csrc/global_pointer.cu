@@ -17,74 +17,21 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "mma_tile.cuh"
+#include "span_common.cuh"
 
 namespace {
 
 using namespace nerdev;
+using namespace mma_tile;
+using namespace span;
 
-constexpr int D = 64;
 constexpr int kMaxTypes = 32;
 constexpr int kMaxLen = 512;     // i, j <= 510 fit the 9-bit fields of the decode's priority key
+static_assert(kMaxLen <= kDecodeRows, "the decode holds a whole sentence in shared memory");
 constexpr int kTile = 64;        // query / key tile
-constexpr int PITCH = D + 8;     // bf16 per smem row (144 B): conflict-free fragment loads / ldmatrix
 constexpr int kThreads = 128;    // 4 warps x 16 rows
 constexpr float kQScale = 0.125f;   // 1 / sqrt(D), exact in every format
-
-__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void ldsm_x2_trans(uint32_t& r0, uint32_t& r1, const void* p) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(smem_u32(p)));
-}
-__device__ __forceinline__ uint32_t pack2(float a, float b) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&v);
-}
-__device__ __forceinline__ uint32_t lds32(const __nv_bfloat16* p) { return *reinterpret_cast<const uint32_t*>(p); }
-
-// A-operand fragments (16 rows x 64 k) of rows r0 / r0 + 8 of a [rows][PITCH] smem matrix
-__device__ __forceinline__ void load_a_frags(uint32_t (&a)[4][4], const __nv_bfloat16* base, int r0, int cq) {
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks) {
-    a[ks][0] = lds32(base + r0 * PITCH + ks * 16 + cq);
-    a[ks][1] = lds32(base + (r0 + 8) * PITCH + ks * 16 + cq);
-    a[ks][2] = lds32(base + r0 * PITCH + ks * 16 + 8 + cq);
-    a[ks][3] = lds32(base + (r0 + 8) * PITCH + ks * 16 + 8 + cq);
-  }
-}
-// acc[nt] (16 x 64 cols in 8 n-tiles) += A(16 x 64) . Bm^T, Bm a [64][PITCH] smem matrix (rows = n index)
-__device__ __forceinline__ void mma_acc_bt(float (&acc)[8][4], const uint32_t (&a)[4][4], const __nv_bfloat16* Bm,
-                                           int lane, int cq) {
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks)
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt) {
-      const __nv_bfloat16* p = Bm + (nt * 8 + (lane >> 2)) * PITCH + ks * 16 + cq;
-      mma16816(acc[nt], a[ks], lds32(p), lds32(p + 8));
-    }
-}
-// out[dt] (16 x 64 dims) += P(16 x 64, C-fragment layout) . Bm[0 .. 64][dims]
-__device__ __forceinline__ void mma_p_b(float (&out)[8][4], const float (&p)[8][4], const __nv_bfloat16* Bm, int lane) {
-#pragma unroll
-  for (int kk = 0; kk < 4; ++kk) {
-    uint32_t pa[4];
-    pa[0] = pack2(p[2 * kk][0], p[2 * kk][1]);
-    pa[1] = pack2(p[2 * kk][2], p[2 * kk][3]);
-    pa[2] = pack2(p[2 * kk + 1][0], p[2 * kk + 1][1]);
-    pa[3] = pack2(p[2 * kk + 1][2], p[2 * kk + 1][3]);
-#pragma unroll
-    for (int dt = 0; dt < 8; ++dt) {
-      uint32_t b0, b1;
-      ldsm_x2_trans(b0, b1, Bm + (kk * 16 + (lane & 15)) * PITCH + dt * 8);
-      mma16816(out[dt], pa, b0, b1);
-    }
-  }
-}
-
-__device__ __forceinline__ int clamp_len(int32_t v, int L) { return min(max((int)v, 0), L); }
 
 // Row layout of sentence b: first row and row count (padded b*L, L rows; packed cu[b], cu[b+1] - cu[b] rows)
 struct Rows {
@@ -188,12 +135,11 @@ gp_tile_kernel(const __nv_bfloat16* __restrict__ hi, const __nv_bfloat16* __rest
     cp_async_wait<0>();
     __syncthreads();
     float acc[8][4];
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
-    mma_acc_bt(acc, qa, sm.b_hi, lane, cq);
+    clear_tile(acc);
+    mma_a_bt(acc, qa, sm.b_hi, 0, lane, cq);
     if constexpr (kSplit) {
-      mma_acc_bt(acc, qa, sm.b_lo, lane, cq);
-      mma_acc_bt(acc, qla, sm.b_hi, lane, cq);
+      mma_a_bt(acc, qa, sm.b_lo, 0, lane, cq);
+      mma_a_bt(acc, qla, sm.b_hi, 0, lane, cq);
     }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -335,8 +281,7 @@ gp_bwd_kernel(const __nv_bfloat16* __restrict__ rot, const int32_t* __restrict__
   const int own_side = kKeys ? 1 : 0;
   const int ra = warp * 16 + (lane >> 2);
   float out[8][4];
-#pragma unroll
-  for (int dt = 0; dt < 8; ++dt) out[dt][0] = out[dt][1] = out[dt][2] = out[dt][3] = 0.f;
+  clear_tile(out);
   if (m >= 1 && o0 <= m) {
     const float ln = __ldg(lse + 2 * bt), lp = __ldg(lse + 2 * bt + 1);
     stage_tile(sm.a_hi, rot, rw.base, T, t, own_side, o0, len - 1, tid);
@@ -361,9 +306,8 @@ gp_bwd_kernel(const __nv_bfloat16* __restrict__ rot, const int32_t* __restrict__
       cp_async_wait<0>();
       __syncthreads();
       float acc[8][4];
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
-      mma_acc_bt(acc, oa, sm.b_hi, lane, cq);
+      clear_tile(acc);
+      mma_a_bt(acc, oa, sm.b_hi, 0, lane, cq);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = o0 + ra + 8 * h;                // own index: i (queries) or j (keys)
@@ -381,7 +325,7 @@ gp_bwd_kernel(const __nv_bfloat16* __restrict__ rot, const int32_t* __restrict__
             acc[nt][2 * h + e] = ds;
           }
       }
-      mma_p_b(out, acc, sm.b_hi, lane);
+      mma_p_b(out, acc, sm.b_hi, 0, lane);
     }
   }
 #pragma unroll
@@ -477,133 +421,31 @@ gp_targets_kernel(const int32_t* __restrict__ labels, const int32_t* __restrict_
   for (int e = threadIdx.x; e < T * L; e += 256) {
     const int t = e / L, s = e - t * L;
     const int tb = __ldg(type_tag + 2 * t), ti = __ldg(type_tag + 2 * t + 1);
-    int r = -1;
-    if (s < len && y[s] == tb) {
-      r = s;
-      while (r + 1 < len && y[r + 1] == ti) ++r;
-    }
-    span_end[((size_t)b * T + t) * L + s] = r;
+    span_end[((size_t)b * T + t) * L + s] = s < len && y[s] == tb ? run_end(y, s, len, ti) : -1;
   }
 }
 
-// Priority of span (t, i, j) with s > 0: higher s first, then lower type, lower start, lower end.
-__device__ __forceinline__ unsigned long long span_key(float zz, int t, int i, int j) {
-  return ((unsigned long long)__float_as_uint(zz) << 32) | ((unsigned)(31 - t) << 18) | ((unsigned)(511 - i) << 9) |
-         (unsigned)(511 - j);
-}
+// Candidates of the decode: every type at every (i, j).
+struct AllTypes {
+  int T;
+  __device__ __forceinline__ bool live(int) const { return true; }
+  template <class F>
+  __device__ __forceinline__ void for_each(int, int, F&& f) const {
+    for (int t = 0; t < T; ++t)
+      if (!f(t)) return;
+  }
+};
 
-// Decode: one CTA per sentence over the candidate scores.  The span list ordered by (start, end, type), then the greedy
-// non-overlapping projection into pred_ids (the loop of ner_mrc_span_decode with every type a start and an end
-// everywhere): each row i keeps the key of its best free span; keeping [a, e] clears rows a..e and rescans only the rows
-// before a whose best span reached into [a, e].
-__global__ void __launch_bounds__(256)
+// Decode: one CTA per sentence over the candidate scores (span_common.cuh).
+__global__ void __launch_bounds__(kDecodeThreads)
 gp_decode_kernel(const float* __restrict__ sc, const int32_t* __restrict__ seq_len, const int32_t* __restrict__ type_tag,
                  int T, int L, int o_id, int cls_id, int sep_id, int cap, int32_t* __restrict__ pred_ids,
                  int32_t* __restrict__ spans, float* __restrict__ probs, int32_t* __restrict__ span_counts) {
-  __shared__ int32_t cnt[kMaxLen + 1], tag[kMaxLen];
-  __shared__ unsigned long long rowkey[kMaxLen];
-  __shared__ uint8_t occ[kMaxLen];
-  const int b = blockIdx.x, tid = threadIdx.x;
-  const int len = clamp_len(__ldg(seq_len + b), L), m = len - 2;
-  auto score = [&](int t, int i, int j) { return sc[(((size_t)b * T + t) * L + i) * L + j]; };
-  for (int s = tid; s < L; s += 256) {
-    tag[s] = o_id;
-    occ[s] = 0;
-    rowkey[s] = 0ull;
-    cnt[s] = 0;
-  }
-  __syncthreads();
-  for (int i = 1 + tid; i <= m; i += 256) {
-    int n = 0;
-    unsigned long long best = 0ull;
-    for (int j = i; j <= m; ++j)
-      for (int t = 0; t < T; ++t) {
-        const float zz = score(t, i, j);
-        if (zz > 0.f) {
-          ++n;
-          const unsigned long long key = span_key(zz, t, i, j);
-          best = key > best ? key : best;
-        }
-      }
-    cnt[i] = n;
-    rowkey[i] = best;
-  }
-  __syncthreads();
-  if (tid == 0) {
-    int run = 0;
-    for (int i = 0; i < L; ++i) {
-      const int c = cnt[i];
-      cnt[i] = run;
-      run += c;
-    }
-    span_counts[b] = run;
-    cnt[L] = run;
-  }
-  __syncthreads();
-  for (int o = cnt[L] + tid; o < cap; o += 256) {
-    spans[(size_t)b * cap + o] = 0;
-    probs[(size_t)b * cap + o] = 0.f;
-  }
-  for (int i = 1 + tid; i <= m; i += 256) {
-    int o = cnt[i];
-    for (int j = i; j <= m && o < cap; ++j)
-      for (int t = 0; t < T && o < cap; ++t) {
-        const float zz = score(t, i, j);
-        if (zz > 0.f) {
-          spans[(size_t)b * cap + o] = i | (j + 1) << 12 | t << 24;
-          probs[(size_t)b * cap + o] = 1.f / (1.f + expf(-zz));
-          ++o;
-        }
-      }
-  }
-  if (tid < 32) {
-    const int lane = tid;
-    for (;;) {
-      unsigned long long best = 0ull;
-      for (int i = 1 + lane; i <= m; i += 32) best = rowkey[i] > best ? rowkey[i] : best;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const unsigned long long v = __shfl_xor_sync(0xffffffffu, best, o);
-        best = v > best ? v : best;
-      }
-      if (best == 0ull) break;
-      const int t = 31 - (int)((best >> 18) & 31), a = 511 - (int)((best >> 9) & 511), e = 511 - (int)(best & 511);
-      const int tb = __ldg(type_tag + 2 * t), tI = __ldg(type_tag + 2 * t + 1);
-      for (int q = a + lane; q <= e; q += 32) {
-        occ[q] = 1;
-        tag[q] = q == a ? tb : tI;
-        rowkey[q] = 0ull;
-      }
-      __syncwarp();
-      for (int i = 1 + lane; i < a; i += 32) {
-        const unsigned long long key = rowkey[i];
-        if (key == 0ull || 511 - (int)(key & 511) < a) continue;
-        unsigned long long nb = 0ull;
-        for (int j = i; j <= m && !occ[j]; ++j)
-          for (int tt = 0; tt < T; ++tt) {
-            const float zz = score(tt, i, j);
-            if (zz > 0.f) {
-              const unsigned long long k2 = span_key(zz, tt, i, j);
-              nb = k2 > nb ? k2 : nb;
-            }
-          }
-        rowkey[i] = nb;
-      }
-      __syncwarp();
-    }
-  }
-  __syncthreads();
-  for (int s = tid; s < L; s += 256) {
-    int out;
-    if (s >= len) out = 0;
-    else if (s == 0) out = cls_id;
-    else if (s == len - 1) out = sep_id;
-    else out = tag[s];
-    pred_ids[(size_t)b * L + s] = out;
-  }
+  __builtin_assume(T >= 1);   // check_shape; keeps the empty-type test out of the (i, j) loops
+  const int len = clamp_len(__ldg(seq_len + blockIdx.x), L);
+  greedy_span_decode(AllTypes{T}, sc, T, L, len, type_tag, o_id, cls_id, sep_id, cap, pred_ids, spans, probs,
+                     span_counts);
 }
-
-bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15u) == 0; }
 
 // shared shape checks: 0 or the status to return
 int check_shape(int B, int T, int L) {
@@ -729,7 +571,7 @@ extern "C" int ner_gp_decode(const void* rot_hi, const void* rot_lo, const int32
     gp_tile_kernel<false, true><<<grid, kThreads, 0, st>>>(hi, lo, seq_len, cu_seqlens, nullptr, T, L, nullptr, sc);
   const int rc = ner_launch_status();
   if (rc != NER_OK) return rc;
-  gp_decode_kernel<<<B, 256, 0, st>>>(sc, seq_len, type_tag, T, L, o_id, cls_id, sep_id, cap, pred_ids, spans, span_probs,
-                                      span_counts);
+  gp_decode_kernel<<<B, kDecodeThreads, 0, st>>>(sc, seq_len, type_tag, T, L, o_id, cls_id, sep_id, cap, pred_ids, spans,
+                                                 span_probs, span_counts);
   return ner_launch_status();
 }

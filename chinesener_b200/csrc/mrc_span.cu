@@ -12,6 +12,7 @@
 // atomics).  The decode runs the forward tile kernel on the compacted start x end lists only, so PREDICT never evaluates the
 // whole triangle unless every position is a start and an end.
 #include "common.cuh"
+#include "span_common.cuh"
 
 namespace {
 
@@ -20,9 +21,11 @@ using nerdev::cp_async_commit;
 using nerdev::cp_async_wait;
 using nerdev::hash3;
 using nerdev::keep_threshold;
+using namespace span;
 
 constexpr int kMaxTypes = 32;
 constexpr int kMaxLen = 511;      // the pair bound: a key packs i and j in 9 bits each
+static_assert(kMaxLen <= kDecodeRows, "the decode holds a whole pair in shared memory");
 constexpr int kMaxInter = 4096;
 constexpr int kTile = 32;         // i x j tile of the match kernel
 constexpr int kKc = 32;           // k-chunk staged per step
@@ -53,8 +56,6 @@ __device__ __forceinline__ bool span_keep(uint32_t seed_lo, uint32_t seed_hi, in
                                           uint32_t thr) {
   return hash3(seed_lo, seed_hi ^ (uint32_t)(p * L + i), (uint32_t)(j * I + k)) < thr;
 }
-
-__device__ __forceinline__ int clamp_len(int32_t v, int L) { return min(max((int)v, 0), L); }
 
 struct TileSmem;
 __device__ __forceinline__ void stage_chunk(TileSmem& s, const float* __restrict__ uv, int ld, const float* __restrict__ b1,
@@ -399,13 +400,8 @@ span_targets_kernel(const int32_t* __restrict__ labels, const int32_t* __restric
   __syncthreads();
   for (int s = threadIdx.x; s < L; s += 128) {
     const bool st = s < len && y[s] == 1;
-    int r = -1;
-    if (st) {
-      r = s;
-      while (r + 1 < len && y[r + 1] == 2) ++r;
-    }
     start_y[base + s] = st ? 1 : 0;
-    span_end[base + s] = r;
+    span_end[base + s] = st ? run_end(y, s, len, 2) : -1;
   }
   __syncthreads();
   for (int s = threadIdx.x; s < L; s += 128) {
@@ -455,27 +451,32 @@ span_flags_kernel(const float* __restrict__ start_logits, const float* __restric
   }
 }
 
-// Priority of span (t, i, j) with z > 0: higher z first, then lower type, lower start, lower end.
-__device__ __forceinline__ unsigned long long span_key(float zz, int t, int i, int j) {
-  return ((unsigned long long)__float_as_uint(zz) << 32) | ((unsigned)(31 - t) << 18) | ((unsigned)(511 - i) << 9) |
-         (unsigned)(511 - j);
-}
+// Candidates of the decode: the types t with position i a start and j an end of t.
+struct StartEndCandidates {
+  const uint32_t* smask;
+  const uint32_t* emask;
+  __device__ __forceinline__ bool live(int i) const { return smask[i] != 0; }
+  template <class F>
+  __device__ __forceinline__ void for_each(int i, int j, F&& f) const {
+    uint32_t bits = smask[i] & emask[j];
+    while (bits) {
+      const int t = __ffs(bits) - 1;
+      bits &= bits - 1;
+      if (!f(t)) return;
+    }
+  }
+};
 
-// Decode 3: one CTA per sentence.  The span list ordered by (start, end, type), then the greedy non-overlapping projection
-// into pred_ids: repeatedly keep the best remaining span that overlaps nothing kept.  Each row i keeps the key of its best
-// free span; keeping [a, b] clears rows a..b and rescans only the rows before a whose best span reached into [a, b].
-__global__ void __launch_bounds__(256)
+// Decode 3: one CTA per sentence: the start / end bits of every position, then span_common.cuh's greedy decode.
+__global__ void __launch_bounds__(kDecodeThreads)
 span_decode_kernel(const float* __restrict__ start_logits, const float* __restrict__ end_logits,
                    const float* __restrict__ zf, const int32_t* __restrict__ seq_len, const int32_t* __restrict__ type_tag,
                    int T, int L, int o_id, int cls_id, int sep_id, int cap, int32_t* __restrict__ pred_ids,
                    int32_t* __restrict__ spans, float* __restrict__ probs, int32_t* __restrict__ span_counts) {
   __shared__ uint32_t smask[kMaxLen + 1], emask[kMaxLen + 1];
-  __shared__ int32_t cnt[kMaxLen + 1], tag[kMaxLen + 1];
-  __shared__ unsigned long long rowkey[kMaxLen + 1];
-  __shared__ uint8_t occ[kMaxLen + 1];
-  const int b = blockIdx.x, tid = threadIdx.x;
+  const int b = blockIdx.x;
   const int len = clamp_len(__ldg(seq_len + b), L), m = len - 2;
-  for (int s = tid; s < L; s += 256) {
+  for (int s = threadIdx.x; s < L; s += kDecodeThreads) {
     uint32_t sm = 0, em = 0;
     if (s >= 1 && s <= m) {
 #pragma unroll 1
@@ -487,121 +488,10 @@ span_decode_kernel(const float* __restrict__ start_logits, const float* __restri
     }
     smask[s] = sm;
     emask[s] = em;
-    tag[s] = o_id;
-    occ[s] = 0;
-    rowkey[s] = 0ull;
-    cnt[s] = 0;
   }
-  __syncthreads();
-  for (int i = 1 + tid; i <= m; i += 256) {
-    const uint32_t si = smask[i];
-    int n = 0;
-    unsigned long long best = 0ull;
-    if (si) {
-      for (int j = i; j <= m; ++j) {
-        uint32_t bits = si & emask[j];
-        while (bits) {
-          const int t = __ffs(bits) - 1;
-          bits &= bits - 1;
-          const float zz = __ldg(zf + (((size_t)b * T + t) * L + i) * L + j);
-          if (zz > 0.f) {
-            ++n;
-            const unsigned long long key = span_key(zz, t, i, j);
-            best = key > best ? key : best;
-          }
-        }
-      }
-    }
-    cnt[i] = n;
-    rowkey[i] = best;
-  }
-  __syncthreads();
-  if (tid == 0) {
-    int run = 0;
-    for (int i = 0; i < L; ++i) {
-      const int c = cnt[i];
-      cnt[i] = run;
-      run += c;
-    }
-    span_counts[b] = run;
-    cnt[L] = run;
-  }
-  __syncthreads();
-  for (int o = cnt[L] + tid; o < cap; o += 256) {
-    spans[(size_t)b * cap + o] = 0;
-    probs[(size_t)b * cap + o] = 0.f;
-  }
-  for (int i = 1 + tid; i <= m; i += 256) {
-    const uint32_t si = smask[i];
-    int o = cnt[i];
-    if (!si || o >= cap) continue;
-    for (int j = i; j <= m && o < cap; ++j) {
-      uint32_t bits = si & emask[j];
-      while (bits && o < cap) {
-        const int t = __ffs(bits) - 1;
-        bits &= bits - 1;
-        const float zz = __ldg(zf + (((size_t)b * T + t) * L + i) * L + j);
-        if (zz > 0.f) {
-          spans[(size_t)b * cap + o] = i | (j + 1) << 12 | t << 24;
-          probs[(size_t)b * cap + o] = 1.f / (1.f + expf(-zz));
-          ++o;
-        }
-      }
-    }
-  }
-  if (tid < 32) {
-    const int lane = tid;
-    for (;;) {
-      unsigned long long best = 0ull;
-      for (int i = 1 + lane; i <= m; i += 32) best = rowkey[i] > best ? rowkey[i] : best;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const unsigned long long v = __shfl_xor_sync(0xffffffffu, best, o);
-        best = v > best ? v : best;
-      }
-      if (best == 0ull) break;
-      const int t = 31 - (int)((best >> 18) & 31), a = 511 - (int)((best >> 9) & 511), e = 511 - (int)(best & 511);
-      const int tb = __ldg(type_tag + 2 * t), tI = __ldg(type_tag + 2 * t + 1);
-      for (int q = a + lane; q <= e; q += 32) {
-        occ[q] = 1;
-        tag[q] = q == a ? tb : tI;
-        rowkey[q] = 0ull;
-      }
-      __syncwarp();
-      for (int i = 1 + lane; i < a; i += 32) {
-        const unsigned long long key = rowkey[i];
-        if (key == 0ull || 511 - (int)(key & 511) < a) continue;
-        unsigned long long nb = 0ull;
-        const uint32_t si = smask[i];
-        for (int j = i; j <= m && !occ[j]; ++j) {
-          uint32_t bits = si & emask[j];
-          while (bits) {
-            const int tt = __ffs(bits) - 1;
-            bits &= bits - 1;
-            const float zz = __ldg(zf + (((size_t)b * T + tt) * L + i) * L + j);
-            if (zz > 0.f) {
-              const unsigned long long k2 = span_key(zz, tt, i, j);
-              nb = k2 > nb ? k2 : nb;
-            }
-          }
-        }
-        rowkey[i] = nb;
-      }
-      __syncwarp();
-    }
-  }
-  __syncthreads();
-  for (int s = tid; s < L; s += 256) {
-    int out;
-    if (s >= len) out = 0;
-    else if (s == 0) out = cls_id;
-    else if (s == len - 1) out = sep_id;
-    else out = tag[s];
-    pred_ids[(size_t)b * L + s] = out;
-  }
+  greedy_span_decode(StartEndCandidates{smask, emask}, zf, T, L, len, type_tag, o_id, cls_id, sep_id, cap, pred_ids,
+                     spans, probs, span_counts);
 }
-
-bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15u) == 0; }
 
 // shared checks of the match entry points: 0 or the status to return
 int check_match_shape(int P, int L, int I, int ld_uv) {
@@ -742,7 +632,7 @@ extern "C" int ner_mrc_span_decode(const float* start_logits, const float* end_l
   span_tile_kernel<false, true><<<dim3(tile_count(L), P), kTileThreads, 0, st>>>(
       uv, ld_uv, b1, w2, b2, seq_len, T, nullptr, lists, counts, L, I, 1.f, 0, zf, nullptr);
   if ((rc = ner_launch_status()) != NER_OK) return rc;
-  span_decode_kernel<<<B, 256, 0, st>>>(start_logits, end_logits, zf, seq_len, type_tag, T, L, o_id, cls_id, sep_id, cap,
-                                        pred_ids, spans, span_probs, span_counts);
+  span_decode_kernel<<<B, kDecodeThreads, 0, st>>>(start_logits, end_logits, zf, seq_len, type_tag, T, L, o_id, cls_id,
+                                                   sep_id, cap, pred_ids, spans, span_probs, span_counts);
   return ner_launch_status();
 }
