@@ -24,22 +24,12 @@
 // weights are stored in the order the lanes consume them, so every step of a dot product is one conflict-free LDS.128.
 #include <cooperative_groups.h>
 
-#include "bigru.cuh"
 #include "common.cuh"
-#include "dsmem.cuh"
+#include "rnn_cluster.cuh"
 
 namespace cg = cooperative_groups;
 
 namespace {
-
-// ex2.approx-based forms, as in bilstm.cu (abs. error ~1e-7, far inside the 1e-4 parity bar).
-__device__ __forceinline__ float sigmoidf_(float x) { return __fdividef(1.f, 1.f + __expf(-x)); }
-
-template <int ACT>
-__device__ __forceinline__ float actf(float x) {
-  if (ACT == 1) return fmaxf(x, 0.f);
-  return 1.f - __fdividef(2.f, 1.f + __expf(2.f * x));   // tanh(x); saturates correctly for |x| large
-}
 
 template <int R, int ACT>
 __global__ void __launch_bounds__(512, 1)
@@ -96,7 +86,7 @@ bigru_rec_kernel(const float* __restrict__ xproj, const float* __restrict__ wh_f
   for (int idx = tid; idx < 4 * R * H; idx += blockDim.x) hbuf[idx] = 0.f;   // hbuf and rhbuf
   if (tid < R) s_len[tid] = (b0 + tid < B) ? min(max(seq_len[b0 + tid], 0), L) : 0;
   if (tid == 0) {
-    for (int k = 0; k < 4; ++k) mbar_init_(&hbar[k], 1);
+    for (int k = 0; k < 4; ++k) rnn::mbar_init_(&hbar[k], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -147,8 +137,8 @@ bigru_rec_kernel(const float* __restrict__ xproj, const float* __restrict__ wh_f
     float* hnxt = hbuf + (pb ^ 1) * R * H;          // h of step s
     float* rhcur = rhbuf + pb * R * H;              // r ⊙ h of step s
     if (tid == 0) {
-      mbar_arrive_expect_tx_(&hbar[pb ^ 1], vec_bytes);
-      mbar_arrive_expect_tx_(&rhbar[pb], vec_bytes);
+      rnn::mbar_arrive_expect_tx_(&hbar[pb ^ 1], vec_bytes);
+      rnn::mbar_arrive_expect_tx_(&rhbar[pb], vec_bytes);
     }
     float xr[RC], xu[RC], xc[RC];
 #pragma unroll
@@ -158,7 +148,7 @@ bigru_rec_kernel(const float* __restrict__ xproj, const float* __restrict__ wh_f
       xc[rr] = nxc[rr];
     }
     fetch(s + 1);
-    if (s > 0) mbar_wait_(&hbar[pb], (uint32_t)((s - 1) >> 1) & 1u);   // h of step s-1 has landed
+    if (s > 0) rnn::mbar_wait_(&hbar[pb], (uint32_t)((s - 1) >> 1) & 1u);   // h of step s-1 has landed
 
     // ---- product 1: reset / update pre-activations over the full h (packed FFMA2, two chains per row)
     nerdev::f32x2 pa[R], pc[R];
@@ -201,14 +191,14 @@ bigru_rec_kernel(const float* __restrict__ xproj, const float* __restrict__ wh_f
       const int row = q + 4 * rr;
       r_s[rr] = u_s[rr] = rh[rr] = 0.f;
       if (s < lenr[rr]) {
-        r_s[rr] = sigmoidf_(zr[rr] + xr[rr]);
-        u_s[rr] = sigmoidf_(zu[rr] + xu[rr]);
+        r_s[rr] = rnn::sigmoid_fast(zr[rr] + xr[rr]);
+        u_s[rr] = rnn::sigmoid_fast(zu[rr] + xu[rr]);
         rh[rr] = r_s[rr] * hown[rr];
       }
       if (ok && row < R)
-        publish_all(nerdev::smem_u32(rhcur + row * H + ug), nerdev::smem_u32(&rhbar[pb]), rh[rr], C);
+        rnn::publish_all(nerdev::smem_u32(rhcur + row * H + ug), nerdev::smem_u32(&rhbar[pb]), rh[rr], C);
     }
-    mbar_wait_(&rhbar[pb], (uint32_t)(s >> 1) & 1u);   // r ⊙ h of step s has landed
+    rnn::mbar_wait_(&rhbar[pb], (uint32_t)(s >> 1) & 1u);   // r ⊙ h of step s has landed
 
     // ---- product 2: candidate pre-activation over the gathered r ⊙ h
 #pragma unroll
@@ -250,21 +240,14 @@ bigru_rec_kernel(const float* __restrict__ xproj, const float* __restrict__ wh_f
       const int pos = dir == 0 ? s : len - 1 - s;
       float h_out = 0.f, h_state = 0.f, c_a = 0.f;
       if (live) {
-        c_a = actf<ACT>(zc[rr] + xc[rr]);
-        const float h_raw = u_s[rr] * hown[rr] + (1.f - u_s[rr]) * c_a;
-        h_out = h_raw;
-        h_state = h_raw;
-        if (keep_prob < 1.f) {
-          // DropoutWrapper(output_keep_prob, state_keep_prob): independent masks for the emitted output and for the
-          // carried state (for GRUCell the whole state is h), fresh per step; the same hashes as bilstm.cu
-          const uint32_t e = (uint32_t)(((size_t)b * L + pos) * 2 * H + (size_t)dir * H + ug);
-          h_out = nerdev::hash3(seed_lo, seed_hi, e) < thr ? h_raw * inv_keep : 0.f;
-          h_state = nerdev::hash3(seed_lo ^ 0x5bd1e995u, seed_hi, e) < thr ? h_raw * inv_keep : 0.f;
-        }
+        c_a = rnn::act_fast<ACT>(zc[rr] + xc[rr]);
+        h_out = h_state = u_s[rr] * hown[rr] + (1.f - u_s[rr]) * c_a;
+        if (keep_prob < 1.f)   // (for GRUCell the whole state is h)
+          rnn::dropout_out_state(h_out, h_state, seed_lo, seed_hi, thr, inv_keep, b, L, pos, H, dir, ug);
         hown[rr] = h_state;
       }
       // (h of a finished row is never read again — its own recurrence has stopped — so 0 is as good as the carried value)
-      if (cell_ok) publish_all(nerdev::smem_u32(hnxt + row * H + ug), nerdev::smem_u32(&hbar[pb ^ 1]), h_state, C);
+      if (cell_ok) rnn::publish_all(nerdev::smem_u32(hnxt + row * H + ug), nerdev::smem_u32(&hbar[pb ^ 1]), h_state, C);
       if (live) {
         const size_t o = ((size_t)b * L + pos) * 2 * H + (size_t)dir * H + ug;
         out[o] = h_out;
@@ -296,27 +279,9 @@ template <int R, int ACT>
 int launch_rec(const float* xproj, const float* wh_fw, const float* wh_bw, const int32_t* seq_len, float* out, int B,
                int L, int H, int ldx, int C, const int32_t* cu_seqlens, float* gates_out, float* hstate_out, float* rh_out,
                float keep_prob, uint64_t seed, cudaStream_t st) {
-  const size_t smem = ner_bigru_smem_bytes(H, C, R);
-  auto kern = bigru_rec_kernel<R, ACT>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
-  const int ngroups = (B + R - 1) / R;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(2 * ngroups * C));
-  cfg.blockDim = dim3((unsigned)((4 * (H / C) + 31) / 32 * 32));
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = (unsigned)C;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  e = cudaLaunchKernelEx(&cfg, kern, xproj, wh_fw, wh_bw, seq_len, out, B, L, H, ldx, C, cu_seqlens, gates_out, hstate_out,
-                         rh_out, keep_prob, (uint32_t)seed, (uint32_t)(seed >> 32));
-  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
-  return ner_launch_status();
+  return rnn::launch_cluster(bigru_rec_kernel<R, ACT>, B, R, C, (4 * (H / C) + 31) / 32 * 32, rnn::gru_smem_bytes(H, C, R),
+                             st, xproj, wh_fw, wh_bw, seq_len, out, B, L, H, ldx, C, cu_seqlens, gates_out, hstate_out,
+                             rh_out, keep_prob, (uint32_t)seed, (uint32_t)(seed >> 32));
 }
 
 }  // namespace
@@ -334,10 +299,10 @@ extern "C" int ner_bigru_recurrence(const float* xproj, const float* wh_fw, cons
   if (!(keep_prob > 0.f) || keep_prob > 1.f) return NER_ERR_INVALID_ARG;
   if (activation != 0 && activation != 1) return NER_ERR_INVALID_ARG;
   if (H % 4 != 0) return NER_ERR_UNSUPPORTED;
-  const int C = ner_bigru_pick_cluster(H);
+  const int C = rnn::gru_pick_cluster(H);
   if (C == 0) return NER_ERR_UNSUPPORTED;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int R = ner_bigru_rows_per_cluster(B, C);
+  const int R = rnn::rows_per_cluster(B, C);
 #define GO(RR)                                                                                                         \
   return activation == 1                                                                                               \
              ? launch_rec<RR, 1>(xproj, wh_fw, wh_bw, seq_len, out, B, L, H, ld_xproj, C, cu_seqlens, gates_out, hstate_out,     \

@@ -13,19 +13,12 @@
 // gradients stay GEMMs / column sums over d_xproj done by the caller.
 #include <cooperative_groups.h>
 
-#include "bigru.cuh"
 #include "common.cuh"
-#include "dsmem.cuh"
+#include "rnn_cluster.cuh"
 
 namespace cg = cooperative_groups;
 
 namespace {
-
-template <int ACT>
-__device__ __forceinline__ float act_grad_from_output(float a) {   // d act(x)/dx expressed through a = act(x)
-  if (ACT == 1) return a > 0.f ? 1.f : 0.f;
-  return 1.f - a * a;
-}
 
 template <int R, int ACT>
 __global__ void __launch_bounds__(512, 1)
@@ -34,13 +27,10 @@ bigru_bwd_kernel(const float* __restrict__ d_out, const float* __restrict__ gate
                  float* __restrict__ d_xproj, int B, int L, int H, int C, float keep_prob, uint32_t seed_lo,
                  uint32_t seed_hi) {
   cg::cluster_group cluster = cg::this_cluster();
-  const int rank = (int)cluster.block_rank();
   const int HU = H / C, NT = 4 * HU, H4 = H / 4;
   const int M1 = (H4 + 3) / 4, M2 = (H4 + 1) / 2;   // float4 steps of the W_c^hᵀ and W_g^hᵀ products per lane
-  const int ngroups = (B + R - 1) / R;
-  const int cid = blockIdx.x / C;
-  const int dir = cid / ngroups;
-  const int b0 = (cid % ngroups) * R;
+  const rnn::RowGroup grp = rnn::row_group(C, B, R);
+  const int rank = grp.rank, dir = grp.dir, b0 = grp.b0;
   const int tid = threadIdx.x;
 
   extern __shared__ __align__(16) float smem[];
@@ -68,25 +58,13 @@ bigru_bwd_kernel(const float* __restrict__ d_out, const float* __restrict__ gate
     V2[idx] = w;
   }
   for (int idx = tid; idx < 6 * R * H; idx += blockDim.x) dcbuf[idx] = 0.f;   // dcbuf and dgbuf
-  if (tid < R) s_len[tid] = (b0 + tid < B) ? min(max(seq_len[b0 + tid], 0), L) : 0;
   if (tid == 0) {
-    for (int k = 0; k < 4; ++k) mbar_init_(&dcbar[k], 1);
+    for (int k = 0; k < 4; ++k) rnn::mbar_init_(&dcbar[k], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  __syncthreads();
-  int maxlen = 0;
-#pragma unroll
-  for (int r = 0; r < R; ++r) maxlen = max(maxlen, s_len[r]);
+  const int maxlen = rnn::load_lengths<R>(s_len, seq_len, b0, B, L);
   cluster.sync();
-
-  // positions never visited by any step of this cluster's rows: d_xproj = 0
-  for (int idx = tid; idx < R * 3 * HU; idx += blockDim.x) {
-    const int r = idx / (3 * HU), c = idx - r * 3 * HU;
-    const int g = c / HU, u = c - g * HU;
-    const int b = b0 + r;
-    if (b < B)
-      for (int t = s_len[r]; t < L; ++t) d_xproj[((size_t)b * L + t) * 6 * H + (size_t)dir * 3 * H + g * H + rank * HU + u] = 0.f;
-  }
+  rnn::zero_unvisited<3>(d_xproj, s_len, R, b0, B, L, H, dir, rank, HU);
 
   const bool ok = tid < NT;
   const int q = tid & 3, ug = rank * HU + (tid >> 2);
@@ -130,8 +108,8 @@ bigru_bwd_kernel(const float* __restrict__ d_out, const float* __restrict__ gate
     float* dccur = dcbuf + pb * R * H;
     float* dgcur = dgbuf + pb * 2 * R * H;
     if (tid == 0) {
-      mbar_arrive_expect_tx_(&dcbar[pb], c_bytes);
-      mbar_arrive_expect_tx_(&dgbar[pb], g_bytes);
+      rnn::mbar_arrive_expect_tx_(&dcbar[pb], c_bytes);
+      rnn::mbar_arrive_expect_tx_(&dgbar[pb], g_bytes);
     }
     float r_s[RC], u_s[RC], hp[RC], dh[RC], dau[RC], dac[RC];
     size_t gi[RC];
@@ -150,23 +128,20 @@ bigru_bwd_kernel(const float* __restrict__ d_out, const float* __restrict__ gate
       dh[rr] = dau[rr] = dac[rr] = 0.f;
       gi[rr] = ((size_t)b * L + pos) * 6 * H + (size_t)dir * 3 * H + ug;
       if (live) {
-        if (keep_prob < 1.f) {   // same masks as the forward DropoutWrapper (output / state)
-          const uint32_t e = (uint32_t)(((size_t)b * L + pos) * 2 * H + (size_t)dir * H + ug);
-          dh_o = nerdev::hash3(seed_lo, seed_hi, e) < thr ? dh_o * inv_keep : 0.f;
-          dh_s = nerdev::hash3(seed_lo ^ 0x5bd1e995u, seed_hi, e) < thr ? dh_s * inv_keep : 0.f;
-        }
+        if (keep_prob < 1.f)   // the forward's DropoutWrapper masks (output / state)
+          rnn::dropout_out_state(dh_o, dh_s, seed_lo, seed_hi, thr, inv_keep, b, L, pos, H, dir, ug);
         dh[rr] = dh_o + dh_s;
-        dac[rr] = dh[rr] * (1.f - u_s[rr]) * act_grad_from_output<ACT>(c_a);
+        dac[rr] = dh[rr] * (1.f - u_s[rr]) * rnn::act_grad_from_output<ACT>(c_a);
         dau[rr] = dh[rr] * (hp[rr] - c_a) * u_s[rr] * (1.f - u_s[rr]);
       }
-      if (ok && row < R) publish_all(nerdev::smem_u32(dccur + row * H + ug), nerdev::smem_u32(&dcbar[pb]), dac[rr], C);
+      if (ok && row < R) rnn::publish_all(nerdev::smem_u32(dccur + row * H + ug), nerdev::smem_u32(&dcbar[pb]), dac[rr], C);
       if (live) {
         d_xproj[gi[rr] + H] = dau[rr];
         d_xproj[gi[rr] + 2 * H] = dac[rr];
       }
     }
     fetch(s - 1);
-    mbar_wait_(&dcbar[pb], (uint32_t)(n >> 1) & 1u);
+    rnn::mbar_wait_(&dcbar[pb], (uint32_t)(n >> 1) & 1u);
 
     // ---- d(rh)[k] = sum_j da_c[j] W_c^h[k, j]
     nerdev::f32x2 pa[R], pc[R];
@@ -176,14 +151,8 @@ bigru_bwd_kernel(const float* __restrict__ d_out, const float* __restrict__ gate
       const float4* d4 = reinterpret_cast<const float4*>(dccur);
 #pragma unroll 4
       for (int i = 0; i < M1; ++i) {
-        const float4 w = V1[i * NT + tid];
         const int j4 = min(4 * i + q, H4 - 1);   // past H the weights are zero
-#pragma unroll
-        for (int r = 0; r < R; ++r) {
-          const float4 v = d4[r * H4 + j4];
-          pa[r] = nerdev::fma2(nerdev::pk2(w.x, w.y), nerdev::pk2(v.x, v.y), pa[r]);
-          pc[r] = nerdev::fma2(nerdev::pk2(w.z, w.w), nerdev::pk2(v.z, v.w), pc[r]);
-        }
+        rnn::fma2_rows<R>(pa, pc, V1[i * NT + tid], d4, H4, j4);
       }
     }
     float drh[RC];
@@ -191,10 +160,7 @@ bigru_bwd_kernel(const float* __restrict__ d_out, const float* __restrict__ gate
     for (int rr = 0; rr < RC; ++rr) drh[rr] = 0.f;
 #pragma unroll
     for (int r = 0; r < R; ++r) {
-      float z0, z1, z2, z3;
-      nerdev::upk2(pa[r], z0, z1);
-      nerdev::upk2(pc[r], z2, z3);
-      float z = (z0 + z1) + (z2 + z3);
+      float z = rnn::sum_chains(pa[r], pc[r]);
       z += __shfl_xor_sync(0xffffffffu, z, 1);
       z += __shfl_xor_sync(0xffffffffu, z, 2);
       if (q == (r & 3)) drh[r >> 2] = z;
@@ -213,11 +179,11 @@ bigru_bwd_kernel(const float* __restrict__ d_out, const float* __restrict__ gate
       }
       if (ok && row < R) {
         const uint32_t lb = nerdev::smem_u32(&dgbar[pb]);
-        publish_all(nerdev::smem_u32(dgcur + row * 2 * H + ug), lb, dar, C);
-        publish_all(nerdev::smem_u32(dgcur + row * 2 * H + H + ug), lb, dau[rr], C);
+        rnn::publish_all(nerdev::smem_u32(dgcur + row * 2 * H + ug), lb, dar, C);
+        rnn::publish_all(nerdev::smem_u32(dgcur + row * 2 * H + H + ug), lb, dau[rr], C);
       }
     }
-    mbar_wait_(&dgbar[pb], (uint32_t)(n >> 1) & 1u);
+    rnn::mbar_wait_(&dgbar[pb], (uint32_t)(n >> 1) & 1u);
 
     // ---- dh_prev[k] = dh u + d(rh) r + sum_j [da_r | da_u][j] W_g^h[k, j]
 #pragma unroll
@@ -226,22 +192,13 @@ bigru_bwd_kernel(const float* __restrict__ d_out, const float* __restrict__ gate
       const float4* d4 = reinterpret_cast<const float4*>(dgcur);
 #pragma unroll 4
       for (int i = 0; i < M2; ++i) {
-        const float4 w = V2[i * NT + tid];
         const int j4 = min(4 * i + q, 2 * H4 - 1);
-#pragma unroll
-        for (int r = 0; r < R; ++r) {
-          const float4 v = d4[r * 2 * H4 + j4];
-          pa[r] = nerdev::fma2(nerdev::pk2(w.x, w.y), nerdev::pk2(v.x, v.y), pa[r]);
-          pc[r] = nerdev::fma2(nerdev::pk2(w.z, w.w), nerdev::pk2(v.z, v.w), pc[r]);
-        }
+        rnn::fma2_rows<R>(pa, pc, V2[i * NT + tid], d4, 2 * H4, j4);
       }
     }
 #pragma unroll
     for (int r = 0; r < R; ++r) {
-      float z0, z1, z2, z3;
-      nerdev::upk2(pa[r], z0, z1);
-      nerdev::upk2(pc[r], z2, z3);
-      float z = (z0 + z1) + (z2 + z3);
+      float z = rnn::sum_chains(pa[r], pc[r]);
       z += __shfl_xor_sync(0xffffffffu, z, 1);
       z += __shfl_xor_sync(0xffffffffu, z, 2);
       // a finished row carries the recurrent gradient through unchanged (dynamic_rnn copies its state)
@@ -255,27 +212,9 @@ template <int R, int ACT>
 int launch_bwd(const float* d_out, const float* gates, const float* hstate, const float* wh_fw, const float* wh_bw,
                const int32_t* seq_len, float* d_xproj, int B, int L, int H, int C, float keep_prob, uint64_t seed,
                cudaStream_t st) {
-  const size_t smem = ner_bigru_smem_bytes(H, C, R);
-  auto kern = bigru_bwd_kernel<R, ACT>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
-  const int ngroups = (B + R - 1) / R;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(2 * ngroups * C));
-  cfg.blockDim = dim3((unsigned)((4 * (H / C) + 31) / 32 * 32));
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = (unsigned)C;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  e = cudaLaunchKernelEx(&cfg, kern, d_out, gates, hstate, wh_fw, wh_bw, seq_len, d_xproj, B, L, H, C, keep_prob,
-                         (uint32_t)seed, (uint32_t)(seed >> 32));
-  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
-  return ner_launch_status();
+  return rnn::launch_cluster(bigru_bwd_kernel<R, ACT>, B, R, C, (4 * (H / C) + 31) / 32 * 32, rnn::gru_smem_bytes(H, C, R),
+                             st, d_out, gates, hstate, wh_fw, wh_bw, seq_len, d_xproj, B, L, H, C, keep_prob,
+                             (uint32_t)seed, (uint32_t)(seed >> 32));
 }
 
 }  // namespace
@@ -289,10 +228,10 @@ extern "C" int ner_bigru_recurrence_bwd(const float* d_out, const float* gates, 
   if (!(keep_prob > 0.f) || keep_prob > 1.f) return NER_ERR_INVALID_ARG;
   if (activation != 0 && activation != 1) return NER_ERR_INVALID_ARG;
   if (H % 4 != 0) return NER_ERR_UNSUPPORTED;
-  const int C = ner_bigru_pick_cluster(H);
+  const int C = rnn::gru_pick_cluster(H);
   if (C == 0) return NER_ERR_UNSUPPORTED;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int R = ner_bigru_rows_per_cluster(B, C);
+  const int R = rnn::rows_per_cluster(B, C);
 #define GO(RR)                                                                                                       \
   return activation == 1 ? launch_bwd<RR, 1>(d_out, gates, hstate, wh_fw, wh_bw, seq_len, d_xproj, B, L, H, C,      \
                                              keep_prob, seed, st)                                                    \

@@ -14,24 +14,13 @@
 // hidden units, applies the cell, and broadcasts the new h slice to every CTA of the cluster
 // through distributed shared memory; one cluster barrier per time step.
 #include <cooperative_groups.h>
-#include <stdlib.h>
 
 #include "common.cuh"
-#include "dsmem.cuh"
+#include "rnn_cluster.cuh"
 
 namespace cg = cooperative_groups;
 
 namespace {
-
-// ex2.approx-based forms (abs. error ~1e-7, far inside the 1e-4 parity bar of tests/test_bilstm_gpu.py):
-// the activations sit on the per-step critical path of the recurrence.
-__device__ __forceinline__ float sigmoidf_(float x) { return __fdividef(1.f, 1.f + __expf(-x)); }
-
-template <int ACT>
-__device__ __forceinline__ float actf(float x) {
-  if (ACT == 1) return fmaxf(x, 0.f);
-  return 1.f - __fdividef(2.f, 1.f + __expf(2.f * x));   // tanh(x); saturates correctly for |x| large
-}
 
 // H4REG > 0: this thread's gate column of W_h (H4REG float4 = H fp32 values) is register-resident
 // for the whole sequence (H <= 128); H4REG == 0: the slice is read from shared memory each step.
@@ -43,14 +32,11 @@ __global__ void __launch_bounds__(H4REG > 0 ? 256 : 512, 1) bilstm_rec_kernel(co
                                   float* __restrict__ cstate_out, float* __restrict__ hstate_out, float keep_prob,
                                   uint32_t seed_lo, uint32_t seed_hi) {
   cg::cluster_group cluster = cg::this_cluster();
-  const int rank = (int)cluster.block_rank();
   const int HU = H / C;       // hidden units owned by this CTA
   const int NC = 4 * HU;      // gate columns owned by this CTA
   const int H4 = H / 4;
-  const int ngroups = (B + R - 1) / R;
-  const int cid = blockIdx.x / C;
-  const int dir = cid / ngroups;
-  const int b0 = (cid % ngroups) * R;
+  const rnn::RowGroup grp = rnn::row_group(C, B, R);
+  const int rank = grp.rank, dir = grp.dir, b0 = grp.b0;
   const int tid = threadIdx.x;
 
   extern __shared__ __align__(16) float smem[];
@@ -88,16 +74,12 @@ __global__ void __launch_bounds__(H4REG > 0 ? 256 : 512, 1) bilstm_rec_kernel(co
     }
   }
   for (int idx = tid; idx < 2 * R * H; idx += blockDim.x) hbuf[idx] = 0.f;
-  if (tid < R) s_len[tid] = (b0 + tid < B) ? min(max(seq_len[b0 + tid], 0), L) : 0;
   if (tid == 0) {
-    mbar_init_(&hbar[0], 1);
-    mbar_init_(&hbar[1], 1);
+    rnn::mbar_init_(&hbar[0], 1);
+    rnn::mbar_init_(&hbar[1], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  __syncthreads();
-  int maxlen = 0;
-#pragma unroll
-  for (int r = 0; r < R; ++r) maxlen = max(maxlen, s_len[r]);
+  const int maxlen = rnn::load_lengths<R>(s_len, seq_len, b0, B, L);
   cluster.sync();  // every CTA's hbuf is zeroed before anyone writes remotely
 
   // Thread t < NC owns gate g = t & 3 of hidden unit u = t >> 2 (of this CTA's slice): the four
@@ -138,11 +120,9 @@ __global__ void __launch_bounds__(H4REG > 0 ? 256 : 512, 1) bilstm_rec_kernel(co
     const float* hcur = hbuf + (s & 1) * R * H;
     float* hnxt = hbuf + ((s + 1) & 1) * R * H;
     if (C > 1) {
-      if (tid == 0) mbar_arrive_expect_tx_(&hbar[(s + 1) & 1], h_bytes);   // arm the buffer written this step
-      if (s > 0) mbar_wait_(&hbar[s & 1], (uint32_t)((s - 1) >> 1) & 1u);   // h of step s-1 has landed (k-th use of the buffer)
+      if (tid == 0) rnn::mbar_arrive_expect_tx_(&hbar[(s + 1) & 1], h_bytes);   // arm the buffer written this step
+      if (s > 0) rnn::mbar_wait_(&hbar[s & 1], (uint32_t)((s - 1) >> 1) & 1u);   // h of step s-1 has landed (k-th use of the buffer)
     }
-    // packed fp32 pairs (FFMA2): (w_k, w_k+1) x (h_k, h_k+1) halves the FMA issue slots of the dot
-    // products, the per-step throughput bound of this kernel; two chains per row for latency
     nerdev::f32x2 pa[R], pb[R];
 #pragma unroll
     for (int r = 0; r < R; ++r) {
@@ -163,26 +143,10 @@ __global__ void __launch_bounds__(H4REG > 0 ? 256 : 512, 1) bilstm_rec_kernel(co
       const float4* hc4 = reinterpret_cast<const float4*>(hcur);
       if constexpr (WREG) {
 #pragma unroll
-        for (int k4 = 0; k4 < H4REG; ++k4) {
-          const float4 w = wreg[k4];
-#pragma unroll
-          for (int r = 0; r < R; ++r) {
-            const float4 hv = hc4[r * H4 + k4];
-            pa[r] = nerdev::fma2(nerdev::pk2(w.x, w.y), nerdev::pk2(hv.x, hv.y), pa[r]);
-            pb[r] = nerdev::fma2(nerdev::pk2(w.z, w.w), nerdev::pk2(hv.z, hv.w), pb[r]);
-          }
-        }
+        for (int k4 = 0; k4 < H4REG; ++k4) rnn::fma2_rows<R>(pa, pb, wreg[k4], hc4, H4, k4);
       } else {
 #pragma unroll 4
-        for (int k4 = 0; k4 < H4; ++k4) {
-          const float4 w = Ws4[k4 * NC + tid];
-#pragma unroll
-          for (int r = 0; r < R; ++r) {
-            const float4 hv = hc4[r * H4 + k4];
-            pa[r] = nerdev::fma2(nerdev::pk2(w.x, w.y), nerdev::pk2(hv.x, hv.y), pa[r]);
-            pb[r] = nerdev::fma2(nerdev::pk2(w.z, w.w), nerdev::pk2(hv.z, hv.w), pb[r]);
-          }
-        }
+        for (int k4 = 0; k4 < H4; ++k4) rnn::fma2_rows<R>(pa, pb, Ws4[k4 * NC + tid], hc4, H4, k4);
       }
     }
     // quad transpose: lane g of the quad receives (z_i, z_j, z_f, z_o) of its rows g, g + 4, ...
@@ -192,10 +156,7 @@ __global__ void __launch_bounds__(H4REG > 0 ? 256 : 512, 1) bilstm_rec_kernel(co
     const int qb = (tid & 31) & ~3;
 #pragma unroll
     for (int r = 0; r < R; ++r) {
-      float z0, z1, z2, z3;
-      nerdev::upk2(pa[r], z0, z1);
-      nerdev::upk2(pb[r], z2, z3);
-      const float z = (z0 + z1) + (z2 + z3);
+      const float z = rnn::sum_chains(pa[r], pb[r]);
       const float a0 = __shfl_sync(0xffffffffu, z, qb + 0);
       const float a1 = __shfl_sync(0xffffffffu, z, qb + 1);
       const float a2 = __shfl_sync(0xffffffffu, z, qb + 2);
@@ -221,28 +182,21 @@ __global__ void __launch_bounds__(H4REG > 0 ? 256 : 512, 1) bilstm_rec_kernel(co
       const bool live = cell_ok && s < len;
       const int pos = dir == 0 ? s : len - 1 - s;
       if (live) {
-        i_s = sigmoidf_(zi[rr]);
-        j_a = actf<ACT>(zj[rr]);
-        f_s = sigmoidf_(zf[rr] + forget_bias);
-        o_s = sigmoidf_(zo[rr]);
+        i_s = rnn::sigmoid_fast(zi[rr]);
+        j_a = rnn::act_fast<ACT>(zj[rr]);
+        f_s = rnn::sigmoid_fast(zf[rr] + forget_bias);
+        o_s = rnn::sigmoid_fast(zo[rr]);
         c_state[rr] = f_s * c_state[rr] + i_s * j_a;
-        const float h_raw = o_s * actf<ACT>(c_state[rr]);
-        h_out = h_raw;
-        h_state = h_raw;
-        if (keep_prob < 1.f) {
-          // DropoutWrapper(output_keep_prob, state_keep_prob): independent masks for the emitted output
-          // and for the h part of the carried state (c is not dropped), fresh per step
-          const uint32_t e = (uint32_t)(((size_t)b * L + pos) * 2 * H + (size_t)dir * H + ug);
-          h_out = nerdev::hash3(seed_lo, seed_hi, e) < thr ? h_raw * inv_keep : 0.f;
-          h_state = nerdev::hash3(seed_lo ^ 0x5bd1e995u, seed_hi, e) < thr ? h_raw * inv_keep : 0.f;
-        }
+        h_out = h_state = o_s * rnn::act_fast<ACT>(c_state[rr]);
+        if (keep_prob < 1.f)   // (c is not dropped)
+          rnn::dropout_out_state(h_out, h_state, seed_lo, seed_hi, thr, inv_keep, b, L, pos, H, dir, ug);
       }
       if (cell_ok) {
         // (h of a finished row is never read again — its own recurrence has stopped — so 0 is as good as
         // the carried value dynamic_rnn keeps)
         if (C > 1) {
           const uint32_t la = nerdev::smem_u32(hnxt + r * H + ug), lb = nerdev::smem_u32(&hbar[(s + 1) & 1]);
-          for (int dst = 0; dst < C; ++dst) st_async_f32(mapa_u32(la, (uint32_t)dst), h_state, mapa_u32(lb, (uint32_t)dst));
+          rnn::publish_all(la, lb, h_state, C);
         } else {
           hnxt[r * H + ug] = h_state;
         }
@@ -265,14 +219,7 @@ __global__ void __launch_bounds__(H4REG > 0 ? 256 : 512, 1) bilstm_rec_kernel(co
     if (C == 1) __syncthreads();
   }
   if (C > 1) cluster.sync();   // nobody exits while a peer may still be sending into its shared memory
-
-  // positions past the longest row of this cluster: zeros
-  for (int idx = tid; idx < R * HU; idx += blockDim.x) {
-    const int r = idx / HU, uu = idx - r * HU;
-    const int b = b0 + r;
-    if (b < B)
-      for (int s = maxlen; s < L; ++s) out[((size_t)b * L + s) * 2 * H + (size_t)dir * H + rank * HU + uu] = 0.f;
-  }
+  rnn::zero_past_maxlen(out, R, b0, B, L, H, dir, rank, HU, maxlen);
 }
 
 int pick_cluster(int H) {
@@ -291,26 +238,9 @@ int launch_rec(const float* xproj, const float* wh_fw, const float* wh_bw, const
                float* hstate_out, float keep_prob, uint64_t seed, cudaStream_t st) {
   const int HU = H / C, NC = 4 * HU;
   const size_t smem = ((H4REG > 0 ? 0 : (size_t)H * NC) + 2 * R * H + 32) * 4;   // + s_len[8] + 2 mbarriers (16-B aligned: R*H even)
-  auto kern = bilstm_rec_kernel<R, ACT, H4REG>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
-  const int ngroups = (B + R - 1) / R;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(2 * ngroups * C));
-  cfg.blockDim = dim3((unsigned)((NC + 31) / 32 * 32));
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = (unsigned)C;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  e = cudaLaunchKernelEx(&cfg, kern, xproj, wh_fw, wh_bw, seq_len, out, B, L, H, C, forget_bias, cu_seqlens, gates_out,
-                         cstate_out, hstate_out, keep_prob, (uint32_t)seed, (uint32_t)(seed >> 32));
-  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
-  return ner_launch_status();
+  return rnn::launch_cluster(bilstm_rec_kernel<R, ACT, H4REG>, B, R, C, (NC + 31) / 32 * 32, smem, st, xproj, wh_fw, wh_bw,
+                             seq_len, out, B, L, H, C, forget_bias, cu_seqlens, gates_out, cstate_out, hstate_out,
+                             keep_prob, (uint32_t)seed, (uint32_t)(seed >> 32));
 }
 
 }  // namespace
@@ -330,22 +260,14 @@ extern "C" int ner_bilstm_recurrence(const float* xproj, const float* wh_fw, con
   const int C = pick_cluster(H);
   if (C == 0) return NER_ERR_UNSUPPORTED;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // rows per cluster: fill the SMs once when the batch is small, amortise W_h reads when large
-  int R = 1;
-  if ((long)2 * B * C > ner_num_sms()) R = 2;
-  if ((long)2 * ((B + 1) / 2) * C > 2 * ner_num_sms()) R = 4;
+  int R = rnn::rows_per_cluster(B, C);
   // four stacked PREDICT batches (B = 256): 4 rows per cluster would be 256 CTAs = two waves of the one-CTA-per-SM kernel
   if (H == 128 && (long)2 * ((B + 3) / 4) * C > ner_num_sms()) R = 8;
-  if (const char* e = getenv("NER_BILSTM_ROWS")) {   // tuning hook: rows per cluster (1, 2, 4 or 8)
-    const int v = atoi(e);
-    if (v == 1 || v == 2 || v == 4 || (v == 8 && H == 128)) R = v;
-  }
 #define GO(RR, HR)                                                                                          \
   return activation == 1 ? launch_rec<RR, 1, HR>(xproj, wh_fw, wh_bw, seq_len, out, B, L, H, C, forget_bias, cu_seqlens, gates_out, cstate_out, hstate_out, keep_prob, seed, st) \
                          : launch_rec<RR, 0, HR>(xproj, wh_fw, wh_bw, seq_len, out, B, L, H, C, forget_bias, cu_seqlens, gates_out, cstate_out, hstate_out, keep_prob, seed, st)
   if (H == 128 && 4 * (H / C) <= 256) {  // register-resident W_h (the bert_bilstm_crf / bilstm_crf shape)
-    if (R == 8) GO(8, 32);
-    if (R == 4) GO(4, 32);
+    if (R == 8) GO(8, 32);   // (R == 4 does not reach here: its rule implies the R = 8 rule)
     if (R == 2) GO(2, 32);
     GO(1, 32);
   }

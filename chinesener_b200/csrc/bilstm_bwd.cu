@@ -14,19 +14,15 @@
 // dW_h = sum_t h_{t-1}^T dz_t is NOT accumulated here: it is one tensor-core GEMM over
 // (h_prev [B*L, H], d_xproj [B*L, 4H]) done by the caller.
 #include <cooperative_groups.h>
-#include <stdlib.h>
 
 #include "common.cuh"
+#include "rnn_cluster.cuh"
 
 namespace cg = cooperative_groups;
 
 namespace {
 
-template <int ACT>
-__device__ __forceinline__ float act_grad_from_output(float a) {  // d act(x)/dx expressed through a = act(x)
-  if (ACT == 1) return a > 0.f ? 1.f : 0.f;
-  return 1.f - a * a;
-}
+// exact tanhf, not the forward kernel's ex2.approx form (rnn::act_fast)
 template <int ACT>
 __device__ __forceinline__ float actf(float x) {
   if (ACT == 1) return fmaxf(x, 0.f);
@@ -46,12 +42,9 @@ bilstm_bwd_kernel(const float* __restrict__ d_out, const float* __restrict__ gat
                   float* __restrict__ d_xproj, int B, int L, int H, int C, float keep_prob, uint32_t seed_lo,
                   uint32_t seed_hi) {
   cg::cluster_group cluster = cg::this_cluster();
-  const int rank = (int)cluster.block_rank();
-  const int HU = H / C, NC = 4 * HU, G4 = 4 * H;
-  const int ngroups = (B + R - 1) / R;
-  const int cid = blockIdx.x / C;
-  const int dir = cid / ngroups;
-  const int b0 = (cid % ngroups) * R;
+  const int HU = H / C, G4 = 4 * H;
+  const rnn::RowGroup grp = rnn::row_group(C, B, R);
+  const int rank = grp.rank, dir = grp.dir, b0 = grp.b0;
   const int tid = threadIdx.x;
 
   extern __shared__ __align__(16) float smem[];
@@ -82,11 +75,7 @@ bilstm_bwd_kernel(const float* __restrict__ d_out, const float* __restrict__ gat
   }
   for (int idx = tid; idx < 2 * R * G4P; idx += blockDim.x) dzbuf[idx] = 0.f;
   for (int idx = tid; idx < R * HU; idx += blockDim.x) dhbuf[idx] = 0.f;
-  if (tid < R) s_len[tid] = (b0 + tid < B) ? min(max(seq_len[b0 + tid], 0), L) : 0;
-  __syncthreads();
-  int maxlen = 0;
-#pragma unroll
-  for (int r = 0; r < R; ++r) maxlen = max(maxlen, s_len[r]);
+  const int maxlen = rnn::load_lengths<R>(s_len, seq_len, b0, B, L);
   cluster.sync();
 
   // cell role: thread (r, u) for tid < R*HU
@@ -94,15 +83,7 @@ bilstm_bwd_kernel(const float* __restrict__ d_out, const float* __restrict__ gat
   const int cr = cell_ok ? tid / HU : 0, cu = cell_ok ? tid - cr * HU : 0;
   float dc_carry = 0.f;
 
-  // positions never visited by any step of this cluster's rows: d_xproj = 0
-  for (int idx = tid; idx < R * NC; idx += blockDim.x) {
-    const int r = idx / NC, c = idx - r * NC;
-    const int g = c / HU, u = c - g * HU;
-    const int b = b0 + r;
-    if (b < B)
-      for (int t = s_len[r]; t < L; ++t)
-        d_xproj[((size_t)b * L + t) * 2 * G4 + (size_t)dir * G4 + g * H + rank * HU + u] = 0.f;
-  }
+  rnn::zero_unvisited<4>(d_xproj, s_len, R, b0, B, L, H, dir, rank, HU);
 
   // Per-step operands (saved gates, cell states, upstream gradient) do not depend on the recurrence: they are
   // fetched one step ahead so their L2/HBM latency overlaps the previous step instead of heading its chain.
@@ -140,19 +121,15 @@ bilstm_bwd_kernel(const float* __restrict__ d_out, const float* __restrict__ gat
     const size_t gi = ((size_t)my_b * L + pos) * 2 * G4 + (size_t)dir * G4;
     if (live) {
       float dh_s = dhbuf[cr * HU + cu];
-      if (keep_prob < 1.f) {  // same masks as the forward DropoutWrapper (output / state)
-        const uint32_t thr = nerdev::keep_threshold(keep_prob);
-        const uint32_t e = (uint32_t)(((size_t)my_b * L + pos) * 2 * H + (size_t)dir * H + ug);
-        const float inv = 1.f / keep_prob;
-        dh_o = nerdev::hash3(seed_lo, seed_hi, e) < thr ? dh_o * inv : 0.f;
-        dh_s = nerdev::hash3(seed_lo ^ 0x5bd1e995u, seed_hi, e) < thr ? dh_s * inv : 0.f;
-      }
+      if (keep_prob < 1.f)   // the forward's DropoutWrapper masks (output / state)
+        rnn::dropout_out_state(dh_o, dh_s, seed_lo, seed_hi, nerdev::keep_threshold(keep_prob), 1.f / keep_prob, my_b, L,
+                               pos, H, dir, ug);
       const float dh = dh_o + dh_s;
       const float ac = actf<ACT>(c_t);
       const float d_o = dh * ac;
-      const float dc = dh * o_s * act_grad_from_output<ACT>(ac) + dc_carry;
+      const float dc = dh * o_s * rnn::act_grad_from_output<ACT>(ac) + dc_carry;
       dzi = dc * j_a * i_s * (1.f - i_s);
-      dzj = dc * i_s * act_grad_from_output<ACT>(j_a);
+      dzj = dc * i_s * rnn::act_grad_from_output<ACT>(j_a);
       dzf = dc * c_prev * f_s * (1.f - f_s);
       dzo = d_o * o_s * (1.f - o_s);
       dc_carry = dc * f_s;
@@ -248,31 +225,13 @@ int launch_bwd(const float* d_out, const float* gates, const float* cstate, cons
   const int HU = H / C;
   const size_t smem = WR > 0 ? ((size_t)2 * R * (4 * H + 16) + (size_t)R * HU + 32) * 4
                             : ((size_t)4 * H * (HU + 1) + 2 * R * 4 * H + (size_t)R * HU + 32) * 4;
-  auto kern = bilstm_bwd_kernel<R, ACT, WR>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
   // threads: R*HU teams x tpt threads, tpt = largest power of two with R*HU*tpt <= 512 (and <= 32)
   int tpt = 1;
   while (tpt < 32 && R * HU * tpt * 2 <= 512) tpt *= 2;
   int threads = ((R * HU * tpt + 31) / 32) * 32;
   if (WR > 0) threads = ((max(HU * 4, R * HU) + 31) / 32) * 32;      // (k, part) GEMV threads; the first R*HU also run the cells
-  const int ngroups = (B + R - 1) / R;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(2 * ngroups * C));
-  cfg.blockDim = dim3((unsigned)threads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = (unsigned)C;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  e = cudaLaunchKernelEx(&cfg, kern, d_out, gates, cstate, wh_fw, wh_bw, seq_len, d_xproj, B, L, H, C, keep_prob,
-                         (uint32_t)seed, (uint32_t)(seed >> 32));
-  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
-  return ner_launch_status();
+  return rnn::launch_cluster(bilstm_bwd_kernel<R, ACT, WR>, B, R, C, threads, smem, st, d_out, gates, cstate, wh_fw, wh_bw,
+                             seq_len, d_xproj, B, L, H, C, keep_prob, (uint32_t)seed, (uint32_t)(seed >> 32));
 }
 
 }  // namespace
@@ -288,14 +247,12 @@ extern "C" int ner_bilstm_recurrence_bwd(const float* d_out, const float* gates,
   const int C = pick_cluster_bwd(H);
   if (C == 0 || (H / C) > 256) return NER_ERR_UNSUPPORTED;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int R = 1;
-  if ((long)2 * B * C > ner_num_sms()) R = 2;
+  int R = min(rnn::rows_per_cluster(B, C), 2);
   if (2 * (H / C) > 512) R = 1;
 #define GO(RR, WRR)                                                                                                \
   return activation == 1 ? launch_bwd<RR, 1, WRR>(d_out, gates, cstate, wh_fw, wh_bw, seq_len, d_xproj, B, L, H, C, keep_prob, seed, st) \
                          : launch_bwd<RR, 0, WRR>(d_out, gates, cstate, wh_fw, wh_bw, seq_len, d_xproj, B, L, H, C, keep_prob, seed, st)
-  const char* ev = getenv("NER_BPTT_VARIANT");              // tuning / test hook: 1 = shared-memory walk everywhere
-  if (H == 128 && C == 2 && !(ev && atoi(ev) == 1)) {       // register-resident recurrent matrix: 4H / 4 = 128 columns per thread
+  if (H == 128 && C == 2) {   // register-resident recurrent matrix: 4H / 4 = 128 columns per thread
     if (R == 2) GO(2, 128);
     GO(1, 128);
   }

@@ -20,6 +20,7 @@
 #include <cooperative_groups.h>
 
 #include "common.cuh"
+#include "rnn_cluster.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -91,12 +92,9 @@ lattice_fwd_kernel(const float* __restrict__ xproj, const float* __restrict__ wp
                    float* __restrict__ norm, float* __restrict__ wgates, float* __restrict__ cw_out,
                    float* __restrict__ aw_out, float* __restrict__ hw_out) {
   cg::cluster_group cluster = cg::this_cluster();
-  const int rank = (int)cluster.block_rank();
   const int HU = H / C, NC = 6 * HU, RK = kRing * Kw;
-  const int ngroups = (B + R - 1) / R;
-  const int cid = blockIdx.x / C;
-  const int dir = cid / ngroups;
-  const int b0 = (cid % ngroups) * R;
+  const rnn::RowGroup grp = rnn::row_group(C, B, R);
+  const int rank = grp.rank, dir = grp.dir, b0 = grp.b0;
   const int tid = threadIdx.x;
   const bool save = gates != nullptr;
 
@@ -125,11 +123,7 @@ lattice_fwd_kernel(const float* __restrict__ xproj, const float* __restrict__ wp
     W2[idx] = wac[(size_t)k * H + rank * HU + u];
   }
   for (int idx = tid; idx < 2 * R * H; idx += blockDim.x) hbuf[idx] = 0.f;
-  if (tid < R) s_len[tid] = (b0 + tid < B) ? min(max(seq_len[b0 + tid], 0), L) : 0;
-  __syncthreads();
-  int maxlen = 0;
-#pragma unroll
-  for (int r = 0; r < R; ++r) maxlen = max(maxlen, s_len[r]);
+  const int maxlen = rnn::load_lengths<R>(s_len, seq_len, b0, B, L);
   cluster.sync();   // every CTA's hbuf is zeroed before anyone writes remotely
 
   // cell role: thread (r, u) for tid < R * HU
@@ -253,12 +247,7 @@ lattice_fwd_kernel(const float* __restrict__ xproj, const float* __restrict__ wp
     }
     cluster.sync();
   }
-  for (int idx = tid; idx < R * HU; idx += blockDim.x) {   // positions past the longest row of this cluster: zeros
-    const int r = idx / HU, u = idx - r * HU;
-    const int b = b0 + r;
-    if (b < B)
-      for (int s = maxlen; s < L; ++s) out[((size_t)b * L + s) * 2 * H + (size_t)dir * H + rank * HU + u] = 0.f;
-  }
+  rnn::zero_past_maxlen(out, R, b0, B, L, H, dir, rank, HU, maxlen);
 }
 
 template <int R>
@@ -270,12 +259,9 @@ lattice_bwd_kernel(const float* __restrict__ d_out, const float* __restrict__ ga
                    const int32_t* __restrict__ seq_len, float* __restrict__ d_xproj, float* __restrict__ d_wproj,
                    float* __restrict__ d_alpha, int B, int L, int H, int Kw, int C) {
   cg::cluster_group cluster = cg::this_cluster();
-  const int rank = (int)cluster.block_rank();
   const int HU = H / C, H6 = 6 * H, RK = kRing * Kw;
-  const int ngroups = (B + R - 1) / R;
-  const int cid = blockIdx.x / C;
-  const int dir = cid / ngroups;
-  const int b0 = (cid % ngroups) * R;
+  const rnn::RowGroup grp = rnn::row_group(C, B, R);
+  const int rank = grp.rank, dir = grp.dir, b0 = grp.b0;
   const int tid = threadIdx.x;
 
   extern __shared__ __align__(16) float smem[];
@@ -299,11 +285,7 @@ lattice_bwd_kernel(const float* __restrict__ d_out, const float* __restrict__ ga
     W2[idx] = wac[(size_t)(rank * HU + u) * H + j];
   }
   for (int idx = tid; idx < 2 * R * H6; idx += blockDim.x) dzx[idx] = 0.f;
-  if (tid < R) s_len[tid] = (b0 + tid < B) ? min(max(seq_len[b0 + tid], 0), L) : 0;
-  __syncthreads();
-  int maxlen = 0;
-#pragma unroll
-  for (int r = 0; r < R; ++r) maxlen = max(maxlen, s_len[r]);
+  const int maxlen = rnn::load_lengths<R>(s_len, seq_len, b0, B, L);
   // positions no step visits: d_xproj = 0
   for (int idx = tid; idx < R * HU; idx += blockDim.x) {
     const int r = idx / HU, u = idx - r * HU;
@@ -488,27 +470,6 @@ void pick_config(int B, int H, int Kw, int* R_out, int* C_out) {
   *C_out = C;
 }
 
-template <typename K, typename... Args>
-int launch_cluster(K kern, int B, int R, int C, size_t smem, cudaStream_t st, Args... args) {
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(2 * ((B + R - 1) / R) * C));
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = (unsigned)C;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  e = cudaLaunchKernelEx(&cfg, kern, args...);
-  if (e != cudaSuccess) return NER_ERR_CUDA_BASE - (int)e;
-  return ner_launch_status();
-}
-
 int check_shape(int B, int L, int H, int Kw) {
   if (B < 0 || L < 1 || H < 1 || Kw < 1) return NER_ERR_INVALID_ARG;
   if (Kw > kMaxKw) return NER_ERR_UNSUPPORTED;
@@ -536,8 +497,8 @@ extern "C" int ner_lattice_recurrence(const float* xproj, const float* wproj, co
   const size_t smem = fwd_smem(H, C, R, Kw);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
 #define GO(RR)                                                                                                        \
-  return launch_cluster(lattice_fwd_kernel<RR>, B, RR, C, smem, s, xproj, wproj, lat_len, wrec_fw, wrec_bw, wac_fw,   \
-                        wac_bw, seq_len, out, B, L, H, Kw, C, gates, cstate, norm, wgates, cw, aw, hw)
+  return rnn::launch_cluster(lattice_fwd_kernel<RR>, B, RR, C, kThreads, smem, s, xproj, wproj, lat_len, wrec_fw,     \
+                             wrec_bw, wac_fw, wac_bw, seq_len, out, B, L, H, Kw, C, gates, cstate, norm, wgates, cw, aw, hw)
   if (R == 4) GO(4);
   if (R == 2) GO(2);
   GO(1);
@@ -560,8 +521,9 @@ extern "C" int ner_lattice_recurrence_bwd(const float* d_out, const float* gates
   const size_t smem = bwd_smem(H, C, R, Kw);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
 #define GO(RR)                                                                                                         \
-  return launch_cluster(lattice_bwd_kernel<RR>, B, RR, C, smem, s, d_out, gates, cstate, norm, wgates, cw, aw, lat_len, \
-                        wrec_fw, wrec_bw, wac_fw, wac_bw, seq_len, d_xproj, d_wproj, d_alpha, B, L, H, Kw, C)
+  return rnn::launch_cluster(lattice_bwd_kernel<RR>, B, RR, C, kThreads, smem, s, d_out, gates, cstate, norm, wgates, cw,  \
+                             aw, lat_len, wrec_fw, wrec_bw, wac_fw, wac_bw, seq_len, d_xproj, d_wproj, d_alpha, B, L, H, \
+                             Kw, C)
   if (R == 4) GO(4);
   if (R == 2) GO(2);
   GO(1);
