@@ -26,6 +26,9 @@ SIGNATURES = {
     "ner_crf_loglik_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c.c_float, _vp, _vp, _i, _i, _i, _vp]),
     "ner_crf_partial_loglik_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "ner_crf_partial_loglik_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c.c_float, _vp, _vp, _i, _i, _i, _vp]),
+    "ner_crf_distill_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _c.c_float, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "ner_crf_distill_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _c.c_float, _vp, _vp, _vp, _c.c_float, _vp, _vp, _vp, _i, _i,
+                                 _i, _i, _vp]),
     "ner_crf_viterbi_nbest_workspace_bytes": (_c.c_size_t, [_i, _i, _i, _i]),
     "ner_crf_viterbi_nbest": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _c.c_size_t, _i, _i, _i, _vp]),
     "ner_gemm_bf16": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),

@@ -39,12 +39,15 @@ def load_plugin(model_name):
 class Estimator:
     """Minimal stand-in for tf.estimator.Estimator over one plugin + one variable store."""
 
-    def __init__(self, model_name, params, store=None, device='cuda'):
+    def __init__(self, model_name, params, store=None, device='cuda', teacher=None):
         self.model_name = model_name
         self.build_graph, train_params = load_plugin(model_name)
         self.params = dict(train_params)
         self.params.update(params)
         self.device = torch.device(device)
+        self.teacher = teacher
+        if teacher is not None:
+            self.distill_settings()
         self.store = store or variables.VariableStore(self.device)
         # data-parallel gradient exchange (N > 1): 'overlap' = bucketed all-reduces behind the backward pass, 'overlap_bf16' =
         # the same with bf16 buckets, 'single' = one all-reduce of the flat buffer after the backward pass
@@ -103,6 +106,50 @@ class Estimator:
             raise ValueError(f"{self.model_name} cannot decode crf_nbest = {n} paths: {NBEST_REFUSED[self.model_name]}")
         return int(n)
 
+    def distill_settings(self):
+        """(alpha, tau) of knowledge distillation from self.teacher: params['distill_alpha'] in (0, 1] (default 0.5) and
+        params['distill_temperature'] > 0 (default 1).  ValueError, before anything is launched, for a teacher or
+        student without exactly one CRF, different tag sets, different tokenizers, or a student word-enhance method
+        other than none or the teacher's own: the two CRFs must score the same tags at the same positions."""
+        from .data.base_preprocess import extract_prefix_surfix
+        t = self.teacher
+        for who, name in (("teacher", t.model_name), ("student", self.model_name)):
+            if name in NBEST_REFUSED:
+                raise ValueError(f"cannot distill with {who} {name}: {NBEST_REFUSED[name]}")
+        for key in ('label_size', 'idx2tag'):
+            if t.params.get(key) != self.params.get(key):
+                raise ValueError(f"teacher {t.model_name} and student {self.model_name} have a different {key}")
+        t_we, t_tok = extract_prefix_surfix(t.model_name)
+        s_we, s_tok = extract_prefix_surfix(self.model_name)
+        if t_tok != s_tok:
+            raise ValueError(f"teacher {t.model_name} ({t_tok} tokenizer) and student {self.model_name} ({s_tok} "
+                             f"tokenizer) do not tag the same positions")
+        if s_we is not None and s_we != t_we:
+            raise ValueError(f"student {self.model_name} needs {s_we} features, which teacher {t.model_name}'s "
+                             f"dataset does not carry")
+        a = self.params.get('distill_alpha', 0.5)
+        tau = self.params.get('distill_temperature', 1.0)
+        if isinstance(a, bool) or not isinstance(a, (int, float, np.number)) or not 0 < a <= 1:
+            raise ValueError(f"distill_alpha must be in (0, 1] (got {a!r})")
+        if isinstance(tau, bool) or not isinstance(tau, (int, float, np.number)) or not 0 < tau < float('inf'):
+            raise ValueError(f"distill_temperature must be > 0 (got {tau!r})")
+        return float(a), float(tau)
+
+    def teacher_potentials(self, dev_features):
+        """The teacher's PREDICT-mode emissions [B,L,K] and CRF transitions on a device batch (its `label_mask`
+        dropped, nothing decoded).  The teacher's store is only read."""
+        from .tools import layer
+        feats = {k: v for k, v in dev_features.items() if k != 'label_mask'}
+        saved = layer.CRF_CAPTURE
+        layer.CRF_CAPTURE = captured = []
+        try:
+            self.teacher.forward_device(feats, False)
+        finally:
+            layer.CRF_CAPTURE = saved
+        if len(captured) != 1:
+            raise ValueError(f"teacher {self.teacher.model_name} ran {len(captured)} CRF layers, not one")
+        return captured[0]
+
     @contextlib.contextmanager
     def _layer_settings(self, dev_features):
         """The module settings of tools/layer.py this Estimator's params select, checked before anything is launched."""
@@ -112,7 +159,7 @@ class Estimator:
         ws = self.document_window()
         if ws is not None and torch.is_tensor(dev_features.get('token_ids')):
             windows.check_batch(self.model_name, dev_features['token_ids'].shape[1], ws[0])
-        keys = ('BERT_PRECISION', 'BERT_WINDOW', 'BERT_WINDOW_STRIDE', 'DOCUMENT_REFUSAL', 'CRF_NBEST')
+        keys = ('BERT_PRECISION', 'BERT_WINDOW', 'BERT_WINDOW_STRIDE', 'DOCUMENT_REFUSAL', 'CRF_NBEST', 'CRF_TEACHER')
         saved = {k: getattr(layer, k) for k in keys}
         layer.BERT_PRECISION = self.params.get('bert_precision', saved['BERT_PRECISION'])
         layer.CRF_NBEST = nbest
@@ -279,8 +326,13 @@ class Estimator:
         backward, then the train op the reference picks by model name (:156-164).  -> loss (float)."""
         from .tools import train_utils
         dev = features if all(not torch.is_tensor(v) or v.is_cuda for v in features.values()) else self.to_device(features)
+        teacher = None
+        if self.teacher is not None:
+            teacher = self.teacher_potentials(dev) + self.distill_settings()
         self.store.dropout_calls = 0
         with self._layer_settings(dev), variables.use_store(self.store), autodiff.recording(self.store) as tape:
+            from .tools import layer
+            layer.CRF_TEACHER = teacher
             loss = self.build_graph(dev, None, self.params, True)[0]
             tape.backward()
             p = self.params

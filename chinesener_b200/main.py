@@ -159,15 +159,42 @@ def singletask_train(args):
     _window_params(TRAIN_PARAMS, args)
     if args.crf_nbest != 1:
         TRAIN_PARAMS['crf_nbest'] = args.crf_nbest
-    input_pipe = NerDataset(data_dir, TRAIN_PARAMS['batch_size'], TRAIN_PARAMS['epoch_size'], model_name, seed=args.seed)
+    teacher_ck = None
+    if not args.teacher_model and (args.teacher_dir or args.teacher_pretrain_dir):
+        raise ValueError('--teacher_dir / --teacher_pretrain_dir need --teacher_model')
+    if args.teacher_model:
+        # a missing teacher checkpoint is an error before anything is built, not a randomly initialised teacher
+        teacher_ck = checkpoint.latest_checkpoint(args.teacher_dir) if args.teacher_dir else None
+        if teacher_ck is None:
+            raise ValueError('--teacher_model {} needs --teacher_dir with a checkpoint (found none in {!r})'.format(
+                args.teacher_model, args.teacher_dir))
+        TRAIN_PARAMS['distill_alpha'] = args.distill_alpha
+        TRAIN_PARAMS['distill_temperature'] = args.distill_temperature
+    # with a teacher, the dataset is the teacher's: its features are a superset of the student's
+    input_pipe = NerDataset(data_dir, TRAIN_PARAMS['batch_size'], TRAIN_PARAMS['epoch_size'],
+                            args.teacher_model or model_name, seed=args.seed)
     TRAIN_PARAMS.update(input_pipe.params)       # label_size, max_seq_len, num_train_steps ... (main.py:25)
     print('=' * 10 + 'TRAIN PARAMS' + '=' * 10)
     print(dict((i, j) for i, j in TRAIN_PARAMS.items() if ('emb' not in i) and ('vocab' not in i)))
     print('=' * 10 + 'RUN PARAMS' + '=' * 10)
     print(RUN_CONFIG)
 
-    estimator = engine.Estimator(args.model_name, TRAIN_PARAMS)
+    teacher = None
+    if teacher_ck is not None:
+        teacher_params = dict(engine.load_plugin(args.teacher_model)[1])
+        teacher_params.update(input_pipe.params)
+        if args.teacher_pretrain_dir or args.pretrain_dir:
+            teacher_params['pretrain_dir'] = args.teacher_pretrain_dir or args.pretrain_dir
+        _window_params(teacher_params, args)     # the teacher encodes the same (document-length) batches as the student
+        teacher = engine.Estimator(args.teacher_model, teacher_params)
+        teacher.document_window()                # ValueError before training: a window the teacher's BERT cannot take
+    estimator = engine.Estimator(args.model_name, TRAIN_PARAMS, teacher=teacher)   # ValueError for a pair it cannot distill
     nbest = estimator.crf_nbest()                # ValueError before training: out of range, or a plugin without one CRF
+    if teacher is not None:
+        first = next(iter(input_pipe.build_input_fn('valid', is_predict=True, with_strings=False)()))
+        teacher.evaluate(first)                  # creates the teacher's variables, then the checkpoint overwrites them
+        print('teacher {} from {} (step {})'.format(args.teacher_model, teacher_ck,
+                                                    checkpoint.restore_checkpoint(teacher.store, teacher_ck)))
     estimator.store.gen.manual_seed(args.seed)
     warm = checkpoint.latest_checkpoint(model_dir)
     if warm:
@@ -190,6 +217,9 @@ def singletask_train(args):
     print('{} sentences -> {}'.format(len(prediction), out_pkl))
 
     summary = {'model': model_name, 'data': args.data, 'history': history, 'n_predict': len(prediction), 'seed': args.seed}
+    if teacher is not None:
+        summary['teacher'] = args.teacher_model
+        summary['distill_alpha'], summary['distill_temperature'] = estimator.distill_settings()
     if nbest > 1:
         summary['crf_nbest'] = nbest
         summary['exact_match_at_1'], summary['exact_match_at_n'] = exact_match_rates(prediction, lens)
@@ -306,6 +336,13 @@ def build_parser():
     parser.add_argument('--crf_nbest', type=int, default=1, help='CRF plugins: decode the N best tag paths (1..16) at '
                         'PREDICT; the pickle gains nbest_ids / nbest_scores / nbest_probs and the summary exact_match_at_1 / '
                         'exact_match_at_n')
+    parser.add_argument('--teacher_model', type=str, default='', help='distil from this CRF plugin (a trained teacher); '
+                        'the dataset is opened by its name')
+    parser.add_argument('--teacher_dir', type=str, default='', help="the teacher's checkpoint directory (latest checkpoint)")
+    parser.add_argument('--teacher_pretrain_dir', type=str, default='', help="the teacher's bert_config.json directory "
+                        '(default --pretrain_dir)')
+    parser.add_argument('--distill_alpha', type=float, default=0.5, help='weight of the distillation term, in (0, 1]')
+    parser.add_argument('--distill_temperature', type=float, default=1.0, help='temperature of the distillation term, > 0')
     return parser
 
 
@@ -321,6 +358,8 @@ def main(argv=None):
     if args.device >= 0:
         os.environ['CUDA_VISIBLE_DEVICES'] = '{}'.format(args.device)
     if len(args.data.split(',')) > 1:
+        if args.teacher_model or args.teacher_dir:
+            raise ValueError('multi-task training (--data a,b) cannot distil from a teacher')
         return multitask_train(args)
     return singletask_train(args)
 

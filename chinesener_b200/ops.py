@@ -510,6 +510,43 @@ def crf_partial_loglik_bwd(logits, label_mask, seq_len, trans, alpha, logz, d_ll
     return d_logits, d_trans
 
 
+def crf_distill_fwd(t_logits, t_trans, s_logits, s_trans, seq_len, temperature=1.0, exact=False):
+    """Forward half of CRF-to-CRF distillation at temperature tau (ner_crf_distill_fwd): teacher and student share
+    [B,L,K].  -> logz [B,2] (logZ_T, logZ_S of the tau-scaled CRFs), alpha [2,B,L,K] for crf_distill_bwd."""
+    require_cuda(t_logits, t_trans, s_logits, s_trans, seq_len)
+    assert all(t.dtype == torch.float32 for t in (t_logits, t_trans, s_logits, s_trans))
+    B, L, K = s_logits.shape
+    assert t_logits.shape == (B, L, K) and t_trans.shape == (K, K) and s_trans.shape == (K, K)
+    t_logits, s_logits = t_logits.contiguous(), s_logits.contiguous()
+    logz = torch.empty((B, 2), dtype=torch.float32, device=s_logits.device)
+    alpha = torch.empty((2, B, L, K), dtype=torch.float32, device=s_logits.device)
+    check(lib().ner_crf_distill_fwd(ptr(t_logits), ptr(t_trans.contiguous()), ptr(s_logits), ptr(s_trans.contiguous()),
+                                    ptr(_i32(seq_len)), 1.0 / float(temperature), ptr(logz), ptr(alpha), B, L, K,
+                                    1 if exact else 0, stream()))
+    return logz, alpha
+
+
+def crf_distill_bwd(t_logits, t_trans, s_logits, s_trans, seq_len, alpha, logz, temperature=1.0, d_kl=None, scale=1.0,
+                    exact=False):
+    """-> kl [B] (KL(teacher || student) over all paths at temperature tau), d_s_logits [B,L,K], d_s_trans [K,K] of
+    sum_b g_b KL_b, g_b = (d_kl|1) * scale (ner_crf_distill_bwd).  The teacher gets no gradient."""
+    require_cuda(t_logits, t_trans, s_logits, s_trans, seq_len, alpha, logz, d_kl)
+    B, L, K = s_logits.shape
+    assert all(t.dtype == torch.float32 for t in (t_logits, t_trans, s_logits, s_trans, alpha, logz)
+               + ((d_kl,) if d_kl is not None else ()))
+    assert t_logits.shape == (B, L, K) and alpha.shape == (2, B, L, K) and logz.shape == (B, 2)
+    assert d_kl is None or d_kl.shape == (B,)
+    t_logits, s_logits = t_logits.contiguous(), s_logits.contiguous()
+    kl = torch.empty((B,), dtype=torch.float32, device=s_logits.device)
+    d_logits = torch.empty_like(s_logits)
+    d_trans = torch.zeros_like(s_trans)
+    check(lib().ner_crf_distill_bwd(ptr(t_logits), ptr(t_trans.contiguous()), ptr(s_logits), ptr(s_trans.contiguous()),
+                                    ptr(_i32(seq_len)), 1.0 / float(temperature), ptr(alpha), ptr(logz),
+                                    ptr(None if d_kl is None else d_kl.contiguous()), scale, ptr(kl), ptr(d_logits),
+                                    ptr(d_trans), B, L, K, 1 if exact else 0, stream()))
+    return kl, d_logits, d_trans
+
+
 # --------------------------------------------------------------------------- fp32-accurate dense (split bf16)
 def split_bf16(x2d, Dp=None):
     """f32 [M,D] -> (hi, lo) bf16 [M,Dp] with hi + lo ~= x to 2^-17."""

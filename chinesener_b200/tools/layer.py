@@ -31,6 +31,12 @@ DOCUMENT_REFUSAL = None
 # N-best decoding: with CRF_NBEST > 1, crf_decode outside TRAIN also returns the CRF_NBEST best paths (as attributes of
 # pred_ids, whose values stay the Viterbi path).  Estimator sets it from params['crf_nbest'] around build_graph.
 CRF_NBEST = 1
+# Knowledge distillation (Estimator(teacher=...)): CRF_TEACHER = (teacher logits [B,L,K], teacher transitions, alpha, tau)
+# makes crf_layer in TRAIN return the row value (1 - alpha) ll - alpha tau^2 KL(teacher || student), so a plugin's
+# (-ll).mean() is the distillation loss.  CRF_CAPTURE = [] makes crf_layer append its (logits, transitions) there and
+# crf_decode decode nothing: how Estimator reads the teacher's potentials.  Estimator sets both around build_graph.
+CRF_TEACHER = None
+CRF_CAPTURE = None
 
 
 class TrainingPathNotBuilt(NotImplementedError):
@@ -591,6 +597,8 @@ def crf_layer(logits, label_ids, seq_len, label_size, is_training, label_mask=No
     log-likelihood is that of the partial-annotation CRF (ner_crf_partial_loglik_fwd); label_ids is then not read."""
     tname = variables.scoped("crf_layer/transitions")
     trans = variables.get_variable(tname, (label_size, label_size), variables.xavier)
+    if CRF_CAPTURE is not None and not is_training:
+        CRF_CAPTURE.append((logits, trans))
     if label_ids is None:
         return trans, None
     if label_mask is None:
@@ -598,6 +606,8 @@ def crf_layer(logits, label_ids, seq_len, label_size, is_training, label_mask=No
     else:
         fwd, bwd_op, labels = ops.crf_partial_loglik_fwd, ops.crf_partial_loglik_bwd, label_mask
     tape = autodiff.current()
+    if is_training and tape is not None and CRF_TEACHER is not None:
+        return trans, _distilled_loglik(logits, labels, seq_len, trans, tname, fwd, bwd_op, tape)
     if is_training and tape is not None:
         store = variables.default_store()
         lg = logits.contiguous()
@@ -614,6 +624,40 @@ def crf_layer(logits, label_ids, seq_len, label_size, is_training, label_mask=No
         return trans, ll
     # EVAL / PREDICT: built lazily — evaluated when the loss is fetched (EVAL), never in PREDICT
     return trans, variables.Deferred(lambda: fwd(logits, labels, seq_len, trans)[0])
+
+
+def _distilled_loglik(logits, labels, seq_len, trans, tname, fwd, bwd_op, tape):
+    """TRAIN row value ll' = (1 - a) ll - a tau^2 KL_b with CRF_TEACHER = (t_logits, t_trans, a, tau), and its tape entry.
+    KL_b is written by the distillation backward kernel, so that kernel runs here, with the coefficient the plugins'
+    (-ll').mean() gives it (a tau^2 / B); a tape that seeds another gradient reruns it with that one.  The gold term is
+    skipped at a = 1.  The teacher's potentials get no gradient."""
+    t_logits, t_trans, a, tau = CRF_TEACHER
+    store = variables.default_store()
+    lg = logits.contiguous()
+    B = lg.shape[0]
+    c = float(a) * float(tau) ** 2
+    logz_d, alpha_d = ops.crf_distill_fwd(t_logits, t_trans, lg, trans, seq_len, tau)
+    kl, dl_kl, dt_kl = ops.crf_distill_bwd(t_logits, t_trans, lg, trans, seq_len, alpha_d, logz_d, tau, scale=c / B)
+    gold = None
+    row = kl * -c
+    if a < 1:
+        gold = fwd(lg, labels, seq_len, trans, want_alpha=True)
+        row = row + gold[0] * (1.0 - a)
+
+    def bwd(g):
+        if g is None:                       # loss = mean(-ll'): d loss / d ll'_b = -1/B
+            d_logits, d_trans = dl_kl, dt_kl
+        else:
+            _, d_logits, d_trans = ops.crf_distill_bwd(t_logits, t_trans, lg, trans, seq_len, alpha_d, logz_d, tau,
+                                                       d_kl=(g * -c).contiguous())
+        if gold is not None:
+            d_ll = g if g is not None else torch.full((B,), -1.0 / B, dtype=torch.float32, device=lg.device)
+            dl_g, dt_g = bwd_op(lg, labels, seq_len, trans, gold[2], gold[1], d_ll.contiguous(), 1.0 - a)
+            d_logits, d_trans = d_logits + dl_g, d_trans + dt_g
+        store.grad(tname).add_(d_trans)
+        tape.add_grad(logits, d_logits)
+    tape.record(row, bwd)
+    return row
 
 
 def concat(tensors, is_training=False):
@@ -684,6 +728,8 @@ def crf_decode(logits, trans, seq_len, idx2tag, is_training, mask=None):
     CRF_NBEST > 1 (PREDICT / EVAL): pred_ids is rank 0 of ops.crf_viterbi_nbest, the same tags, and carries the
     CRF_NBEST best paths as .nbest_ids [B,N,L] int32, .nbest_scores [B,N] f32, .nbest_counts [B] int32 and .nbest_logz
     [B] f32 (log Z of ner_crf_loglik_fwd), so that path r has probability exp(nbest_scores[:, r] - nbest_logz)."""
+    if CRF_CAPTURE is not None and not is_training:
+        return torch.zeros(logits.shape[:2], dtype=torch.int32, device=logits.device)
     if CRF_NBEST <= 1 or is_training:
         return ops.crf_viterbi(logits, seq_len, trans)
     tags, scores, counts = ops.crf_viterbi_nbest(logits, seq_len, trans, CRF_NBEST)

@@ -112,6 +112,33 @@ int ner_crf_partial_loglik_bwd(const float* logits, const int32_t* label_mask, c
                                const float* trans, const float* alpha_ws, const float* logz, const float* d_ll,
                                float scale, float* d_logits, float* d_trans, int B, int L, int K, ner_stream_t stream);
 
+/* CRF-to-CRF knowledge distillation, forward half (csrc/crf_distill.cu).  A teacher CRF (t_logits [B,L,K],
+ * t_trans [K,K]) and a student CRF (s_logits, s_trans) over the same K tags define, at temperature tau = 1/inv_temp,
+ * the path distributions p^tau(y) ~ exp(score(y) / tau).  One pass runs both forward recursions on the potentials
+ * scaled by inv_temp as they are read, and writes:
+ *   logz [B,2] f32: (logZ_T, logZ_S) of p^tau, 0 for seq_len <= 0;  alpha_ws [2,B,L,K] f32: (alpha_T, alpha_S).
+ * Both are required and feed ner_crf_distill_bwd.  seq_len > L counts as L.  flags: bit0 = force the exact
+ * (per-column max) logsumexp path; without it the scaled-probability step runs when both scaled transition
+ * matrices span < 30 nats and are finite.  NER_ERR_INVALID_ARG for B < 0, L < 1, K < 1, inv_temp not a positive
+ * finite number, or a null pointer (B > 0); NER_ERR_UNSUPPORTED for K > 32 or L > 4095.  B = 0 is a no-op. */
+int ner_crf_distill_fwd(const float* t_logits, const float* t_trans, const float* s_logits, const float* s_trans,
+                        const int32_t* seq_len, float inv_temp, float* logz, float* alpha_ws, int B, int L, int K,
+                        int flags, ner_stream_t stream);
+
+/* CRF-to-CRF knowledge distillation, backward half: both backward recursions in one reverse pass.  With mu / xi the
+ * unary / pairwise marginals of p^tau and g_b = (d_kl ? d_kl[b] : 1) * scale:
+ *   kl[b] = sum_t mu_T[t]·(x_T - x_S)[t] / tau + sum_{t>=1} xi_T[t]·(T_T - T_S) / tau - logZ_T + logZ_S   (KL(T||S))
+ *   d_s_logits[b,t,j] = g_b * (mu_S[t][j] - mu_T[t][j]) / tau                       (0 beyond seq_len)
+ *   d_s_trans[i,j]   += sum_b g_b * sum_{t>=1} (xi_S[t][i][j] - xi_T[t][i][j]) / tau
+ * A term whose teacher marginal is 0 adds 0 to kl (a teacher transition of -inf).  seq_len <= 0: kl = 0, no gradient.
+ * A teacher equal to the student gives kl = 0.0 and zero gradients exactly.  alpha_ws / logz from ner_crf_distill_fwd
+ * with the same inputs; kl [B], d_s_logits [B,L,K] (fully written) and d_s_trans (accumulated into, as for
+ * ner_crf_loglik_bwd) are required, d_kl is optional.  flags and error codes as ner_crf_distill_fwd. */
+int ner_crf_distill_bwd(const float* t_logits, const float* t_trans, const float* s_logits, const float* s_trans,
+                        const int32_t* seq_len, float inv_temp, const float* alpha_ws, const float* logz,
+                        const float* d_kl, float scale, float* kl, float* d_s_logits, float* d_s_trans, int B, int L,
+                        int K, int flags, ner_stream_t stream);
+
 /* N-best extension of tools/layer.py:140-142's tf.contrib.crf.crf_decode: the N highest-scoring tag paths of every
  * sequence, best first (list Viterbi, csrc/crf_nbest.cu).  Row b decodes n = min(max(seq_len[b], 1), L) positions, as
  * ner_crf_viterbi does.  A path's score is the fp32 left-to-right sum s_0 = x[0][y_0],
