@@ -61,6 +61,9 @@ SIGNATURES = {
     "ner_token_xent": (_i, [_vp] * 6 + [_c.c_float, _vp, _i, _i, _i, _vp]),
     "ner_token_xent_scratch_floats": (_c.c_size_t, []),
     "ner_token_dice": (_i, [_vp] * 6 + [_c.c_float] * 3 + [_vp, _i, _i, _i, _vp]),
+    "ner_mlm_mask": (_i, [_vp] * 4 + [_i, _i, _c.c_uint64, _i, _i] + [_vp] * 4),
+    "ner_vocab_xent_scratch_floats": (_c.c_size_t, [_i]),
+    "ner_vocab_xent": (_i, [_vp, _i, _vp, _i, _i, _c.c_float] + [_vp] * 7),
     "ner_mrc_pairs": (_i, [_vp] * 6 + [_i] * 6 + [_vp] * 7),
     "ner_mrc_merge": (_i, [_vp] * 3 + [_i] * 6 + [_vp, _vp]),
     "ner_mrc_span_targets": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),

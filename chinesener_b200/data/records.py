@@ -32,7 +32,7 @@ MAGIC = b'NERREC01'
 _ALIGN = 64
 # features that travel to the device (dataset.py:21-37) and the dtype build_graph receives them in
 DEVICE_INT = ('token_ids', 'mask', 'segment_ids', 'label_ids', 'seq_len', 'softword_ids', 'bichar_ids', 'softlexicon_ids',
-              'task_ids', 'lattice_ids', 'lattice_lens', 'label_mask')
+              'task_ids', 'lattice_ids', 'lattice_lens', 'label_mask', 'word_start')
 DEVICE_FLOAT = ('softlexicon_weights', 'ex_softword_ids')
 STRING_COLS = ('tokens', 'labels')
 PAD_STRING = '[PAD]'

@@ -714,6 +714,46 @@ def token_dice(logits, labels, seq_len, alpha=1.0, gamma=1.0, want_pred=True, wa
     return pred, loss, dz
 
 
+# --------------------------------------------------------------------------- masked-LM pretraining (mlm.py)
+def mlm_mask(token_ids, seq_len, pred_offsets, M, seed, V, mask_id, word_start=None):
+    """Dynamic whole-word masking (ner_mlm_mask) -> (masked_ids [B,L] i32, positions [M] i32, labels [M] i32).
+    pred_offsets [B+1] i32 is the exclusive prefix sum of the per-row budgets and M = pred_offsets[B], known on the host."""
+    require_cuda(token_ids, seq_len, pred_offsets, word_start)
+    B, L = token_ids.shape
+    token_ids, seq_len, pred_offsets = _i32(token_ids), _i32(seq_len), _i32(pred_offsets)
+    assert tuple(seq_len.shape) == (B,) and tuple(pred_offsets.shape) == (B + 1,)
+    if word_start is not None:
+        assert word_start.dtype == torch.uint8 and tuple(word_start.shape) == (B, L)
+    dev = token_ids.device
+    masked = torch.empty((B, L), dtype=torch.int32, device=dev)
+    pos_buf = torch.empty((max(M, 1),), dtype=torch.int32, device=dev)      # one slot at M = 0: never a null pointer
+    lab_buf = torch.empty((max(M, 1),), dtype=torch.int32, device=dev)
+    check(lib().ner_mlm_mask(ptr(token_ids), ptr(seq_len), ptr(word_start), ptr(pred_offsets), B, L,
+                             int(seed) & 0xFFFFFFFFFFFFFFFF, V, mask_id, ptr(masked), ptr(pos_buf), ptr(lab_buf), stream()))
+    return masked, pos_buf[:M], lab_buf[:M]
+
+
+def vocab_xent(logits, labels, V, want_pred=True, want_grad=False, d_loss=1.0):
+    """Masked-LM cross-entropy over logits [M, ld] f32, classes in columns < V (ner_vocab_xent).
+    -> (loss [] f32, count [] i32, correct [] i32, pred [M] i32 | None, d_logits [M, ld] bf16 | None).  Labels outside
+    [0, V) (-1: an unused prediction slot) are not counted; d_logits = d_loss * d loss / d logits, 0 there and in the
+    columns >= V."""
+    require_cuda(logits, labels)
+    assert logits.dtype == torch.float32 and logits.dim() == 2 and labels.dtype == torch.int32
+    M, ld = logits.shape
+    assert tuple(labels.shape) == (M,)
+    dev = logits.device
+    loss = torch.zeros((), dtype=torch.float32, device=dev)
+    count = torch.zeros((), dtype=torch.int32, device=dev)
+    correct = torch.zeros((), dtype=torch.int32, device=dev)
+    pred = torch.empty((M,), dtype=torch.int32, device=dev) if want_pred else None
+    dz = torch.empty((M, ld), dtype=torch.bfloat16, device=dev) if want_grad else None
+    scratch = torch.empty(int(lib().ner_vocab_xent_scratch_floats(M)), dtype=torch.float32, device=dev)
+    check(lib().ner_vocab_xent(ptr(logits), ld, ptr(labels), M, V, float(d_loss), ptr(loss), ptr(count), ptr(correct),
+                               ptr(pred), ptr(dz), ptr(scratch), stream()))
+    return loss, count, correct, pred, dz
+
+
 # --------------------------------------------------------------------------- MRC pairs and tag merge (bert_mrc)
 def mrc_pairs(token_ids, seq_len, query_ids, query_len, type_tag, L2, sep_id, label_ids=None):
     """[B, L] BERT batch -> its B*T query/context pairs (ner_mrc_pairs): dict of ids / segment_ids / mask [B*T, L2] i32,

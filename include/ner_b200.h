@@ -636,6 +636,38 @@ int ner_token_xent(const float* logits, const int32_t* labels, const int32_t* se
 int ner_token_dice(const float* logits, const int32_t* labels, const int32_t* seq_len, int32_t* pred_ids, float* loss,
                    float* d_logits, float d_loss, float alpha, float gamma, float* scratch, int B, int L, int K,
                    ner_stream_t stream);
+/* ---- masked-LM pretraining (chinesener_b200/mlm.py; a restatement of google-research/bert's create_pretraining_data.py
+ * and run_pretraining.py, not pinned to them) ---- */
+#define NER_MLM_MAX_LEN 512       /* L of ner_mlm_mask */
+#define NER_MLM_MAX_VOCAB 50000   /* V of both entry points */
+/* Dynamic whole-word masking of token_ids [B,L] i32.  Row b: n = clamp(seq_len[b], 0, L); candidates are the positions
+ * 1 .. n-2 ([CLS] at 0 and [SEP] at n-1 are never chosen).  A word is a maximal run of candidates starting at a position
+ * with word_start[b,t] = 1 (or at position 1) followed by positions with word_start = 0; word_start [B,L] u8 NULL makes
+ * every candidate its own word.  With h_k(b, t) = hash3(lo(seed) + k * 0x9E3779B9, hi(seed) ^ b, t) (common.cuh), word w
+ * starting at s_w gets the key h_0(b, s_w); the words are walked in (key, s_w) order and a word is taken when
+ * taken + |w| <= k_b, else skipped (k_b = pred_offsets[b+1] - pred_offsets[b], the row's budget, computed by the caller).
+ * Every position t of a taken word is a prediction: with u = (h_1(b, t) >> 8) / 2^24, masked_ids[b,t] = mask_id for
+ * u < 0.8, umulhi(h_2(b, t), V) (a uniform id in [0, V)) for 0.8 <= u < 0.9, else token_ids[b,t]; every other element
+ * of masked_ids is token_ids.  positions / labels [M = pred_offsets[B]] i32: from pred_offsets[b] on, b*L + t and
+ * token_ids[b,t] of row b's predictions in ascending t, then its unused slots (skipped words can leave fewer than k_b)
+ * with b*L and -1.  B < 0, L < 1, V < 1, mask_id outside [0, V) or a null pointer (word_start aside) is
+ * NER_ERR_INVALID_ARG; L > NER_MLM_MAX_LEN, V > NER_MLM_MAX_VOCAB or B*L >= 2^31 is NER_ERR_UNSUPPORTED; all before any
+ * CUDA call.  B = 0 is a no-op.  One launch, no allocation, no atomics, bit-identical repeats. */
+int ner_mlm_mask(const int32_t* token_ids, const int32_t* seq_len, const uint8_t* word_start, const int32_t* pred_offsets,
+                 int B, int L, uint64_t seed, int V, int mask_id, int32_t* masked_ids, int32_t* positions, int32_t* labels,
+                 ner_stream_t stream);
+/* Masked-LM loss, gradient and argmax over logits [M, ld] f32 (columns 0 .. V-1 are the classes).  A row is counted when
+ * 0 <= labels[r] < V; other labels, -1 included, add nothing to any output but pred.  count [1] = the counted rows;
+ * loss [1] = sum over counted rows of (logsumexp(z) - z[y]) / count, 0 when count = 0; correct [1] = counted rows whose
+ * first argmax equals the label; pred [M] (nullable) = the first argmax of every row.  d_logits [M, ld] bf16 (nullable,
+ * fully written) = d_loss / count * (softmax(z) - onehot(y)) on counted rows in columns < V, exactly 0 elsewhere.
+ * Deterministic: per-row losses in scratch (>= ner_vocab_xent_scratch_floats(M) floats) summed in index order; no float
+ * atomics; the count is taken on the device.  M < 0, V < 1, ld < V, ld % 4 != 0, a logits pointer not 16-byte aligned, a
+ * d_logits pointer not 8-byte aligned or a null logits / labels / loss / count / correct / scratch is NER_ERR_INVALID_ARG;
+ * V > NER_MLM_MAX_VOCAB is NER_ERR_UNSUPPORTED; all before any CUDA call.  M = 0 is a no-op.  Three launches. */
+size_t ner_vocab_xent_scratch_floats(int M);
+int ner_vocab_xent(const float* logits, int ld, const int32_t* labels, int M, int V, float d_loss, float* loss,
+                   int32_t* count, int32_t* correct, int32_t* pred, void* d_logits, float* scratch, ner_stream_t stream);
 /* model/bert_mrc.py (MRC-style NER, one BERT query per entity type; a restatement, not pinned to the reference's mrc/):
  * expands the [B,L] BERT batch (token_ids, seq_len [B] counting [CLS] and [SEP]) into the B*T pairs p = b*T + t,
  *   pair row p = token_ids[b,0] ([CLS]), query_ids[t, 0:q_t], sep_id, token_ids[b, 1:len_b]
