@@ -44,6 +44,7 @@ SIGNATURES = {
     "ner_bilstm_recurrence_bwd": (_i, [_vp] * 7 + [_i, _i, _i, _i, _c.c_float, _c.c_uint64, _vp]),
     "ner_bigru_recurrence": (_i, [_vp] * 5 + [_i, _i, _i, _i, _i] + [_vp] * 4 + [_c.c_float, _c.c_uint64, _vp]),
     "ner_bigru_recurrence_bwd": (_i, [_vp] * 7 + [_i, _i, _i, _i, _c.c_float, _c.c_uint64, _vp]),
+    "ner_rnn_plan": (_i, [_i] * 5 + [_c.POINTER(_i)] * 3),
     "ner_transpose_cast_bf16": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "ner_colsum_add": (_i, [_vp, _vp, _i, _i, _i, _c.c_float, _vp]),
     "ner_dense_small_n_bwd": (_i, [_vp] * 6 + [_i, _i, _i, _vp]),

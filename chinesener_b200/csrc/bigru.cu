@@ -298,11 +298,10 @@ extern "C" int ner_bigru_recurrence(const float* xproj, const float* wh_fw, cons
     return NER_ERR_INVALID_ARG;
   if (!(keep_prob > 0.f) || keep_prob > 1.f) return NER_ERR_INVALID_ARG;
   if (activation != 0 && activation != 1) return NER_ERR_INVALID_ARG;
-  if (H % 4 != 0) return NER_ERR_UNSUPPORTED;
-  const int C = rnn::gru_pick_cluster(H);
-  if (C == 0) return NER_ERR_UNSUPPORTED;
+  int R, C;
+  const int status = ner_rnn_plan(NER_RNN_GRU_FWD, B, H, 0, ner_num_sms(), &R, &C, nullptr);
+  if (status != NER_OK) return status;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int R = rnn::rows_per_cluster(B, C);
 #define GO(RR)                                                                                                         \
   return activation == 1                                                                                               \
              ? launch_rec<RR, 1>(xproj, wh_fw, wh_bw, seq_len, out, B, L, H, ld_xproj, C, cu_seqlens, gates_out, hstate_out,     \

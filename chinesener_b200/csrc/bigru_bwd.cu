@@ -227,11 +227,10 @@ extern "C" int ner_bigru_recurrence_bwd(const float* d_out, const float* gates, 
   if (!d_out || !gates || !hstate || !wh_fw || !wh_bw || !seq_len || !d_xproj) return NER_ERR_INVALID_ARG;
   if (!(keep_prob > 0.f) || keep_prob > 1.f) return NER_ERR_INVALID_ARG;
   if (activation != 0 && activation != 1) return NER_ERR_INVALID_ARG;
-  if (H % 4 != 0) return NER_ERR_UNSUPPORTED;
-  const int C = rnn::gru_pick_cluster(H);
-  if (C == 0) return NER_ERR_UNSUPPORTED;
+  int R, C;
+  const int status = ner_rnn_plan(NER_RNN_GRU_BWD, B, H, 0, ner_num_sms(), &R, &C, nullptr);
+  if (status != NER_OK) return status;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int R = rnn::rows_per_cluster(B, C);
 #define GO(RR)                                                                                                       \
   return activation == 1 ? launch_bwd<RR, 1>(d_out, gates, hstate, wh_fw, wh_bw, seq_len, d_xproj, B, L, H, C,      \
                                              keep_prob, seed, st)                                                    \

@@ -222,16 +222,6 @@ __global__ void __launch_bounds__(H4REG > 0 ? 256 : 512, 1) bilstm_rec_kernel(co
   rnn::zero_past_maxlen(out, R, b0, B, L, H, dir, rank, HU, maxlen);
 }
 
-int pick_cluster(int H) {
-  // smallest power-of-two cluster whose W_h slice (H * 4H/C floats) fits ~190 KB and divides H
-  for (int C = 1; C <= 8; C *= 2) {
-    if (H % C != 0) continue;
-    const size_t bytes = (size_t)H * 4 * (H / C) * 4;
-    if (bytes <= 190 * 1024 && 4 * (H / C) <= 512) return C;
-  }
-  return 0;
-}
-
 template <int R, int ACT, int H4REG>
 int launch_rec(const float* xproj, const float* wh_fw, const float* wh_bw, const int32_t* seq_len, float* out, int B,
                int L, int H, int C, float forget_bias, const int32_t* cu_seqlens, float* gates_out, float* cstate_out,
@@ -256,22 +246,19 @@ extern "C" int ner_bilstm_recurrence(const float* xproj, const float* wh_fw, con
   if ((gates_out == nullptr) != (cstate_out == nullptr)) return NER_ERR_INVALID_ARG;
   if (!(keep_prob > 0.f) || keep_prob > 1.f) return NER_ERR_INVALID_ARG;
   if (activation != 0 && activation != 1) return NER_ERR_INVALID_ARG;
-  if (H % 4 != 0) return NER_ERR_UNSUPPORTED;
-  const int C = pick_cluster(H);
-  if (C == 0) return NER_ERR_UNSUPPORTED;
+  int R, C, resident;
+  const int status = ner_rnn_plan(NER_RNN_LSTM_FWD, B, H, 0, ner_num_sms(), &R, &C, &resident);
+  if (status != NER_OK) return status;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int R = rnn::rows_per_cluster(B, C);
-  // four stacked PREDICT batches (B = 256): 4 rows per cluster would be 256 CTAs = two waves of the one-CTA-per-SM kernel
-  if (H == 128 && (long)2 * ((B + 3) / 4) * C > ner_num_sms()) R = 8;
 #define GO(RR, HR)                                                                                          \
   return activation == 1 ? launch_rec<RR, 1, HR>(xproj, wh_fw, wh_bw, seq_len, out, B, L, H, C, forget_bias, cu_seqlens, gates_out, cstate_out, hstate_out, keep_prob, seed, st) \
                          : launch_rec<RR, 0, HR>(xproj, wh_fw, wh_bw, seq_len, out, B, L, H, C, forget_bias, cu_seqlens, gates_out, cstate_out, hstate_out, keep_prob, seed, st)
-  if (H == 128 && 4 * (H / C) <= 256) {  // register-resident W_h (the bert_bilstm_crf / bilstm_crf shape)
-    if (R == 8) GO(8, 32);   // (R == 4 does not reach here: its rule implies the R = 8 rule)
+  if (resident) {   // register-resident W_h (H = 128: the bert_bilstm_crf / bilstm_crf shape)
+    if (R == 8) GO(8, 32);
     if (R == 2) GO(2, 32);
     GO(1, 32);
   }
-  if (R >= 4) GO(4, 0);
+  if (R == 4) GO(4, 0);
   if (R == 2) GO(2, 0);
   GO(1, 0);
 #undef GO

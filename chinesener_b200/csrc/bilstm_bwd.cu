@@ -209,15 +209,6 @@ bilstm_bwd_kernel(const float* __restrict__ d_out, const float* __restrict__ gat
   }
 }
 
-int pick_cluster_bwd(int H) {
-  for (int C = 1; C <= 8; C *= 2) {
-    if (H % C != 0) continue;
-    const size_t bytes = (size_t)4 * H * (H / C + 1) * 4;
-    if (bytes <= 180 * 1024) return C;
-  }
-  return 0;
-}
-
 template <int R, int ACT, int WR>
 int launch_bwd(const float* d_out, const float* gates, const float* cstate, const float* wh_fw, const float* wh_bw,
                const int32_t* seq_len, float* d_xproj, int B, int L, int H, int C, float keep_prob, uint64_t seed,
@@ -244,15 +235,14 @@ extern "C" int ner_bilstm_recurrence_bwd(const float* d_out, const float* gates,
   if (B == 0) return NER_OK;
   if (!d_out || !gates || !cstate || !wh_fw || !wh_bw || !seq_len || !d_xproj) return NER_ERR_INVALID_ARG;
   if (activation != 0 && activation != 1) return NER_ERR_INVALID_ARG;
-  const int C = pick_cluster_bwd(H);
-  if (C == 0 || (H / C) > 256) return NER_ERR_UNSUPPORTED;
+  int R, C, resident;
+  const int status = ner_rnn_plan(NER_RNN_LSTM_BWD, B, H, 0, ner_num_sms(), &R, &C, &resident);
+  if (status != NER_OK) return status;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int R = min(rnn::rows_per_cluster(B, C), 2);
-  if (2 * (H / C) > 512) R = 1;
 #define GO(RR, WRR)                                                                                                \
   return activation == 1 ? launch_bwd<RR, 1, WRR>(d_out, gates, cstate, wh_fw, wh_bw, seq_len, d_xproj, B, L, H, C, keep_prob, seed, st) \
                          : launch_bwd<RR, 0, WRR>(d_out, gates, cstate, wh_fw, wh_bw, seq_len, d_xproj, B, L, H, C, keep_prob, seed, st)
-  if (H == 128 && C == 2) {   // register-resident recurrent matrix: 4H / 4 = 128 columns per thread
+  if (resident) {   // register-resident recurrent matrix (H = 128, C = 2): 4H / 4 = 128 columns per thread
     if (R == 2) GO(2, 128);
     GO(1, 128);
   }

@@ -455,12 +455,16 @@ int pick_cluster(int H, int R, int Kw) {
   return 0;
 }
 
+}  // namespace
+
 // Rows per cluster: one wave of CTAs over the SMs when the batch allows, as in bilstm.cu.
-void pick_config(int B, int H, int Kw, int* R_out, int* C_out) {
-  const int sms = ner_num_sms();
+int rnn::lattice_config(int B, int H, int Kw, int num_sms, int* R_out, int* C_out) {
+  if (B < 0 || H < 1 || Kw < 1) return NER_ERR_INVALID_ARG;
+  if (Kw > kMaxKw) return NER_ERR_UNSUPPORTED;
   int R = 1, C = pick_cluster(H, 1, Kw);
+  if (C == 0) return NER_ERR_UNSUPPORTED;
   for (int r = 2; r <= 4; r *= 2) {
-    if ((long)2 * ((B + R - 1) / R) * C <= sms) break;
+    if ((long)2 * ((B + R - 1) / R) * C <= num_sms) break;
     const int c = pick_cluster(H, r, Kw);
     if (c == 0) break;
     R = r;
@@ -468,13 +472,15 @@ void pick_config(int B, int H, int Kw, int* R_out, int* C_out) {
   }
   *R_out = R;
   *C_out = C;
+  return NER_OK;
 }
 
-int check_shape(int B, int L, int H, int Kw) {
-  if (B < 0 || L < 1 || H < 1 || Kw < 1) return NER_ERR_INVALID_ARG;
-  if (Kw > kMaxKw) return NER_ERR_UNSUPPORTED;
-  if (pick_cluster(H, 1, Kw) == 0) return NER_ERR_UNSUPPORTED;
-  return NER_OK;
+namespace {
+
+// The instantiation of a call of `kernel`: NER_OK and (R, C) from ner_rnn_plan, or the status to return.
+int check_shape(int kernel, int B, int L, int H, int Kw, int* R, int* C) {
+  if (L < 1) return NER_ERR_INVALID_ARG;
+  return ner_rnn_plan(kernel, B, H, Kw, ner_num_sms(), R, C, nullptr);
 }
 
 }  // namespace
@@ -484,7 +490,8 @@ extern "C" int ner_lattice_recurrence(const float* xproj, const float* wproj, co
                                       const int32_t* seq_len, float* out, int B, int L, int H, int Kw, float* gates,
                                       float* cstate, float* norm, float* wgates, float* cw, float* aw, float* hw,
                                       ner_stream_t stream) {
-  const int st = check_shape(B, L, H, Kw);
+  int R, C;
+  const int st = check_shape(NER_RNN_LATTICE_FWD, B, L, H, Kw, &R, &C);
   if (st != NER_OK) return st;
   if (B == 0) return NER_OK;
   if (!xproj || !wproj || !lat_len || !wrec_fw || !wrec_bw || !wac_fw || !wac_bw || !seq_len || !out)
@@ -492,8 +499,6 @@ extern "C" int ner_lattice_recurrence(const float* xproj, const float* wproj, co
   const int n_saved = (gates != nullptr) + (cstate != nullptr) + (norm != nullptr) + (wgates != nullptr) +
                       (cw != nullptr) + (aw != nullptr) + (hw != nullptr);
   if (n_saved != 0 && n_saved != 7) return NER_ERR_INVALID_ARG;
-  int R, C;
-  pick_config(B, H, Kw, &R, &C);
   const size_t smem = fwd_smem(H, C, R, Kw);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
 #define GO(RR)                                                                                                        \
@@ -510,14 +515,13 @@ extern "C" int ner_lattice_recurrence_bwd(const float* d_out, const float* gates
                                           const float* wrec_fw, const float* wrec_bw, const float* wac_fw,
                                           const float* wac_bw, const int32_t* seq_len, float* d_xproj, float* d_wproj,
                                           float* d_alpha, int B, int L, int H, int Kw, ner_stream_t stream) {
-  const int st = check_shape(B, L, H, Kw);
+  int R, C;
+  const int st = check_shape(NER_RNN_LATTICE_BWD, B, L, H, Kw, &R, &C);
   if (st != NER_OK) return st;
   if (B == 0) return NER_OK;
   if (!d_out || !gates || !cstate || !norm || !wgates || !cw || !aw || !lat_len || !wrec_fw || !wrec_bw || !wac_fw ||
       !wac_bw || !seq_len || !d_xproj || !d_wproj || !d_alpha)
     return NER_ERR_INVALID_ARG;
-  int R, C;
-  pick_config(B, H, Kw, &R, &C);
   const size_t smem = bwd_smem(H, C, R, Kw);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
 #define GO(RR)                                                                                                         \

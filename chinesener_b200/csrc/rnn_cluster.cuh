@@ -181,13 +181,34 @@ int launch_cluster(K kern, int B, int R, int C, int threads, size_t smem, cudaSt
   return ner_launch_status();
 }
 
-// Rows per cluster of the BiLSTM and BiGRU recurrences: fill the SMs once when the batch is small, amortise the weight
-// reads when it is large.
-static inline int rows_per_cluster(int B, int C) {
+// Rows per cluster of the BiLSTM and BiGRU recurrences: fill the num_sms SMs once when the batch is small, amortise the
+// weight reads when it is large.
+static inline int rows_per_cluster(int B, int C, int num_sms) {
   int R = 1;
-  if ((long)2 * B * C > ner_num_sms()) R = 2;
-  if ((long)2 * ((B + 1) / 2) * C > 2 * ner_num_sms()) R = 4;
+  if ((long)2 * B * C > num_sms) R = 2;
+  if ((long)2 * ((B + 1) / 2) * C > 2 * (long)num_sms) R = 4;
   return R;
+}
+
+// Smallest power-of-two cluster of the BiLSTM recurrence (bilstm.cu) whose W_h slice (H * 4H/C floats) fits ~190 KB
+// and divides H; 0 if none.
+static inline int lstm_pick_cluster(int H) {
+  for (int C = 1; C <= 8; C *= 2) {
+    if (H % C != 0) continue;
+    const size_t bytes = (size_t)H * 4 * (H / C) * 4;
+    if (bytes <= 190 * 1024 && 4 * (H / C) <= 512) return C;
+  }
+  return 0;
+}
+
+// The same for its back-propagation through time (bilstm_bwd.cu): a [4H][H/C + 1] transposed slice within 180 KB.
+static inline int lstm_pick_cluster_bwd(int H) {
+  for (int C = 1; C <= 8; C *= 2) {
+    if (H % C != 0) continue;
+    const size_t bytes = (size_t)4 * H * (H / C + 1) * 4;
+    if (bytes <= 180 * 1024) return C;
+  }
+  return 0;
 }
 
 // The GRU recurrence (bigru.cu) and its back-propagation through time (bigru_bwd.cu) keep the same recurrent weights
@@ -207,5 +228,9 @@ static inline int gru_pick_cluster(int H) {
   }
   return 0;
 }
+
+// Rows per cluster and cluster size of the Lattice LSTM kernels (lattice.cu, where their shared-memory layout lives):
+// NER_OK, or the status ner_lattice_recurrence returns for the shape.
+int lattice_config(int B, int H, int Kw, int num_sms, int* R, int* C);
 
 }  // namespace rnn

@@ -537,6 +537,25 @@ int ner_bigru_recurrence_bwd(const float* d_out, const float* gates, const float
                              const float* wh_bw, const int32_t* seq_len, float* d_xproj, int B, int L, int H,
                              int activation, float keep_prob, uint64_t seed, ner_stream_t stream);
 
+/* Which instantiation a recurrence call runs (csrc/rnn_plan.cu holds the rules).  The launchers of the six kernels
+ * below (ner_bilstm_recurrence, _bwd, ner_bigru_recurrence, _bwd, ner_lattice_recurrence, _bwd) call it with the
+ * device's SM count and launch what it returns, so the answer for a shape is the launch.  Out: *rows = batch rows per
+ * cluster (the kernel's template R), *cluster = CTAs per cluster, *resident = 1 when the recurrent matrix is held in
+ * registers (LSTM at H = 128) and 0 otherwise; each may be NULL.  Kw (words per lattice position) is read only for
+ * the lattice kernels.  Returns NER_OK, or the status the launcher returns for that shape before any CUDA call
+ * (NER_ERR_INVALID_ARG for B < 0, H < 1, num_sms < 1, Kw < 1 (lattice) or an unknown kernel; NER_ERR_UNSUPPORTED
+ * for an H no cluster holds, H % 4 != 0 (LSTM forward, GRU) or Kw > 8), with the outputs set to 0.  A pure host
+ * function: no CUDA call and no environment variable enters it. */
+enum {
+  NER_RNN_LSTM_FWD = 0,
+  NER_RNN_LSTM_BWD = 1,
+  NER_RNN_GRU_FWD = 2,
+  NER_RNN_GRU_BWD = 3,
+  NER_RNN_LATTICE_FWD = 4,
+  NER_RNN_LATTICE_BWD = 5
+};
+int ner_rnn_plan(int kernel, int B, int H, int Kw, int num_sms, int* rows, int* cluster, int* resident);
+
 /* ------------------------------------------------------------------------ *
  * SoftLexicon gather-and-pool — model/bilstm_crf_softlexicon.py:37-44
  * ------------------------------------------------------------------------ */

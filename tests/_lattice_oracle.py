@@ -34,9 +34,11 @@ def words_of(lens_row, n, Kw):
     return out
 
 
-def lattice_lstm(x, xw, lens, seq_len, w, H):
+def lattice_lstm(x, xw, lens, seq_len, w, H, alpha_shift=None):
     """x [B, L, Ec], xw [B, L, Kw, Ew] (slot embeddings), lens [B, L * Kw] int, seq_len [B], w: name -> tensor.
-    -> out [B, L, 2H] in the dtype of x (use float64 tensors, with requires_grad where gradients are wanted)."""
+    -> out [B, L, 2H] in the dtype of x (use float64 tensors, with requires_grad where gradients are wanted).
+    alpha_shift: optional [B, L, Kw, 2H] added to the alpha pre-activation of the word in slot (b, start, k), direction
+    d at [..., d*H:(d+1)*H]; a zero leaf there collects each word's alpha gradient."""
     B, L, Ec = x.shape
     Kw, Ew = xw.shape[2], xw.shape[3]
     nm = names()
@@ -65,7 +67,10 @@ def lattice_lstm(x, xw, lens, seq_len, w, H):
                     num, den = ei * g, ei
                     for wd in merged:
                         cw = pending.pop(wd)
-                        a = torch.sigmoid(x[b, pos] @ Wa[:Ec] + cw @ Wa[Ec:] + ba)
+                        za = x[b, pos] @ Wa[:Ec] + cw @ Wa[Ec:] + ba
+                        if alpha_shift is not None:
+                            za = za + alpha_shift[b, wd[0], wd[2], di * H:(di + 1) * H]
+                        a = torch.sigmoid(za)
                         ea = torch.exp(a)
                         num, den = num + ea * cw, den + ea
                     c = num / den

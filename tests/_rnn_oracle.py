@@ -22,9 +22,12 @@ def gru_direction(x, kernel, bias, seq_len, activation="tanh", reverse=False, em
 
 
 def rnn_direction(x, kernel, bias, seq_len, cell="lstm", activation="tanh", forget_bias=1.0, reverse=False,
-                  emulate_bf16=False, out_mask=None, state_mask=None):
+                  emulate_bf16=False, out_mask=None, state_mask=None, saved=False):
     """One direction of dynamic_rnn(DropoutWrapper(cell)), cell 'lstm' (kernel [D+H, 4H], gates i, j, f, o; as
-    lstm_direction) or 'gru' (see gru_direction).  For t >= seq_len the output is 0 and the state is carried."""
+    lstm_direction) or 'gru' (see gru_direction).  For t >= seq_len the output is 0 and the state is carried.
+    saved=True: -> (out, per-step values [B, L, .] in original positions, 0 past seq_len): 'gates' (LSTM: sigmoid(i),
+    act(j), sigmoid(f + forget_bias), sigmoid(o); GRU: r, u, act(c)), 'h' (the carried, state-dropped h) and, LSTM,
+    'c' (the cell state) or, GRU, 'rh' (r * h_prev) -- what the recurrence kernels save for back-propagation."""
     B, L, D = x.shape
     H = kernel.shape[1] // (4 if cell == "lstm" else 3)
     act = torch.relu if activation == "relu" else torch.tanh
@@ -35,6 +38,8 @@ def rnn_direction(x, kernel, bias, seq_len, cell="lstm", activation="tanh", forg
     out = x.new_zeros(B, L, H)
     lens = seq_len.long()
     ar = torch.arange(B)
+    per_step = {k: x.new_zeros(B, L, n * H) for k, n in
+                (("gates", 4 if cell == "lstm" else 3), ("h", 1), ("c" if cell == "lstm" else "rh", 1))}
     for s in range(L):
         active = s < lens
         if not bool(active.any()):
@@ -43,19 +48,25 @@ def rnn_direction(x, kernel, bias, seq_len, cell="lstm", activation="tanh", forg
         xp = xproj[ar, pos]
         if cell == "lstm":
             i, j, f, o = (xp + h @ wh).split(H, dim=1)
-            c_new = torch.sigmoid(f + forget_bias) * c + torch.sigmoid(i) * act(j)
-            h_new = torch.sigmoid(o) * act(c_new)
+            gates = (torch.sigmoid(i), act(j), torch.sigmoid(f + forget_bias), torch.sigmoid(o))
+            c_new = gates[2] * c + gates[0] * gates[1]
+            h_new = gates[3] * act(c_new)
             c = torch.where(active[:, None], c_new, c)
+            extra = c_new
         else:
             r, u = torch.sigmoid(xp[:, :2 * H] + h @ wh[:, :2 * H]).split(H, dim=1)
             cand = act(xp[:, 2 * H:] + (r * h) @ wh[:, 2 * H:])
             h_new = u * h + (1 - u) * cand
+            gates, extra = (r, u, cand), r * h
         h_state = h_new if state_mask is None else h_new * state_mask[ar, pos]
         h_out = h_new if out_mask is None else h_new * out_mask[ar, pos]
         h = torch.where(active[:, None], h_state, h)
         idx = ar[active]
         out[idx, pos[active]] = h_out[active]
-    return out
+        if saved:
+            for k, v in (("gates", torch.cat(gates, 1)), ("h", h_state), ("c" if cell == "lstm" else "rh", extra)):
+                per_step[k][idx, pos[active]] = v[active].detach()
+    return (out, per_step) if saved else out
 
 
 def rnn_cell_weights(w, prefix, d, i, cell, dtype=torch.float64):
