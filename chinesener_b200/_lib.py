@@ -31,6 +31,11 @@ SIGNATURES = {
                                  _i, _i, _vp]),
     "ner_crf_viterbi_nbest_workspace_bytes": (_c.c_size_t, [_i, _i, _i, _i]),
     "ner_crf_viterbi_nbest": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _c.c_size_t, _i, _i, _i, _vp]),
+    "ner_crf_wide_viterbi_workspace_bytes": (_c.c_size_t, [_i, _i, _i]),
+    "ner_crf_wide_viterbi": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _c.c_size_t, _i, _i, _i, _vp]),
+    "ner_crf_wide_loglik_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "ner_crf_wide_loglik_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _c.c_float, _vp, _vp, _i, _i, _i, _vp]),
+    "ner_crf_wide_plan": (_i, [_i, _i, _i, _i]),
     "ner_gemm_bf16": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "ner_pack_weight_bf16": (_i, [_vp, _vp, _i, _i, _vp]),
     "ner_cast_bf16": (_i, [_vp, _vp, _c.c_size_t, _vp]),
@@ -182,6 +187,7 @@ class WgradProblem(_c.Structure):
 SIGNATURES["ner_wgrad_group_bf16"] = (_i, [_c.POINTER(WgradProblem), _i, _i, _vp])
 SIGNATURES["ner_bert_train_bwd_set_layer_events"] = (_i, [_vp, _i])
 SIGNATURES["ner_extract_spans"] = (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp])
+SIGNATURES["ner_extract_spans_wide"] = (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp])
 SIGNATURES["ner_lexicon_create"] = (_vp, [_vp, _vp, _vp, _i])
 SIGNATURES["ner_lexicon_destroy"] = (None, [_vp])
 SIGNATURES["ner_lexicon_num_nodes"] = (_c.c_int64, [_vp])

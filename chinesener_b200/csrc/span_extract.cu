@@ -21,10 +21,12 @@
 namespace {
 constexpr int kWarpsPerCta = 4;
 
-// tag_class byte: bits 0-1 kind (0 other, 1 B, 2 I), bit 2 = "first character is B or I" (what the reference tests on the
-// previous tag), bits 3-7 entity type id.
+// tag class: bits 0-1 kind (0 other, 1 B, 2 I), bit 2 = "first character is B or I" (what the reference tests on the
+// previous tag), bits 3.. entity type id: 5 bits in the byte-wide table (ner_extract_spans), 7 in the 16-bit one
+// (ner_extract_spans_wide).
+template <typename Cls>
 __global__ void __launch_bounds__(kWarpsPerCta * 32) span_extract_kernel(const int32_t* __restrict__ pred_ids,
-                                                                        const uint8_t* __restrict__ tag_class,
+                                                                        const Cls* __restrict__ tag_class,
                                                                         int32_t* __restrict__ spans,
                                                                         int32_t* __restrict__ counts, int B, int L, int K,
                                                                         int cap) {
@@ -32,11 +34,11 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) span_extract_kernel(const i
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int b = blockIdx.x * kWarpsPerCta + warp;
   if (b >= B) return;
-  uint8_t* cls = smem + (size_t)warp * L;
+  Cls* cls = reinterpret_cast<Cls*>(smem) + (size_t)warp * L;
   const int32_t* row = pred_ids + (size_t)b * L;
   for (int p = lane; p < L; p += 32) {
     const int id = row[p];
-    cls[p] = (id >= 0 && id < K) ? tag_class[id] : (uint8_t)0;
+    cls[p] = (id >= 0 && id < K) ? tag_class[id] : (Cls)0;
   }
   __syncwarp();
   int n_emitted = 0;
@@ -67,17 +69,28 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) span_extract_kernel(const i
   }
   if (lane == 0) counts[b] = n_emitted;
 }
+
+template <typename Cls>
+int extract_spans(const int32_t* pred_ids, const Cls* tag_class, int32_t* spans, int32_t* counts, int B, int L, int K,
+                  int cap, ner_stream_t stream) {
+  if (B < 0 || L < 1 || K < 1 || cap < 1) return NER_ERR_INVALID_ARG;
+  if (B == 0) return NER_OK;
+  if (!pred_ids || !tag_class || !spans || !counts) return NER_ERR_INVALID_ARG;
+  if (L > 4095 || K > 256) return NER_ERR_UNSUPPORTED;      // span word: start 12 bits | end 12 bits | type
+  const size_t smem = (size_t)kWarpsPerCta * L * sizeof(Cls);
+  const int grid = (B + kWarpsPerCta - 1) / kWarpsPerCta;
+  span_extract_kernel<Cls><<<grid, kWarpsPerCta * 32, smem, static_cast<cudaStream_t>(stream)>>>(pred_ids, tag_class, spans,
+                                                                                               counts, B, L, K, cap);
+  return ner_launch_status();
+}
 }  // namespace
 
 extern "C" int ner_extract_spans(const int32_t* pred_ids, const uint8_t* tag_class, int32_t* spans, int32_t* counts, int B,
                                  int L, int K, int cap, ner_stream_t stream) {
-  if (B < 0 || L < 1 || K < 1 || cap < 1) return NER_ERR_INVALID_ARG;
-  if (B == 0) return NER_OK;
-  if (!pred_ids || !tag_class || !spans || !counts) return NER_ERR_INVALID_ARG;
-  if (L > 4095 || K > 256) return NER_ERR_UNSUPPORTED;      // span word: start 12 bits | end 12 bits | type 5 bits
-  const size_t smem = (size_t)kWarpsPerCta * L;
-  const int grid = (B + kWarpsPerCta - 1) / kWarpsPerCta;
-  span_extract_kernel<<<grid, kWarpsPerCta * 32, smem, static_cast<cudaStream_t>(stream)>>>(pred_ids, tag_class, spans, counts,
-                                                                                          B, L, K, cap);
-  return ner_launch_status();
+  return extract_spans(pred_ids, tag_class, spans, counts, B, L, K, cap, stream);
+}
+
+extern "C" int ner_extract_spans_wide(const int32_t* pred_ids, const uint16_t* tag_class, int32_t* spans, int32_t* counts,
+                                      int B, int L, int K, int cap, ner_stream_t stream) {
+  return extract_spans(pred_ids, tag_class, spans, counts, B, L, K, cap, stream);
 }

@@ -11,6 +11,11 @@ TFRecords.
         --tokenizer giga --giga_vec <gigaword .vec>  [--bert_vocab <vocab.txt>]
         [--word_enhance bichar --bichar_vec <bigram .vec> | --word_enhance ex_softword --word_vec <word .vec>
          | --word_enhance lattice --word_vec <word .vec> | --word_enhance softword]  [--partial_labels]
+        [--tag_set msra|data]  [--tag_scheme bio|bioes]
+
+--tag_set data takes the tag set from the train split's tags.txt instead of MSRA's (data_tag2idx); --tag_scheme bioes
+rewrites B/I/E/S/M-T tags to BIO as they are read (bioes_to_bio), so evaluation and entity extraction, which follow
+BIO, see the same entities.
 """
 import argparse
 import os
@@ -30,6 +35,54 @@ MAPPING = {'train': 'train', 'val': 'valid', 'test': 'predict'}
 # data/msr/preprocess.py:7-22 (Chinese word segmentation as a tagging task: the auxiliary task of the multi-task plugins)
 MSR_TAG2IDX = {'[PAD]': 0, 'B': 1, 'I': 2, 'E': 3, 'S': 4, '[CLS]': 5, '[SEP]': 6}
 MSR_MAPPING = {'training': 'train', 'test_gold': 'valid', 'test': 'predict'}
+
+MAX_TAGS = 128          # the wide CRF kernels' limit (NER_MAX_TAGS_WIDE)
+MAX_PARTIAL_TAGS = 32   # a partial label is a 32-bit mask of allowed tags
+_BIOES_TO_BIO = {'B': 'B', 'I': 'I', 'E': 'I', 'M': 'I', 'S': 'B'}
+
+
+def bioes_to_bio(tag_line):
+    """One tags.txt line from BIOES (with M as a synonym of I) to BIO: E-T, M-T -> I-T and S-T -> B-T.  Partial labels
+    ('?' and 'T1|T2' alternatives) are rewritten alternative by alternative."""
+    def one(tag):
+        if tag == '?':
+            return tag
+        if '|' in tag:
+            return '|'.join(one(t) for t in tag.split('|'))
+        prefix, sep, typ = tag.partition('-')
+        if sep and prefix in _BIOES_TO_BIO:
+            return _BIOES_TO_BIO[prefix] + '-' + typ
+        return tag
+    return ' '.join(one(t) for t in tag_line.split(' '))
+
+
+def data_tag2idx(tag_lines):
+    """The tag set of a corpus in the MSRA layout: [PAD] = 0, O = 1, then B-T, I-T for each entity type T in sorted
+    order, then [CLS], [SEP].  tag_lines are BIO lines (partial-label alternatives count; '?' adds nothing)."""
+    types = set()
+    for line in tag_lines:
+        for tag in line.split(' '):
+            for t in tag.split('|'):
+                prefix, sep, typ = t.partition('-')
+                if sep and prefix in ('B', 'I') and typ:
+                    types.add(typ)
+    tags = ['[PAD]', 'O'] + [p + '-' + t for t in sorted(types) for p in ('B', 'I')] + ['[CLS]', '[SEP]']
+    if len(tags) > MAX_TAGS:
+        raise ValueError('the train split has {} entity types, {} tags; the CRF kernels take at most {} tags'.format(
+            len(types), len(tags), MAX_TAGS))
+    return {t: i for i, t in enumerate(tags)}
+
+
+def scheme_loader(tag_scheme, load=None):
+    """load_data for a tag scheme: BIO files as they are, BIOES files rewritten to BIO line by line."""
+    load = load or load_data
+    if tag_scheme == 'bio':
+        return load
+
+    def load_bioes(data_dir, file_name):
+        sentences, tags = load(data_dir, file_name)
+        return sentences, [bioes_to_bio(t) for t in tags]
+    return load_bioes
 
 
 def msr_gen_tag(length):
@@ -115,16 +168,31 @@ def main(argv=None):
     ap.add_argument('--word_vec', default='./pretrain_model/ctb50/ctb.50d.vec',
                     help='word vectors (giga .vec format) whose vocabulary is the lexicon of --word_enhance ex_softword / '
                          'lattice (lattice also keeps the vectors as the word table)')
+    ap.add_argument('--tag_set', default='msra', choices=['msra', 'data'],
+                    help="'msra': MSRA's ten tags; 'data': [PAD], O, B-/I- of every entity type in the train split's "
+                         "tags.txt (sorted), [CLS], [SEP]; at most 128 tags")
+    ap.add_argument('--tag_scheme', default='bio', choices=['bio', 'bioes'],
+                    help="'bioes': tags.txt uses B/I/E/S(/M)-T; they are rewritten to BIO before indexing")
     ap.add_argument('--partial_labels', action='store_true',
                     help="tags.txt may leave a token's tag open: '?' (any tag) or a set 'T1|T2|...'; such splits get a "
                          "label_mask column and label_id -1 at the open positions, for the CRF plugins")
     args = ap.parse_args(argv)
+    msr = args.format == 'msr'
+    if msr and (args.tag_set != 'msra' or args.tag_scheme != 'bio'):
+        ap.error("--format msr has its own tag set: --tag_set and --tag_scheme apply to --format ner")
+    load = scheme_loader(args.tag_scheme)
+    tag2idx = MSR_TAG2IDX if msr else MSRA_TAG2IDX
+    if args.tag_set == 'data':
+        tag2idx = data_tag2idx(load(args.src, 'train')[1])
+        print('tag set from the train split: {} tags'.format(len(tag2idx)))
+    if args.partial_labels and len(tag2idx) > MAX_PARTIAL_TAGS:
+        ap.error('--partial_labels takes at most {} tags (a 32-bit mask of allowed tags); this tag set has {}'.format(
+            MAX_PARTIAL_TAGS, len(tag2idx)))
     if args.tokenizer == TokenizerGiga:
         tok = get_giga_tokenizer(args.giga_vec)
         emb = tok.embedding(args.seed)
     else:
         tok, emb = get_bert_tokenizer(args.bert_dir), None
-    msr = args.format == 'msr'
     kwargs, bichar_emb = {}, None
     if args.word_enhance == BiChar:
         kwargs['bichar_tokenizer'] = get_giga_tokenizer(args.bichar_vec)
@@ -136,13 +204,13 @@ def main(argv=None):
         vec = TextVectors(args.word_vec)
         kwargs['vocab'] = WordVocab(vec.index2word, dict.fromkeys(vec.index2word, 1))
         kwargs['word_embedding'] = lattice_word_embedding(vec, args.seed)
-    proc = get_instance(args.tokenizer, args.max_seq_len, MSR_TAG2IDX if msr else MSRA_TAG2IDX, tok,
+    proc = get_instance(args.tokenizer, args.max_seq_len, tag2idx, tok,
                         word_enhance=args.word_enhance, **kwargs)
     proc.partial_labels = args.partial_labels
     for file in (MSR_MAPPING if msr else MAPPING):
         print('Dumping records for {} tokenizer = {}'.format(file, args.tokenizer))
         dump_records(proc, args.src, args.out, file, mapping=MSR_MAPPING if msr else MAPPING, embedding=emb,
-                     load_data=load_msr_data if msr else None, word_enhance=args.word_enhance, bichar_embedding=bichar_emb)
+                     load_data=load_msr_data if msr else load, word_enhance=args.word_enhance, bichar_embedding=bichar_emb)
         if args.word_enhance == Lattice:
             print('lattice words dropped by the max_lattice_words cap so far: {}'.format(proc.dropped))
 

@@ -29,6 +29,13 @@ NBEST_REFUSED = {
     'bert_bilstm_crf_adv': "its pred_ids are a per-task selection of several CRF decodes",
 }
 NBEST_MAX = 16
+# The CRF kernels take up to 128 tags (ner_crf_wide_*), but N-best decoding, the partial-label loss (a 32-bit mask of
+# allowed tags), distillation and the token heads of these plugins stop at 32: past that, Estimator refuses them.
+NARROW_TAGS = 32
+WIDE_TAGS_REFUSED = {
+    'bert_ce': "its fused cross-entropy kernel takes at most 32 tags",
+    'bert_dice': "its fused Dice-loss kernel takes at most 32 tags",
+}
 
 
 def load_plugin(model_name):
@@ -46,6 +53,7 @@ class Estimator:
         self.params.update(params)
         self.device = torch.device(device)
         self.teacher = teacher
+        self.tag_set_limits()
         if teacher is not None:
             self.distill_settings()
         self.store = store or variables.VariableStore(self.device)
@@ -96,6 +104,23 @@ class Estimator:
         max_pos = bert.load_bert_config(self.params.get('pretrain_dir', ''))["max_position_embeddings"]
         return windows.settings(self.params.get('bert_window'), self.params.get('bert_window_stride'), max_pos)
 
+    def label_size(self):
+        K = self.params.get('label_size')
+        return int(K) if isinstance(K, (int, np.integer)) and not isinstance(K, bool) else 0
+
+    def tag_set_limits(self, features=None):
+        """ValueError, before anything is launched, for what does not run past 32 tags: the plugins in
+        WIDE_TAGS_REFUSED, and a batch with a `label_mask` (partial labels).  N-best decoding and distillation are
+        refused by crf_nbest and distill_settings."""
+        K = self.label_size()
+        if K <= NARROW_TAGS:
+            return
+        if self.model_name in WIDE_TAGS_REFUSED:
+            raise ValueError(f"{self.model_name} cannot run label_size = {K} tags: {WIDE_TAGS_REFUSED[self.model_name]}")
+        if features is not None and features.get('label_mask') is not None:
+            raise ValueError(f"partial labels (label_mask) take at most {NARROW_TAGS} tags, a 32-bit mask of allowed "
+                             f"tags; this tag set has label_size = {K}")
+
     def crf_nbest(self):
         """params['crf_nbest'] (default 1): how many best CRF paths PREDICT / EVAL decode.  ValueError outside
         1..NBEST_MAX, or above 1 for a plugin in NBEST_REFUSED."""
@@ -104,6 +129,9 @@ class Estimator:
             raise ValueError(f"crf_nbest must be an integer in 1..{NBEST_MAX} (got {n!r})")
         if n > 1 and self.model_name in NBEST_REFUSED:
             raise ValueError(f"{self.model_name} cannot decode crf_nbest = {n} paths: {NBEST_REFUSED[self.model_name]}")
+        if n > 1 and self.label_size() > NARROW_TAGS:
+            raise ValueError(f"crf_nbest = {n} takes at most {NARROW_TAGS} tags; this tag set has label_size = "
+                             f"{self.label_size()}")
         return int(n)
 
     def distill_settings(self):
@@ -113,6 +141,9 @@ class Estimator:
         other than none or the teacher's own: the two CRFs must score the same tags at the same positions."""
         from .data.base_preprocess import extract_prefix_surfix
         t = self.teacher
+        if self.label_size() > NARROW_TAGS:
+            raise ValueError(f"distillation takes at most {NARROW_TAGS} tags; this tag set has label_size = "
+                             f"{self.label_size()}")
         for who, name in (("teacher", t.model_name), ("student", self.model_name)):
             if name in NBEST_REFUSED:
                 raise ValueError(f"cannot distill with {who} {name}: {NBEST_REFUSED[name]}")
@@ -156,6 +187,7 @@ class Estimator:
         from . import windows
         from .tools import layer
         nbest = self.crf_nbest()
+        self.tag_set_limits(dev_features)
         ws = self.document_window()
         if ws is not None and torch.is_tensor(dev_features.get('token_ids')):
             windows.check_batch(self.model_name, dev_features['token_ids'].shape[1], ws[0])
@@ -325,6 +357,7 @@ class Estimator:
         """TRAIN mode of model_fn (reference tools/train_utils.py:151-168): forward with the tape,
         backward, then the train op the reference picks by model name (:156-164).  -> loss (float)."""
         from .tools import train_utils
+        self.tag_set_limits(features)
         dev = features if all(not torch.is_tensor(v) or v.is_cuda for v in features.values()) else self.to_device(features)
         teacher = None
         if self.teacher is not None:

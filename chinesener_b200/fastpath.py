@@ -37,6 +37,8 @@ def bert_bilstm_crf_predict(est, dev):
         return None                                    # N-best decoding: build_graph's crf_decode attaches the paths
     if dev['token_ids'].shape[1] > est.document_window()[0]:
         return None                                    # document mode: build_graph stitches the windows
+    if params['label_size'] > 32:
+        return None                                    # the fused executor's CRF takes 32 tags: build_graph's takes 128
     Hl, K = params['hidden_units_list'][0], params['label_size']
     v = store.vars
     lscope = "bilstm_layer/bidirectional_rnn"

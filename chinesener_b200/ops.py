@@ -23,16 +23,34 @@ def _i32(t):
 
 
 # --------------------------------------------------------------------------- CRF
-def crf_viterbi(logits, seq_len, trans, return_score=False):
-    """tf.contrib.crf.crf_decode (reference tools/layer.py:140).  -> tags [B,L] int32 (+ best_score [B])."""
+MAX_TAGS = 32        # K of the K-specialised CRF kernels (NER_MAX_TAGS); ops.crf_* send larger K to the wide ones
+MAX_TAGS_WIDE = 128  # NER_MAX_TAGS_WIDE
+
+
+def _wide(K, wide):
+    """Whether a CRF call runs the wide-tag-set kernels (ner_crf_wide_*): always past MAX_TAGS; wide=True forces them
+    for any K (the tests pin them to the K-specialised kernels, the bench compares the two)."""
+    return K > MAX_TAGS or bool(wide)
+
+
+def crf_viterbi(logits, seq_len, trans, return_score=False, wide=None):
+    """tf.contrib.crf.crf_decode (reference tools/layer.py:140).  -> tags [B,L] int32 (+ best_score [B]).
+    K <= 32: ner_crf_viterbi; K <= 128 (or wide=True): ner_crf_wide_viterbi with its backpointer workspace."""
     require_cuda(logits, seq_len, trans)
     assert logits.dtype == torch.float32 and trans.dtype == torch.float32
     B, L, K = logits.shape
     assert trans.shape == (K, K)
     seq_len = _i32(seq_len)
-    tags = torch.empty((B, L), dtype=torch.int32, device=logits.device)
-    score = torch.empty((B,), dtype=torch.float32, device=logits.device) if return_score else None
-    check(lib().ner_crf_viterbi(ptr(logits), ptr(seq_len), ptr(trans), ptr(tags), ptr(score), B, L, K, stream()))
+    dev = logits.device
+    tags = torch.empty((B, L), dtype=torch.int32, device=dev)
+    score = torch.empty((B,), dtype=torch.float32, device=dev) if return_score else None
+    if _wide(K, wide):
+        nbytes = int(lib().ner_crf_wide_viterbi_workspace_bytes(B, L, K))
+        ws = torch.empty((max(nbytes, 16),), dtype=torch.uint8, device=dev)
+        check(lib().ner_crf_wide_viterbi(ptr(logits), ptr(seq_len), ptr(trans), ptr(tags), ptr(score), ptr(ws), nbytes,
+                                         B, L, K, stream()))
+    else:
+        check(lib().ner_crf_viterbi(ptr(logits), ptr(seq_len), ptr(trans), ptr(tags), ptr(score), B, L, K, stream()))
     return (tags, score) if return_score else tags
 
 
@@ -59,8 +77,9 @@ def crf_viterbi_nbest(logits, seq_len, trans, n):
     return tags, scores, counts
 
 
-def crf_loglik_fwd(logits, tags, seq_len, trans, want_alpha=False, exact=False):
-    """tf.contrib.crf.crf_log_likelihood forward (reference tools/layer.py:122). -> ll [B], logz [B], alpha|None."""
+def crf_loglik_fwd(logits, tags, seq_len, trans, want_alpha=False, exact=False, wide=None):
+    """tf.contrib.crf.crf_log_likelihood forward (reference tools/layer.py:122). -> ll [B], logz [B], alpha|None.
+    K <= 32: ner_crf_loglik_fwd; K <= 128 (or wide=True): ner_crf_wide_loglik_fwd."""
     require_cuda(logits, tags, seq_len, trans)
     assert logits.dtype == torch.float32 and trans.dtype == torch.float32
     B, L, K = logits.shape
@@ -68,8 +87,9 @@ def crf_loglik_fwd(logits, tags, seq_len, trans, want_alpha=False, exact=False):
     ll = torch.empty((B,), dtype=torch.float32, device=logits.device)
     logz = torch.empty((B,), dtype=torch.float32, device=logits.device)
     alpha = torch.empty((B, L, K), dtype=torch.float32, device=logits.device) if want_alpha else None
-    check(lib().ner_crf_loglik_fwd(ptr(logits), ptr(tags), ptr(seq_len), ptr(trans), ptr(ll), ptr(logz), ptr(alpha),
-                                   B, L, K, 1 if exact else 0, stream()))
+    fn = lib().ner_crf_wide_loglik_fwd if _wide(K, wide) else lib().ner_crf_loglik_fwd
+    check(fn(ptr(logits), ptr(tags), ptr(seq_len), ptr(trans), ptr(ll), ptr(logz), ptr(alpha), B, L, K,
+             1 if exact else 0, stream()))
     return ll, logz, alpha
 
 
@@ -465,8 +485,9 @@ def small_table_grad(d_table, d_out, ids=None, weights=None, col_offset=0):
     return d_table
 
 
-def crf_loglik_bwd(logits, tags, seq_len, trans, alpha, logz, d_ll=None, scale=1.0):
-    """-> d_logits [B,L,K], d_trans [K,K] for g_b = (d_ll|1) * scale."""
+def crf_loglik_bwd(logits, tags, seq_len, trans, alpha, logz, d_ll=None, scale=1.0, wide=None):
+    """-> d_logits [B,L,K], d_trans [K,K] for g_b = (d_ll|1) * scale.  K <= 32: ner_crf_loglik_bwd; K <= 128 (or
+    wide=True): ner_crf_wide_loglik_bwd."""
     require_cuda(logits, tags, seq_len, trans, alpha, logz, d_ll)
     B, L, K = logits.shape
     assert all(t.dtype == torch.float32 for t in (logits, trans, alpha, logz) + ((d_ll,) if d_ll is not None else ()))
@@ -474,8 +495,9 @@ def crf_loglik_bwd(logits, tags, seq_len, trans, alpha, logz, d_ll=None, scale=1
     assert d_ll is None or d_ll.shape == (B,)
     d_logits = torch.empty_like(logits)
     d_trans = torch.zeros_like(trans)
-    check(lib().ner_crf_loglik_bwd(ptr(logits), ptr(_i32(tags)), ptr(_i32(seq_len)), ptr(trans), ptr(alpha), ptr(logz),
-                                   ptr(d_ll), scale, ptr(d_logits), ptr(d_trans), B, L, K, stream()))
+    fn = lib().ner_crf_wide_loglik_bwd if _wide(K, wide) else lib().ner_crf_loglik_bwd
+    check(fn(ptr(logits), ptr(_i32(tags)), ptr(_i32(seq_len)), ptr(trans), ptr(alpha), ptr(logz), ptr(d_ll), scale,
+             ptr(d_logits), ptr(d_trans), B, L, K, stream()))
     return d_logits, d_trans
 
 
@@ -1213,7 +1235,8 @@ def bert_attention_bwd(qkv, mask, ctx, dctx, B, L, num_heads, head_dim=64, scale
 
 # --------------------------------------------------------------------------- entity spans (serving tail)
 def tag_classes(idx2tag):
-    """idx2tag -> (uint8 class table [K] for ner_extract_spans, list of entity types)."""
+    """idx2tag -> (class table [K] for ner_extract_spans, list of entity types).  The table is uint8 (5 type bits) up to
+    32 entity types, and int16 for ner_extract_spans_wide (7 type bits) up to 128."""
     K = max(idx2tag) + 1
     types, table = [], [0] * K
     for i, tag in idx2tag.items():
@@ -1226,8 +1249,8 @@ def tag_classes(idx2tag):
                 types.append(name)
             t = types.index(name)
         table[i] = kind | (4 if tag[:1] in ('B', 'I') else 0) | (t << 3)
-    assert len(types) <= 32
-    return torch.tensor(table, dtype=torch.uint8), types
+    assert len(types) <= 128
+    return torch.tensor(table, dtype=torch.uint8 if len(types) <= 32 else torch.int16), types
 
 
 def extract_spans(pred_ids, tag_class, cap=None):
@@ -1237,7 +1260,9 @@ def extract_spans(pred_ids, tag_class, cap=None):
     cap = cap or L            # 'B B B ...': every position can be a span of its own
     spans = torch.empty((B, cap), dtype=torch.int32, device=pred_ids.device)
     counts = torch.empty((B,), dtype=torch.int32, device=pred_ids.device)
-    check(lib().ner_extract_spans(ptr(_i32(pred_ids)), ptr(tag_class), ptr(spans), ptr(counts), B, L, tag_class.numel(), cap, stream()))
+    fn = lib().ner_extract_spans if tag_class.dtype == torch.uint8 else lib().ner_extract_spans_wide
+    assert tag_class.dtype in (torch.uint8, torch.int16)
+    check(fn(ptr(_i32(pred_ids)), ptr(tag_class), ptr(spans), ptr(counts), B, L, tag_class.numel(), cap, stream()))
     return spans, counts
 
 

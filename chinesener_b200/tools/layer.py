@@ -555,13 +555,70 @@ def cnn_layer(embedding, filter_list, kernel_size_list, activation, drop_out, is
     return output
 
 
+def _dense_wide_pack(store, name, F, N, for_dx=False):
+    """Split-bf16 (hi, lo) weight operands of ner_gemm_bf16 from `name/kernel` [F, N], zero-padded; rebuilt when the
+    store's variables change.  Forward: packs of W, [Np, Fp] (N padded to the GEMM's 32-column granule, F to 8).
+    for_dx: packs of W^T, [Fo, Np] (F padded to 32), the operand of dx = dy·W^T."""
+    Fp, Fo, Np = (F + 7) // 8 * 8, (F + 31) // 32 * 32, (N + 31) // 32 * 32
+
+    def build():
+        w = variables.default_store().vars[f"{name}/kernel"]
+        w = (torch.nn.functional.pad(w, (0, Np - N, 0, Fo - F)).t() if for_dx
+             else torch.nn.functional.pad(w, (0, Np - N, 0, Fp - F))).contiguous()
+        hi = ops.pack_weight_bf16(w)
+        lo = ops.pack_weight_bf16((w - hi.float().t()).contiguous())
+        return hi, lo
+    return store.cached(("dense_wide_pack", name, F, N, for_dx), build)
+
+
+def _dense_wide(inputs, units, name, b, is_training):
+    """dense() for units > 32: the fp32-accurate split-bf16 wgmma GEMM of the transformer plugins (A_hi·W_hi + A_hi·W_lo +
+    A_lo·W_hi), on N padded to 32 columns and sliced.  TRAIN records db = colsum(dy) in fp32, dW = x^T·dy on bf16
+    operands (fp32 accumulation) as tools/transformer/modules.py's dense_train does, and dx = dy·W^T on the same split
+    GEMM as the forward, so the gradient that reaches the encoder keeps fp32 accuracy."""
+    F = inputs.shape[-1]
+    lead = inputs.shape[:-1]
+    store = variables.default_store()
+    x2d = inputs.reshape(-1, F).contiguous()
+    w_hi, w_lo = _dense_wide_pack(store, name, F, units)
+    a_hi, a_lo = ops.split_bf16(x2d, w_hi.shape[1])
+    Np = w_hi.shape[0]
+    bias = torch.nn.functional.pad(b, (0, Np - units)) if Np != units else b
+    y = ops.gemm_split_f32(a_hi, a_lo, w_hi, w_lo, bias)[:, :units]
+    pack = getattr(inputs, "pack", None)
+    if pack is not None:                  # packed rows -> padded [B, L, units]; padded positions stay 0
+        out = ops.scatter_rows(y.contiguous(), pack.tok_src[:x2d.shape[0]], pack.B * pack.L)
+        return out.view(pack.B, pack.L, units)
+    out = y.contiguous().view(*lead, units)
+    tape = autodiff.current()
+    if is_training and tape is not None:
+        need_dx = tape.needs_grad(inputs)
+
+        def bwd(g):
+            if g is None:
+                return
+            g2d = g.reshape(-1, units).contiguous()
+            ops.colsum_add(g2d, store.grad(f"{name}/bias"))
+            ops.wgrad_gemm(x2d, g2d, out=store.grad(f"{name}/kernel"))
+            if need_dx:
+                wt_hi, wt_lo = _dense_wide_pack(store, name, F, units, for_dx=True)
+                g_hi, g_lo = ops.split_bf16(g2d, Np)
+                dx = ops.gemm_split_f32(g_hi, g_lo, wt_hi, wt_lo)[:, :F]
+                tape.add_grad(inputs, dx.contiguous().view(*lead, F))
+        tape.record(out, bwd)
+    return out
+
+
 def dense(inputs, units, name='logits', is_training=False):
-    """tf.layers.dense(inputs, units, activation=None, use_bias=True, name=name) for units <= 32."""
+    """tf.layers.dense(inputs, units, activation=None, use_bias=True, name=name): ner_dense_small_n for units <= 32,
+    the split-bf16 tensor-core GEMM above that."""
     F = inputs.shape[-1]
     lead = inputs.shape[:-1]
     name = variables.scoped(name)
     w = variables.get_variable(f"{name}/kernel", (F, units), variables.glorot_uniform)
     b = variables.get_variable(f"{name}/bias", (units,), variables.zeros)
+    if units > 32:
+        return _dense_wide(inputs, units, name, b, is_training)
     tape = autodiff.current()
     if is_training and tape is not None:
         store = variables.default_store()

@@ -157,6 +157,37 @@ int ner_crf_viterbi_nbest(const float* logits, const int32_t* seq_len, const flo
                           float* scores_out, int32_t* count_out, void* workspace, size_t workspace_bytes, int B, int L,
                           int K, ner_stream_t stream);
 
+/* Wide tag sets (csrc/crf_wide.cu): ner_crf_viterbi, ner_crf_loglik_fwd and ner_crf_loglik_bwd for
+ * 1 <= K <= NER_MAX_TAGS_WIDE, with the same arguments, row rules (seq_len <= 0 decodes one position, seq_len > L
+ * counts as L), alpha workspace, flags, d_ll / scale and d_trans accumulation.  Viterbi's tags and best_score are
+ * bit-exact with ner_crf_viterbi where both run.  Viterbi also takes a backpointer workspace of at least
+ * ner_crf_wide_viterbi_workspace_bytes(B, L, K) = B*L*K bytes (0 for B = 0).  NER_ERR_INVALID_ARG for B < 0, L < 1 or
+ * a required null pointer (B > 0); NER_ERR_UNSUPPORTED for K outside 1..NER_MAX_TAGS_WIDE; NER_ERR_WORKSPACE for a
+ * missing or short workspace; B = 0 is a no-op.  All checked before any CUDA call. */
+#define NER_MAX_TAGS_WIDE 128
+size_t ner_crf_wide_viterbi_workspace_bytes(int B, int L, int K);
+int ner_crf_wide_viterbi(const float* logits, const int32_t* seq_len, const float* trans, int32_t* tags_out,
+                         float* best_score, void* workspace, size_t workspace_bytes, int B, int L, int K,
+                         ner_stream_t stream);
+int ner_crf_wide_loglik_fwd(const float* logits, const int32_t* tags, const int32_t* seq_len, const float* trans,
+                            float* ll, float* logz_out, float* alpha_ws, int B, int L, int K, int flags,
+                            ner_stream_t stream);
+int ner_crf_wide_loglik_bwd(const float* logits, const int32_t* tags, const int32_t* seq_len, const float* trans,
+                            const float* alpha_ws, const float* logz, const float* d_ll, float scale, float* d_logits,
+                            float* d_trans, int B, int L, int K, ner_stream_t stream);
+
+/* Which kernel configuration the three wide entry points run for a call of this shape: W = 64 threads (K <= 64) or
+ * 128, one CTA per G = 1 or 4 sequences (G = 4 from B >= 8 * num_sms).  A pure function of its arguments; no CUDA
+ * call, no environment.  NER_CRF_WIDE_NONE for B < 1, L < 1, num_sms < 1 or K outside 1..NER_MAX_TAGS_WIDE. */
+enum {
+  NER_CRF_WIDE_64_G1 = 0,
+  NER_CRF_WIDE_64_G4 = 1,
+  NER_CRF_WIDE_128_G1 = 2,
+  NER_CRF_WIDE_128_G4 = 3,
+  NER_CRF_WIDE_NONE = 4
+};
+int ner_crf_wide_plan(int B, int L, int K, int num_sms);
+
 
 /* ------------------------------------------------------------------------ *
  * Dense layers on wgmma tensor cores — replaces tf.layers.dense /
@@ -935,6 +966,10 @@ int ner_bert_train_bwd_set_layer_events(void* const* events_host, int n_events);
  * a span is typed by its LAST tag).  L <= 4095. */
 int ner_extract_spans(const int32_t* pred_ids, const uint8_t* tag_class, int32_t* spans, int32_t* counts, int B, int L,
                       int K, int cap, ner_stream_t stream);
+/* ner_extract_spans for tag sets of more than 32 entity types: tag_class [K] u16 with the same bits 0-2 and the type id
+ * in bits 3-9 (up to 128 types); the span word carries it in bits 24-30. */
+int ner_extract_spans_wide(const int32_t* pred_ids, const uint16_t* tag_class, int32_t* spans, int32_t* counts, int B,
+                           int L, int K, int cap, ner_stream_t stream);
 
 /* ------------------------------------------------------------------------ *
  * SoftLexicon HOST builder — replaces data/word_enhance.py:302-337 (build_soft_lexicon), :89-119 (align_with_token),
