@@ -188,6 +188,8 @@ SIGNATURES["ner_wgrad_group_bf16"] = (_i, [_c.POINTER(WgradProblem), _i, _i, _vp
 SIGNATURES["ner_bert_train_bwd_set_layer_events"] = (_i, [_vp, _i])
 SIGNATURES["ner_extract_spans"] = (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp])
 SIGNATURES["ner_extract_spans_wide"] = (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp])
+SIGNATURES["ner_featurize_wordpiece"] = (_i, [_vp] * 3 + [_i, _i] + [_vp] * 4 + [_i, _vp, _vp] + [_i] * 6 + [_vp] * 6)
+SIGNATURES["ner_featurize_chars"] = (_i, [_vp] * 3 + [_i, _i] + [_vp] * 3 + [_i, _vp, _vp, _i, _i] + [_vp] * 6)
 SIGNATURES["ner_lexicon_create"] = (_vp, [_vp, _vp, _vp, _i])
 SIGNATURES["ner_lexicon_destroy"] = (None, [_vp])
 SIGNATURES["ner_lexicon_num_nodes"] = (_c.c_int64, [_vp])

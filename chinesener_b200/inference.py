@@ -2,6 +2,7 @@
 """In-process counterpart of reference inference.py:33-99: `InferHelper.infer(text)` featurises one sentence exactly
 like the reference's serving client and runs PREDICT on the local engine instead of a TF-Serving gRPC round trip."""
 import re
+from collections import defaultdict
 
 import numpy as np
 
@@ -27,6 +28,7 @@ class InferHelper(object):
         self.idx2tag = dict((v, k) for k, v in tag2idx.items())
         self.estimator = estimator
         self.feature = None
+        self.featurizer = None
 
     def make_feature(self, sentence):
         """reference inference.py:64-82: sequence features + fake labels ('0.0' strings / zero ids), task id for the
@@ -72,12 +74,42 @@ class InferHelper(object):
     def infer_batch(self, texts):
         """Many sentences per call: one PREDICT batch, the tag scan of extract_entity on the GPU (ner_extract_spans) —
         the tag tensor stays on the device, only the spans come back.  -> one entity dict per text, as infer() gives.
-        A span-pointer plugin (bert_mrc_span) returns its own spans instead, nested and overlapping ones included."""
-        from .tools.infer_utils import extract_entity_device, span_entities, span_lists
-        feats = [dict(self.make_feature(t)) for t in texts]
-        dev = self.estimator.to_device(features_to_batch(feats, pin_memory=True))
+        A span-pointer plugin (bert_mrc_span) returns its own spans instead, nested and overlapping ones included.
+
+        Plugins whose features are BasicProc's alone (no word-enhance method) featurise the raw texts on the device
+        (data/device_featurize.py, built on first use and kept), and the entity strings are rebuilt for the returned
+        spans only; the word-enhance plugins featurise on the host with make_feature."""
+        import torch
+        from .tools.infer_utils import extract_entity_device, span_entities, span_lists, tag_spans_device
+        if self.word_enhance is not None or not texts:
+            feats = [dict(self.make_feature(t)) for t in texts]
+            dev = self.estimator.to_device(features_to_batch(feats, pin_memory=True))
+            pred = self.estimator.predict_device(dev)
+            spans = span_lists(pred)
+            if spans is not None:
+                return span_entities([f['tokens'] for f in feats], spans)
+            return extract_entity_device([f['tokens'] for f in feats], pred, self.idx2tag)
+        if self.featurizer is None:
+            from .data.device_featurize import DeviceFeaturizer
+            self.featurizer = DeviceFeaturizer(self.proc.tokenizer, self.max_seq_len, self.estimator.device)
+        dev = self.featurizer.featurize(texts, task_id=1 if self.mtl else None)
+        host = {}
+        for k in ('token_ids', 'unk_cursor'):        # read only for the spans' strings, after the span scan's sync
+            host[k] = torch.empty(dev[k].shape, dtype=torch.int32, pin_memory=True)
+            host[k].copy_(dev[k], non_blocking=True)
+        del dev['unk_cursor']
         pred = self.estimator.predict_device(dev)
         spans = span_lists(pred)
-        if spans is not None:
-            return span_entities([f['tokens'] for f in feats], spans)
-        return extract_entity_device([f['tokens'] for f in feats], pred, self.idx2tag)
+        if spans is None:
+            spans = tag_spans_device(pred, self.idx2tag)
+        text = self.featurizer.entity_text(texts, host['token_ids'].numpy(), host['unk_cursor'].numpy(),
+                                           dev['mask'].row_lengths)
+        out = []
+        for b, row in enumerate(spans):
+            found = defaultdict(set)
+            for span in row:
+                s = text(b, span[1], span[2])
+                if s != '':
+                    found[span[0]].add(s)
+            out.append(found)
+        return out

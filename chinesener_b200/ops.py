@@ -1266,6 +1266,30 @@ def extract_spans(pred_ids, tag_class, cap=None):
     return spans, counts
 
 
+# --------------------------------------------------------------------------- raw text -> features (serving head)
+def _featurize_args(text_dev, offsets_host, B, uni, vocab, out):
+    require_cuda(text_dev, *out.values())
+    head = 8 * (B + 1)
+    return ([ptr(text_dev) + head, ptr(text_dev), offsets_host.data_ptr(), B],
+            [vocab['slots'].data_ptr(), vocab['slots'].numel(), ptr(vocab['entries']), ptr(vocab['blob'])],
+            [ptr(out[k]) for k in ('token_ids', 'mask', 'segment_ids', 'seq_len', 'unk_cursor')] + [stream()])
+
+
+def featurize_wordpiece(text_dev, offsets_host, B, L, uni, vocab, max_piece, lower, special, out):
+    """ner_featurize_wordpiece.  text_dev uint8 (device) = offsets int64 [B+1] then the UTF-8 bytes; offsets_host the
+    host buffer it was copied from; uni / vocab the device tables of data/device_featurize.py; special = ([CLS], [SEP],
+    [PAD], [UNK]) ids; out the five [B, L] / [B] int32 outputs."""
+    head, tab, tail = _featurize_args(text_dev, offsets_host, B, uni, vocab, out)
+    check(lib().ner_featurize_wordpiece(*head, L, ptr(uni['stage1']), ptr(uni['stage2']), ptr(uni['expand']), *tab,
+                                        int(max_piece), int(bool(lower)), *special, *tail))
+
+
+def featurize_chars(text_dev, offsets_host, B, L, uni, vocab, max_piece, lower, special, out):
+    """ner_featurize_chars: as featurize_wordpiece with special = ([PAD], [UNK]) ids (max_piece / lower unused)."""
+    head, tab, tail = _featurize_args(text_dev, offsets_host, B, uni, vocab, out)
+    check(lib().ner_featurize_chars(*head, L, ptr(uni['stage1']), ptr(uni['stage2']), *tab, *special, *tail))
+
+
 def wgrad_group(problems, rows):
     """problems: list of (x bf16 [rows, ld_x], dy bf16 [rows, ld_dy], dy_col0, dw f32 [k_in, n_out]) -> dw += x[:, :k_in]^T dy[:, col0:col0+n_out],
     all in one launch (ner_wgrad_group_bf16)."""

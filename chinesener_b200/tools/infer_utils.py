@@ -102,10 +102,24 @@ def span_entities(tokens_batch, spans_batch):
     return out
 
 
-def extract_entity_device(tokens_batch, pred_ids, idx2tag, _cache={}):
+def extract_entity_device(tokens_batch, pred_ids, idx2tag):
     """Batched extract_entity with the tag scan on the GPU (ner_extract_spans): pred_ids [B, L] int32 on the device,
     tokens_batch B lists of L token strings -> list of {type: set of surface strings}, equal to
     [extract_entity(tokens, pred_ids[b], idx2tag) for b ...].  Only the spans (4 bytes each) cross to the host."""
+    out = []
+    for toks, spans in zip(tokens_batch, tag_spans_device(pred_ids, idx2tag)):
+        found = defaultdict(set)
+        for t, s, e in spans:
+            text = ''.join(toks[s:e])
+            if text != '':
+                found[t].add(text)
+        out.append(found)
+    return out
+
+
+def tag_spans_device(pred_ids, idx2tag, _cache={}):
+    """The spans of extract_entity's tag scan, run on the GPU (ner_extract_spans): pred_ids [B, L] int32 on the device ->
+    per sentence a list of (entity type, start, end_exclusive) in scan order."""
     from .. import ops
     key = tuple(sorted(idx2tag.items()))
     ent = _cache.get(key)
@@ -118,13 +132,5 @@ def extract_entity_device(tokens_batch, pred_ids, idx2tag, _cache={}):
     spans, counts = ops.extract_spans(pred_ids, table)
     counts = counts.cpu().numpy()
     spans = spans[:, :max(int(counts.max()), 1)].cpu().numpy() if len(counts) else spans.cpu().numpy()
-    out = []
-    for b, toks in enumerate(tokens_batch):
-        found = defaultdict(set)
-        for w in spans[b, :counts[b]]:
-            s, e, t = int(w) & 0xFFF, (int(w) >> 12) & 0xFFF, int(w) >> 24
-            text = ''.join(toks[s:e])
-            if text != '':
-                found[types[t]].add(text)
-        out.append(found)
-    return out
+    return [[(types[int(w) >> 24], int(w) & 0xFFF, (int(w) >> 12) & 0xFFF) for w in spans[b, :counts[b]]]
+            for b in range(len(counts))]

@@ -972,6 +972,40 @@ int ner_extract_spans_wide(const int32_t* pred_ids, const uint16_t* tag_class, i
                            int L, int K, int cap, ner_stream_t stream);
 
 /* ------------------------------------------------------------------------ *
+ * Raw text -> BasicProc.build_seq_feature features (data/device_featurize.py builds the tables).
+ * text: the B texts' UTF-8 bytes (Python's encode('utf-8', 'surrogatepass')) back to back, text b =
+ * [offsets[b], offsets[b+1]); offsets [B+1] i64 on the device and the same values in host memory (offsets_host), which
+ * is checked: offsets_host[0] == 0 and non-decreasing.  Malformed UTF-8 reads as U+FFFD.
+ * Unicode tables: uni_stage2[(uni_stage1[cp >> 8] << 8) + (cp & 255)] u32 = flags (bit 0 _is_control, 1 _is_whitespace,
+ * 2 str.isspace, 3 _is_punctuation, 4 _is_chinese_char, 5 category Mn, 6 cased and not case-ignorable, 7
+ * case-ignorable) | combining class << 8 | x << 16, where x > 0 names NFD(lower(cp)) = uni_expand[4x .. 4x+3] (zero
+ * padded) and x = 0 means cp itself.
+ * Vocabulary: open addressing over the UTF-8 bytes of every key (FNV-1a 32, linear probing): slots [n_slots] i32 (a
+ * power of two, -1 = empty) -> entry e; entries [n_keys, 3] i32 = blob offset, byte length, id; blob = the keys' bytes.
+ * Outputs [B, L] i32 token_ids / mask / segment_ids / unk_cursor and seq_len [B] i32.  One launch, no host
+ * synchronisation, shared memory independent of the texts' length; a row stops scanning once it is full.
+ * NER_ERR_INVALID_ARG for B < 0, L < 1 (L < 2 for WordPiece), a null pointer, bad offsets, n_slots not a power of two, a
+ * negative special id or max_piece < 1; NER_ERR_UNSUPPORTED for B*L >= 2^31; all before any CUDA call.  B = 0 is a
+ * no-op. */
+/* FullTokenizer.tokenize (BasicTokenizer(do_lower_case) + WordPiece, 200-character [UNK] rule) + format_sequence:
+ * [CLS] + the first L-2 tokens + [SEP], then [PAD].  Token ids must be below 2^24; max_piece = the longest key in code
+ * points.  unk_cursor = fix_tokens' cursor at each [UNK] (characters of the tokens before it, '##' removed, an [UNK]
+ * counting one), -1 elsewhere. */
+int ner_featurize_wordpiece(const uint8_t* text, const int64_t* offsets, const int64_t* offsets_host, int B, int L,
+                            const uint16_t* uni_stage1, const uint32_t* uni_stage2, const uint32_t* uni_expand,
+                            const int32_t* slots, int n_slots, const int32_t* entries, const uint8_t* blob,
+                            int max_piece, int do_lower_case, int cls_id, int sep_id, int pad_id, int unk_id,
+                            int32_t* token_ids, int32_t* mask, int32_t* segment_ids, int32_t* seq_len,
+                            int32_t* unk_cursor, ner_stream_t stream);
+/* TokenizerAdapter.tokenize + format_sequence: characters for which str.strip() is empty are skipped, full2half, the
+ * character's id or unk_id, the first L tokens, then pad_id.  unk_cursor = the raw character index of each [UNK]. */
+int ner_featurize_chars(const uint8_t* text, const int64_t* offsets, const int64_t* offsets_host, int B, int L,
+                        const uint16_t* uni_stage1, const uint32_t* uni_stage2, const int32_t* slots, int n_slots,
+                        const int32_t* entries, const uint8_t* blob, int pad_id, int unk_id, int32_t* token_ids,
+                        int32_t* mask, int32_t* segment_ids, int32_t* seq_len, int32_t* unk_cursor,
+                        ner_stream_t stream);
+
+/* ------------------------------------------------------------------------ *
  * SoftLexicon HOST builder — replaces data/word_enhance.py:302-337 (build_soft_lexicon), :89-119 (align_with_token),
  * :163-205 (postproc_soft_lexicon) and data/base_preprocess.py:397-412 (format_soft_seq) for whole datasets at a time.
  * Host code (no CUDA call, no stream): all pointers are HOST pointers.  Output layout = the input of
