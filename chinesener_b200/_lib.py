@@ -70,6 +70,10 @@ SIGNATURES = {
     "ner_mlm_mask": (_i, [_vp] * 4 + [_i, _i, _c.c_uint64, _i, _i] + [_vp] * 4),
     "ner_vocab_xent_scratch_floats": (_c.c_size_t, [_i]),
     "ner_vocab_xent": (_i, [_vp, _i, _vp, _i, _i, _c.c_float] + [_vp] * 7),
+    "ner_augment_rows_smem_bytes": (_c.c_size_t, [_i]),
+    "ner_augment_rows": (_i, [_vp] * 5 + [_i, _i, _vp, _i, _vp, _i] + [_vp] * 3 + [_i, _i, _vp, _vp, _i]
+                         + [_c.c_float] * 5 + [_c.c_uint64, _i, _i, _i] + [_vp] * 7 + [_vp]),
+    "ner_vocab_sample": (_i, [_vp, _i, _i, _vp, _vp, _i, _c.c_longlong, _c.c_float, _c.c_uint64, _vp, _vp]),
     "ner_mrc_pairs": (_i, [_vp] * 6 + [_i] * 6 + [_vp] * 7),
     "ner_mrc_merge": (_i, [_vp] * 3 + [_i] * 6 + [_vp, _vp]),
     "ner_mrc_span_targets": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),

@@ -56,6 +56,9 @@ class Estimator:
         self.tag_set_limits()
         if teacher is not None:
             self.distill_settings()
+        if self.params.get('augment'):
+            from . import augment
+            augment.check_estimator(self)
         self.store = store or variables.VariableStore(self.device)
         # data-parallel gradient exchange (N > 1): 'overlap' = bucketed all-reduces behind the backward pass, 'overlap_bf16' =
         # the same with bf16 buckets, 'single' = one all-reduce of the flat buffer after the backward pass

@@ -78,7 +78,12 @@ def train_and_evaluate(estimator, input_pipe, model_dir, run_config=RUN_CONFIG, 
         # stop_if_no_decrease_hook: the best (lowest) eval loss is at least max_steps_without_decrease steps old
         return store.global_step - best[1] >= max_no_decrease
 
-    for feats in input_pipe.build_input_fn('train')():
+    batches = input_pipe.build_input_fn('train')()
+    if p.get('augment'):
+        from . import augment
+        aug = augment.build(p, p['idx2tag'], input_pipe.file_path('train'), estimator.device, estimator.model_name)
+        batches = aug.pipeline(batches, store.global_step, estimator.to_device)
+    for feats in batches:
         loss = estimator.train_step(feats)
         loss_sum = loss.detach() if loss_sum is None else loss_sum + loss.detach()
         loss_n += 1
@@ -159,6 +164,7 @@ def singletask_train(args):
     _window_params(TRAIN_PARAMS, args)
     if args.crf_nbest != 1:
         TRAIN_PARAMS['crf_nbest'] = args.crf_nbest
+    _augment_params(TRAIN_PARAMS, args)
     teacher_ck = None
     if not args.teacher_model and (args.teacher_dir or args.teacher_pretrain_dir):
         raise ValueError('--teacher_dir / --teacher_pretrain_dir need --teacher_model')
@@ -256,6 +262,8 @@ def multitask_train(args):
     if args.crf_nbest != 1:
         raise ValueError('--crf_nbest is for single-task plugins: the multi-task pred_ids are a per-task selection of '
                          'several CRF decodes')
+    if args.augment:
+        raise ValueError('--augment is for single-task plugins: a multi-task batch mixes tag sets')
     model_dir = os.path.join(args.checkpoint_root, 'ner_{}_{}'.format(joined, model_name))
     data_root = args.data_dir or './data'
     if args.clear_model:
@@ -343,7 +351,30 @@ def build_parser():
                         '(default --pretrain_dir)')
     parser.add_argument('--distill_alpha', type=float, default=0.5, help='weight of the distillation term, in (0, 1]')
     parser.add_argument('--distill_temperature', type=float, default=1.0, help='temperature of the distillation term, > 0')
+    parser.add_argument('--augment', type=str, default='', help='augment every TRAIN batch on the GPU: op=p[,op=p ...] '
+                        'with op in mr (mention replacement), lwtr (label-wise token replacement), sis (shuffle within '
+                        'segments), mlm (masked-LM replacement), e.g. mr=0.3,lwtr=0.3,sis=0.3,mlm=0.15')
+    parser.add_argument('--augment_rows', type=float, default=None, help='share of rows augmented at all (default 0.5)')
+    parser.add_argument('--augment_mlm_dir', type=str, default='', help='BERT with its masked-LM head for mlm (default '
+                        '--pretrain_dir)')
+    parser.add_argument('--augment_mlm_temperature', type=float, default=None, help='sampling temperature of mlm '
+                        '(default 1)')
     return parser
+
+
+def _augment_params(params, args):
+    """--augment* over the params (read by augment.settings); nothing is set without --augment."""
+    if not args.augment:
+        return
+    from .augment import parse_augment
+    params['augment'] = parse_augment(args.augment)
+    params['augment_seed'] = args.seed
+    if args.augment_rows is not None:
+        params['augment_rows'] = args.augment_rows
+    if args.augment_mlm_dir:
+        params['augment_mlm_dir'] = args.augment_mlm_dir
+    if args.augment_mlm_temperature is not None:
+        params['augment_mlm_temperature'] = args.augment_mlm_temperature
 
 
 def _window_params(params, args):

@@ -109,6 +109,21 @@ def _decoder(store, cfg):
     return ent
 
 
+def head_logits(h16, positions, M, cfg, store):
+    """The head's forward on the encoder output h16 [rows, H] bf16 at the flat row indices positions [M] i32: gather,
+    transform (dense, GELU, LayerNorm) and the tied decoder.  -> (logits [M, V_pad] f32, (h, pre, act, t16, decoder
+    operands), what the backward reads)."""
+    v = store.vars
+    dec = _decoder(store, cfg)
+    h = ops.gather_rows(h16, positions, M)
+    pre = ops.gemm_bf16(h, dec["w_nk"], v[f"{SCOPE}/transform/dense/bias"], epilogue=ops.EPI_BF16)
+    act = ops.gelu_bf16(pre, GELU == "erf")
+    _, t16 = ops.layernorm(act, v[f"{SCOPE}/transform/LayerNorm/gamma"], v[f"{SCOPE}/transform/LayerNorm/beta"],
+                           eps=1e-12, want_f32=False)
+    logits = ops.gemm_bf16(t16, dec["E"], dec["bias"], epilogue=ops.EPI_F32)          # [M, V_pad]
+    return logits, (h, pre, act, t16, dec)
+
+
 class MaskedLMOutput:
     """loss [] f32, count / correct [] i32 (device scalars), pred [M] i32, and the masking: masked_ids [B,L],
     positions / labels [M]."""
@@ -150,14 +165,9 @@ def masked_lm(features, cfg, store, seed, masked_lm_prob, max_predictions_per_se
         zi = torch.zeros((), dtype=torch.int32, device=dev)
         return MaskedLMOutput(z, zi, zi.clone(), positions, masked, positions, labels)
     v = store.vars
-    dec = _decoder(store, cfg)
     erf = GELU == "erf"
-    h = ops.gather_rows(h16, positions, M)
-    pre = ops.gemm_bf16(h, dec["w_nk"], v[f"{SCOPE}/transform/dense/bias"], epilogue=ops.EPI_BF16)
-    act = ops.gelu_bf16(pre, erf)
+    logits, (h, pre, act, t16, dec) = head_logits(h16, positions, M, cfg, store)
     gamma = v[f"{SCOPE}/transform/LayerNorm/gamma"]
-    _, t16 = ops.layernorm(act, gamma, v[f"{SCOPE}/transform/LayerNorm/beta"], eps=1e-12, want_f32=False)
-    logits = ops.gemm_bf16(t16, dec["E"], dec["bias"], epilogue=ops.EPI_F32)          # [M, V_pad]
     loss, count, correct, pred, d_logits = ops.vocab_xent(logits, labels, V, want_grad=is_training)
     res = MaskedLMOutput(loss, count, correct, pred, masked, positions, labels)
     if not is_training:

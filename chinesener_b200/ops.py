@@ -776,6 +776,51 @@ def vocab_xent(logits, labels, V, want_pred=True, want_grad=False, d_loss=1.0):
     return loss, count, correct, pred, dz
 
 
+# --------------------------------------------------------------------------- training-data augmentation (augment.py)
+AUGMENT_MLM_BUDGET = 20        # NER_AUGMENT_MLM_BUDGET
+
+
+def augment_rows(token_ids, label_ids, seq_len, mask, segment_ids, tables, probs, seed, pad_id, pad_tag, mask_id=-1,
+                 want_mlm=False):
+    """MR, LwTR, SiS and the masked-LM [MASK]ing of a BIO batch (ner_augment_rows; rules in ner_b200.h).  tables: dict of
+    int32 device tensors tag_class [K], type_tag [T,2], mention_type_off [T+1], mention_tok_off [n_mentions+1],
+    mention_tokens, tag_tok_off [K+1], tag_tokens (each at least one element).  probs: (row, mr, lwtr, sis, mlm).
+    -> dict token_ids, label_ids, mask, segment_ids [B,L], seq_len [B] (i32) and, with want_mlm, mlm_ids [B,L] and
+    mlm_positions [B, AUGMENT_MLM_BUDGET]."""
+    require_cuda(token_ids, label_ids, seq_len, mask, segment_ids)
+    B, L = token_ids.shape
+    ids, lab, sl, msk, seg = (_i32(x) for x in (token_ids, label_ids, seq_len, mask, segment_ids))
+    tb = tables
+    dev = ids.device
+    out = {k: torch.empty((B, L), dtype=torch.int32, device=dev) for k in ('token_ids', 'label_ids', 'mask', 'segment_ids')}
+    out['seq_len'] = torch.empty((B,), dtype=torch.int32, device=dev)
+    if want_mlm:
+        out['mlm_ids'] = torch.empty((B, L), dtype=torch.int32, device=dev)
+        out['mlm_positions'] = torch.empty((B, AUGMENT_MLM_BUDGET), dtype=torch.int32, device=dev)
+    check(lib().ner_augment_rows(
+        ptr(ids), ptr(lab), ptr(sl), ptr(msk), ptr(seg), B, L, ptr(tb['tag_class']), tb['tag_class'].numel(),
+        ptr(tb['type_tag']), tb['n_types'], ptr(tb['mention_type_off']), ptr(tb['mention_tok_off']),
+        ptr(tb['mention_tokens']), tb['n_mentions'], tb['n_mention_tokens'], ptr(tb['tag_tok_off']),
+        ptr(tb['tag_tokens']), tb['n_tag_tokens'], *(float(p) for p in probs), int(seed) & 0xFFFFFFFFFFFFFFFF,
+        int(pad_id), int(pad_tag), int(mask_id), ptr(out['token_ids']), ptr(out['label_ids']), ptr(out['seq_len']),
+        ptr(out['mask']), ptr(out['segment_ids']), ptr(out.get('mlm_ids')), ptr(out.get('mlm_positions')), stream()))
+    return out
+
+
+def vocab_sample(logits, V, eligible, positions, token_ids, temperature, seed):
+    """Gumbel-max draw from softmax(logits[:, :V] / temperature) over the eligible ids other than the current one, written
+    into token_ids (in place) at positions (ner_vocab_sample; slots at -1 are skipped).  logits [M, ld] f32, eligible [V]
+    u8, positions [M] i32."""
+    require_cuda(logits, eligible, positions, token_ids)
+    assert logits.dtype == torch.float32 and logits.dim() == 2 and eligible.dtype == torch.uint8
+    assert positions.dtype == torch.int32 and token_ids.dtype == torch.int32
+    M, ld = logits.shape
+    assert positions.numel() == M
+    check(lib().ner_vocab_sample(ptr(logits), ld, V, ptr(eligible), ptr(positions), M, token_ids.numel(),
+                                 float(temperature), int(seed) & 0xFFFFFFFFFFFFFFFF, ptr(token_ids), stream()))
+    return token_ids
+
+
 # --------------------------------------------------------------------------- MRC pairs and tag merge (bert_mrc)
 def mrc_pairs(token_ids, seq_len, query_ids, query_len, type_tag, L2, sep_id, label_ids=None):
     """[B, L] BERT batch -> its B*T query/context pairs (ner_mrc_pairs): dict of ids / segment_ids / mask [B*T, L2] i32,

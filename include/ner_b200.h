@@ -718,6 +718,56 @@ int ner_mlm_mask(const int32_t* token_ids, const int32_t* seq_len, const uint8_t
 size_t ner_vocab_xent_scratch_floats(int M);
 int ner_vocab_xent(const float* logits, int ld, const int32_t* labels, int M, int V, float d_loss, float* loss,
                    int32_t* count, int32_t* correct, int32_t* pred, void* d_logits, float* scratch, ner_stream_t stream);
+/* ---- training-data augmentation (chinesener_b200/augment.py; Dai & Adel, COLING 2020, and masked-LM replacement after
+ * Kobayashi, NAACL 2018) ---- */
+#define NER_AUGMENT_MAX_LEN 4095      /* L of ner_augment_rows */
+#define NER_AUGMENT_MLM_BUDGET 20     /* masked-LM replacements per row */
+/* Augments a BIO batch token_ids / label_ids / mask / segment_ids [B,L] i32, seq_len [B] i32 into the *_out arrays (not
+ * in place).  h_k(b, t) = hash3(lo(seed) + k * 0x9E3779B9, hi(seed) ^ b, t); "drawn with p" means
+ * (h >> 8) < (uint32)(p * 2^24); "pick from n" means umulhi(h, n).  Streams k: 0 row, 1 / 2 MR choice / draw, 3 / 4
+ * LwTR choice / draw, 5 / 6 SiS choice / key, 7 MLM choice, 8 ner_vocab_sample's Gumbel draws.
+ * tag_class [K] gives each tag id its class: 0 special (never touched), 1 O, 2 + 2x B of type x, 3 + 2x I of type x;
+ * a label outside [0, K) is special.  type_tag [T, 2] = (B id, I id or -1) of type x.  Pools (CSR, offsets relative to
+ * their arrays, a malformed range is an empty pool): mention_type_off [T+1] into the mention list, mention_tok_off
+ * [n_mentions+1] into mention_tokens [n_mention_tokens]; tag_tok_off [K+1] into tag_tokens [n_tag_tokens].
+ * Row b is augmented when h_0(b, 0) is drawn with p_row; any other row is copied unchanged (seq_len included).  For an
+ * augmented row with n = clamp(seq_len[b], 0, L), in this order:
+ *   MR   A mention is a B-x token and the run of I-x tokens after it (span::run_end).  Mentions left to right; with s the
+ *        mention's start in the input row, the mention is chosen when h_1(b, s) is drawn with p_mr, and replaced by
+ *        mention pick(h_2(b, s), count of type x) of type x's pool (tags B-x, I-x ...) when the row's running length
+ *        minus the old plus the new mention's length stays <= L; otherwise it stays.  Other tokens are copied.
+ *   LwTR Every non-special position t of the new row with h_3(b, t) drawn with p_lwtr takes the token
+ *        pick(h_4(b, t), count) of its tag's pool (unchanged when that pool is empty).
+ *   SiS  Segments of the new row: a mention, a maximal run of O, or any other single token (a stray I-x, a special tag).
+ *        A segment starting at s with length >= 2 is chosen when h_5(b, s) is drawn with p_sis; its tokens are reordered
+ *        by ascending (h_6(b, t), t) of their positions t.  Tags stay in place.
+ *   MLM  (mlm_ids non-NULL) The first NER_AUGMENT_MLM_BUDGET O positions t, ascending, with h_7(b, t) drawn with p_mlm:
+ *        mlm_ids holds mask_id there and the row elsewhere; mlm_positions [B, NER_AUGMENT_MLM_BUDGET] holds b*L + t of
+ *        them in order, then -1 (all -1 in a row that is not augmented).
+ * Outputs of an augmented row with new length n': token / label ids of the row, then pad_id / pad_tag; mask 1 below n'
+ * and 0 from it; segment ids 0; seq_len_out = n'.  B < 0, L < 1, K < 1, T < 0, a probability outside [0, 1], a negative
+ * pool size, p_mlm > 0 without mlm_ids, only one of mlm_ids / mlm_positions, mask_id < 0 with them, or a null pointer an
+ * enabled operation reads is NER_ERR_INVALID_ARG; L > NER_AUGMENT_MAX_LEN, K > NER_MAX_TAGS_WIDE or B*L >= 2^31 is
+ * NER_ERR_UNSUPPORTED; all before any CUDA call.  B = 0 is a no-op.  One launch with
+ * ner_augment_rows_smem_bytes(L) bytes of dynamic shared memory, no allocation, bit-identical repeats. */
+size_t ner_augment_rows_smem_bytes(int L);
+int ner_augment_rows(const int32_t* token_ids, const int32_t* label_ids, const int32_t* seq_len, const int32_t* mask,
+                     const int32_t* segment_ids, int B, int L, const int32_t* tag_class, int K, const int32_t* type_tag,
+                     int T, const int32_t* mention_type_off, const int32_t* mention_tok_off, const int32_t* mention_tokens,
+                     int n_mentions, int n_mention_tokens, const int32_t* tag_tok_off, const int32_t* tag_tokens,
+                     int n_tag_tokens, float p_row, float p_mr, float p_lwtr, float p_sis, float p_mlm, uint64_t seed,
+                     int pad_id, int pad_tag, int mask_id, int32_t* token_out, int32_t* label_out, int32_t* seq_len_out,
+                     int32_t* mask_out, int32_t* segment_out, int32_t* mlm_ids, int32_t* mlm_positions,
+                     ner_stream_t stream);
+/* Gumbel-max sample of one id per slot r < M from softmax(logits[r, :V] / temperature) restricted to the ids j with
+ * eligible[j] != 0 and j != token_ids[positions[r]]: argmax_j logits[r, j] / temperature - log(-log(u_j)), u_j =
+ * ((h_8(positions[r], j) >> 9) + 0.5) / 2^23 in fp32 (ties to the lower id).  The id is written to
+ * token_ids[positions[r]]; a slot with positions[r] outside [0, n_tokens) is skipped, and a row without an eligible id
+ * leaves its token.  logits [M, ld] f32, 16-byte aligned, ld % 4 == 0.  M < 0, V < 1, ld < V, ld % 4 != 0,
+ * n_tokens < 0, a temperature that is not a positive finite number, a misaligned logits or a null pointer is
+ * NER_ERR_INVALID_ARG; V > NER_MLM_MAX_VOCAB is NER_ERR_UNSUPPORTED; all before any CUDA call.  M = 0 is a no-op. */
+int ner_vocab_sample(const float* logits, int ld, int V, const uint8_t* eligible, const int32_t* positions, int M,
+                     long long n_tokens, float temperature, uint64_t seed, int32_t* token_ids, ner_stream_t stream);
 /* model/bert_mrc.py (MRC-style NER, one BERT query per entity type; a restatement, not pinned to the reference's mrc/):
  * expands the [B,L] BERT batch (token_ids, seq_len [B] counting [CLS] and [SEP]) into the B*T pairs p = b*T + t,
  *   pair row p = token_ids[b,0] ([CLS]), query_ids[t, 0:q_t], sep_id, token_ids[b, 1:len_b]
